@@ -705,18 +705,21 @@ extern "C" int mpmb_debug_check(MpmbHandle h, int *out8);
 
 // ------------------------------------------------------------------------------ P2G
 // Replaces MPM<3>::rasterize_optimized / block_op_normal (src/transfer.cpp:467-569).
-// One 64-thread CTA per active tile (persistent round-robin).  A tile's rows are its run (unit
+// One 128-thread CTA per active tile (persistent round-robin).  A tile's rows are its run (unit
 // stride, holes where a particle left) followed by its arrivals.  Per chunk of <=CH rows:
 //   1. stage: 16-byte async copies (LDGSTS) of the P2G set (64 B/particle) into padded shared rows,
 //      all in flight at once;
-//   2. sort:  stable counting sort of the rows by cell (warp match + per-(pass,warp) histograms),
+//   2. sort:  stable counting sort of the rows by cell (warp match + per-32-row-group histograms),
 //             bit-reproducible; publishes each particle's row in the next storage (outpos);
-//   3. accumulate: thread c owns cell c and streams that cell's particles, accumulating all
-//      27 nodes x (p_x,p_y,p_z,m) in 108 REGISTERS — every particle of a cell shares one stencil;
-//   4. flush: each warp adds its registers into the shared 6x6x6 arena, conflict-free by layout
-//      (node strides 68/8/1 put the 32 cells of a warp on 32 banks), warp after warp;
+//   3. accumulate: two threads own cell c (tid = c and c + 64) and both stream that cell's particles;
+//      each accumulates HALF of the 27-node stencil x (p_x,p_y,p_z,m) in registers — every particle of
+//      a cell shares one stencil.  Flush steps n = i*9 + j*3 + k in [0, 14) belong to warps 0-1,
+//      [14, 27) to warps 2-3; both halves compute every particle's weights and Q;
+//   4. flush: each warp adds its registers into a shared 6x6x6 arena, conflict-free by layout
+//      (node strides 68/8/1 put the 32 cells of a warp on 32 banks), step after step;
 // then one coalesced store of the arena.  No atomics on floats anywhere.
-constexpr int P2G_T = 64;          // threads = cells per tile
+constexpr int P2G_T = 128;         // threads = 2 per cell of the tile
+constexpr int P2G_SPLIT = 14;      // flush steps of the first stencil half
 // particles staged per chunk: a full interior tile is 512 rows at 8 particles per cell, and in a developed flow a quarter
 // of the tiles sit a little above that — 576 keeps most of them in ONE chunk; the per-row passes below skip the empty
 // tail of a short chunk
@@ -724,15 +727,91 @@ constexpr int P2G_T = 64;          // threads = cells per tile
 #define MPMB_P2G_CH 576
 #endif
 constexpr int P2G_CH = MPMB_P2G_CH;
-constexpr int P2G_K = P2G_CH / P2G_T;
+static_assert(P2G_CH % 32 == 0 && P2G_CH <= 65536, "P2G chunk: whole warps of rows, row ids in 16 bits");
+constexpr int P2G_K = (P2G_CH + P2G_T - 1) / P2G_T;  // staging passes (r = k*T + tid); the last one may be partial
+constexpr int P2G_G = P2G_CH / 32;                   // 32-row groups = (pass, warp) histogram buckets, row order
 constexpr int P2G_ROWS = P2G_CH + P2G_CH / 8;  // padded row index r + (r>>3): cell-run reads hit distinct banks
 constexpr int P2G_DYN_BYTES = 4 * P2G_ROWS * (int)sizeof(float4);
 constexpr int AR_SX = 68, AR_SY = 8;           // arena strides in shared memory
 constexpr int AR_SIZE = 6 * AR_SX;
 
-// The time of this kernel is in-warp latency of the per-particle dependency chain; the resident CTAs per SM follow from
-// its registers and its 51.7 KB of shared memory, and the persistent grid is sized from the occupancy query in mpmb_create.
-__global__ void __launch_bounds__(P2G_T) k_p2g(View V, Params P, int part) {
+// Step 3 for one stencil half H: the cell's particles s_order[i0, i1) into acc[n - lo] for the flush steps n in [lo, hi).
+// The half is a template parameter, so the unrolled node chain keeps only its own nodes, straight-line.  Each node gets
+// the same operations as in a whole-stencil loop, so the sums do not depend on the split.
+template <int H>
+__device__ __forceinline__ void p2g_accumulate(F4 (&acc)[P2G_SPLIT], const float4 (*s_rows)[P2G_ROWS], const unsigned short *s_order,
+                                               int i0, int i1, const Params &P, float fbx, float fby, float fbz) {
+  constexpr int lo = H ? P2G_SPLIT : 0, hi = H ? 27 : P2G_SPLIT;
+  for (int it = i0; it < i1; it++) {
+    const int r = s_order[it];
+    const int ri = r + (r >> 3);
+    const float4 a0 = s_rows[0][ri], a1 = s_rows[1][ri], a2 = s_rows[2][ri], a3 = s_rows[3][ri];
+    const float mass = fabsf(a0.w);
+    float vx = a1.x, vy = a1.y, vz = a1.z;
+    if (P.particle_gravity) {  // src/transfer.cpp:485-487
+      vx += P.gdt[0]; vy += P.gdt[1]; vz += P.gdt[2];
+    }
+    // rel = pos/dx - base node of this cell (src/transfer.cpp:490,518)
+    const float rx = __fsub_rn(__fmul_rn(a0.x, P.inv_dx), fbx), ry = __fsub_rn(__fmul_rn(a0.y, P.inv_dx), fby),
+                rz = __fsub_rn(__fmul_rn(a0.z, P.inv_dx), fbz);
+    float wx[3], wy[3], wz[3];
+    bspline_weights(rx, wx);
+    bspline_weights(ry, wy);
+    bspline_weights(rz, wz);
+    // A columns: c0 = (a1.w,a2.x,a2.y) c1 = (a2.z,a2.w,a3.x) c2 = (a3.y,a3.z,a3.w)
+    // q = m v + A rel ;  node (i,j,k): q - i c0 - j c1 - k c2   (dpos = rel - node, 528-536)
+    const float q0 = fmaf(a3.y, rz, fmaf(a2.z, ry, fmaf(a1.w, rx, mass * vx)));
+    const float q1 = fmaf(a3.z, rz, fmaf(a2.w, ry, fmaf(a2.x, rx, mass * vy)));
+    const float q2 = fmaf(a3.w, rz, fmaf(a3.x, ry, fmaf(a2.y, rx, mass * vz)));
+    // (momentum | mass) as register pairs; the mass lane rides along with zero column entries
+    const F4 Q = {make_float2(q0, q1), make_float2(q2, mass)};
+    const F4 c0 = {make_float2(a1.w, a2.x), make_float2(a2.y, 0.f)}, c1 = {make_float2(a2.z, a2.w), make_float2(a3.x, 0.f)},
+             c2 = {make_float2(a3.y, a3.z), make_float2(a3.w, 0.f)};
+    const float2 m2 = bc2(-2.0f);
+    const float2 wx2[3] = {bc2(wx[0]), bc2(wx[1]), bc2(wx[2])}, wy2[3] = {bc2(wy[0]), bc2(wy[1]), bc2(wy[2])},
+                 wz2[3] = {bc2(wz[0]), bc2(wz[1]), bc2(wz[2])};
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+      if (i * 9 + 8 < lo || i * 9 >= hi) continue;
+      const F4 U = i == 0 ? Q : (i == 1 ? f4_sub(Q, c0) : f4_fma(m2, c0, Q));    // q - i c0
+#pragma unroll
+      for (int j = 0; j < 3; j++) {
+        if (i * 9 + j * 3 + 2 < lo || i * 9 + j * 3 >= hi) continue;
+        const F4 T = j == 0 ? U : (j == 1 ? f4_sub(U, c1) : f4_fma(m2, c1, U));  // ... - j c1
+        const float2 wij = mul2(wx2[i], wy2[j]);
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+          const int n = i * 9 + j * 3 + k;
+          if (n < lo || n >= hi) continue;
+          const float2 w = mul2(wij, wz2[k]);
+          const F4 N = k == 0 ? T : (k == 1 ? f4_sub(T, c2) : f4_fma(m2, c2, T));  // ... - k c2
+          acc[n - lo] = f4_fma(w, N, acc[n - lo]);
+        }
+      }
+    }
+  }
+}
+
+// Step 4 for one stencil half H: add acc into the arena `ar` at the cell's base node nb, flush step after flush step.
+template <int H>
+__device__ __forceinline__ void p2g_flush(const F4 (&acc)[P2G_SPLIT], float (*ar)[AR_SIZE], int nb) {
+  constexpr int lo = H ? P2G_SPLIT : 0, hi = H ? 27 : P2G_SPLIT;
+#pragma unroll
+  for (int n = lo; n < hi; n++) {
+    const int node = nb + (n / 9) * AR_SX + ((n / 3) % 3) * AR_SY + n % 3;
+    const F4 &a = acc[n - lo];
+    ar[0][node] += a.lo.x;
+    ar[1][node] += a.lo.y;
+    ar[2][node] += a.hi.x;
+    ar[3][node] += a.hi.y;
+    __syncwarp();
+  }
+}
+
+// The time of this kernel is in-warp latency of the per-particle dependency chain.  Two threads per cell halve the
+// accumulators (56 registers instead of 108), so 4 CTAs per SM — the limit of its 51.7 KB of shared memory — are 16 warps
+// instead of 8.  The persistent grid is sized from the occupancy query in mpmb_create.
+__global__ void __launch_bounds__(P2G_T, 4) k_p2g(View V, Params P, int part) {
   // the row staging area is dynamic shared memory (static + dynamic = 51.7 KB, above the 48 KB static limit)
 #ifndef MPMB_SIMT_HOST
   extern __shared__ __align__(16) unsigned char p2g_dyn[];
@@ -741,12 +820,13 @@ __global__ void __launch_bounds__(P2G_T) k_p2g(View V, Params P, int part) {
 #endif
   float4 (*s_rows)[P2G_ROWS] = reinterpret_cast<float4 (*)[P2G_ROWS]>(p2g_dyn);
   __shared__ unsigned short s_order[P2G_CH];
-  __shared__ unsigned short s_hist[P2G_K * 2][64];
+  __shared__ unsigned short s_hist[P2G_G][64];
   __shared__ int s_start[65];
   __shared__ float s_arena[4][AR_SIZE];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int own = tid & 63, half = tid >> 6;  // my cell, and which half of its stencil I accumulate (warp-uniform)
+  const int cx = own >> 4, cy = (own >> 2) & 3, cz = own & 3;
   const int n_tiles = V.cnt->n_tiles;
-  const int cx = tid >> 4, cy = (tid >> 2) & 3, cz = tid & 3;
   for (int slot = blockIdx.x; slot < n_tiles; slot += gridDim.x) {
     const TileMeta tm = V.meta[slot];
     const int tile = tm.tile;
@@ -756,9 +836,9 @@ __global__ void __launch_bounds__(P2G_T) k_p2g(View V, Params P, int part) {
                              tm.out_begin + nrow_tile <= V.cap_particles, 3, slot, tm.run_begin, tm.run_len)) continue;
     MPMB_TILE_XYZ(P, tm, tx, ty, tz);
     const float fbx = (float)(tx * 4 + cx), fby = (float)(ty * 4 + cy), fbz = (float)(tz * 4 + cz);
-    F4 acc[27];  // (p_x, p_y | p_z, m) of the 27 nodes of my cell's stencil
+    F4 acc[P2G_SPLIT];  // (p_x, p_y | p_z, m) of my half of my cell's stencil
 #pragma unroll
-    for (int n = 0; n < 27; n++) acc[n] = f4_zero();
+    for (int n = 0; n < P2G_SPLIT; n++) acc[n] = f4_zero();
     for (int n = tid; n < AR_SIZE; n += P2G_T) { s_arena[0][n] = 0.f; s_arena[1][n] = 0.f; s_arena[2][n] = 0.f; s_arena[3][n] = 0.f; }
     int vbase = 0;  // valid rows in the chunks already processed
     // storage row of tile-row g: run rows first, then arrivals
@@ -768,8 +848,7 @@ __global__ void __launch_bounds__(P2G_T) k_p2g(View V, Params P, int part) {
 
     for (int cb = 0; cb < nrow_tile; cb += P2G_CH) {
       const int nrows = min(P2G_CH, nrow_tile - cb);
-#pragma unroll
-      for (int e = 0; e < P2G_K * 2; e++) s_hist[e][tid] = 0;
+      for (int n = tid; n < P2G_G * 64; n += P2G_T) (&s_hist[0][0])[n] = 0;
       // ---- 1: stage rows: all copies of the chunk in flight at once
       uint32_t pidx[P2G_K];
       if (cb + nrows <= tm.run_len) {  // whole chunk inside the run (the common case): pure arithmetic, no loads
@@ -797,7 +876,7 @@ __global__ void __launch_bounds__(P2G_T) k_p2g(View V, Params P, int part) {
       cp_async_commit();
       cp_async_wait_all();
       __syncthreads();
-      // ---- 2a: per-(pass,warp) cell histograms (each thread reads back its own rows)
+      // ---- 2a: per-32-row-group cell histograms (each thread reads back its own rows; group r>>5 = (pass, warp))
       uint32_t cr[P2G_K];
 #pragma unroll
       for (int k = 0; k < P2G_K; k++) {
@@ -821,32 +900,33 @@ __global__ void __launch_bounds__(P2G_T) k_p2g(View V, Params P, int part) {
         }
         const unsigned m = __match_any_sync(0xffffffffu, cell);
         const int rank = __popc(m & ((1u << lane) - 1u));
-        if (cell < 64) {
-          if (rank == 0) s_hist[k * 2 + warp][cell] = (unsigned short)__popc(m);
+        if (cell < 64) {  // implies r < nrows <= CH: the group exists
+          if (rank == 0) s_hist[r >> 5][cell] = (unsigned short)__popc(m);
         }
         cr[k] = ((uint32_t)cell << 16) | (uint32_t)rank;
       }
       __syncthreads();
-      // ---- 2b: exclusive scan over (pass,warp) per cell, then over cells
+      // ---- 2b: exclusive scan over the row groups per cell (threads 0..63, one per cell), then over cells
       {
-        const int c = tid;
-        int run = 0;
+        int run = 0, incl = 0;
+        if (tid < 64) {
 #pragma unroll
-        for (int e = 0; e < P2G_K * 2; e++) {
-          const int h = s_hist[e][c];
-          s_hist[e][c] = (unsigned short)run;
-          run += h;
-        }
-        int incl = run;
+          for (int e = 0; e < P2G_G; e++) {
+            const int h = s_hist[e][tid];
+            s_hist[e][tid] = (unsigned short)run;
+            run += h;
+          }
+          incl = run;
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const int y = __shfl_up_sync(0xffffffffu, incl, o);
-          if (lane >= o) incl += y;
+          for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+          }
+          if (tid == 31) s_start[64] = incl;  // total of warp 0, fixed up below
         }
-        if (tid == 31) s_start[64] = incl;  // total of warp 0, fixed up below
         __syncthreads();
         const int base0 = warp ? s_start[64] : 0;
-        s_start[c] = base0 + incl - run;
+        if (tid < 64) s_start[tid] = base0 + incl - run;
         __syncthreads();
         if (tid == 63) s_start[64] = base0 + incl;
       }
@@ -856,7 +936,7 @@ __global__ void __launch_bounds__(P2G_T) k_p2g(View V, Params P, int part) {
         const int r = k * P2G_T + tid;
         const int cell = (int)(cr[k] >> 16);
         if (cell < 64) {
-          const int pos = s_start[cell] + s_hist[k * 2 + warp][cell] + (int)(cr[k] & 0xffffu);
+          const int pos = s_start[cell] + s_hist[r >> 5][cell] + (int)(cr[k] & 0xffffu);
           s_order[pos] = (unsigned short)r;
           V.outpos[pidx[k]] = (uint32_t)(tm.out_begin + vbase + pos);
         }
@@ -864,84 +944,36 @@ __global__ void __launch_bounds__(P2G_T) k_p2g(View V, Params P, int part) {
         // its new one, and two CTAs must not write different values to one outpos entry
       }
       __syncthreads();
-      // ---- 3: accumulate my cell's run in registers.  A warp iterates as long as its fullest cell has particles; in a
-      // developed flow (cells hold 0..30 particles) that is the kernel's cost.  Tried and dropped: capping the loop and
-      // adding the excess particles with one lane per stencil node (the serialised excess pass costs more than the idle
-      // tail), re-assigning cells to threads per tile so that warp 0 owns the fuller cells, and software-pipelining the
-      // row fetch: the kernel is latency-bound, an early warp's issue slots are not what it lacks.
-      const int i0 = s_start[tid], i1 = s_start[tid + 1];
-      for (int it = i0; it < i1; it++) {
-        const int r = s_order[it];
-        const int ri = r + (r >> 3);
-        const float4 a0 = s_rows[0][ri], a1 = s_rows[1][ri], a2 = s_rows[2][ri], a3 = s_rows[3][ri];
-        const float mass = fabsf(a0.w);
-        float vx = a1.x, vy = a1.y, vz = a1.z;
-        if (P.particle_gravity) {  // src/transfer.cpp:485-487
-          vx += P.gdt[0]; vy += P.gdt[1]; vz += P.gdt[2];
-        }
-        // rel = pos/dx - base node of this cell (src/transfer.cpp:490,518)
-        const float rx = __fsub_rn(__fmul_rn(a0.x, P.inv_dx), fbx), ry = __fsub_rn(__fmul_rn(a0.y, P.inv_dx), fby),
-                    rz = __fsub_rn(__fmul_rn(a0.z, P.inv_dx), fbz);
-        float wx[3], wy[3], wz[3];
-        bspline_weights(rx, wx);
-        bspline_weights(ry, wy);
-        bspline_weights(rz, wz);
-        // A columns: c0 = (a1.w,a2.x,a2.y) c1 = (a2.z,a2.w,a3.x) c2 = (a3.y,a3.z,a3.w)
-        // q = m v + A rel ;  node (i,j,k): q - i c0 - j c1 - k c2   (dpos = rel - node, 528-536)
-        const float q0 = fmaf(a3.y, rz, fmaf(a2.z, ry, fmaf(a1.w, rx, mass * vx)));
-        const float q1 = fmaf(a3.z, rz, fmaf(a2.w, ry, fmaf(a2.x, rx, mass * vy)));
-        const float q2 = fmaf(a3.w, rz, fmaf(a3.x, ry, fmaf(a2.y, rx, mass * vz)));
-        // (momentum | mass) as register pairs; the mass lane rides along with zero column entries
-        const F4 Q = {make_float2(q0, q1), make_float2(q2, mass)};
-        const F4 c0 = {make_float2(a1.w, a2.x), make_float2(a2.y, 0.f)}, c1 = {make_float2(a2.z, a2.w), make_float2(a3.x, 0.f)},
-                 c2 = {make_float2(a3.y, a3.z), make_float2(a3.w, 0.f)};
-        const float2 m2 = bc2(-2.0f);
-        const float2 wx2[3] = {bc2(wx[0]), bc2(wx[1]), bc2(wx[2])}, wy2[3] = {bc2(wy[0]), bc2(wy[1]), bc2(wy[2])},
-                     wz2[3] = {bc2(wz[0]), bc2(wz[1]), bc2(wz[2])};
-#pragma unroll
-        for (int i = 0; i < 3; i++) {
-          const F4 U = i == 0 ? Q : (i == 1 ? f4_sub(Q, c0) : f4_fma(m2, c0, Q));    // q - i c0
-#pragma unroll
-          for (int j = 0; j < 3; j++) {
-            const F4 T = j == 0 ? U : (j == 1 ? f4_sub(U, c1) : f4_fma(m2, c1, U));  // ... - j c1
-            const float2 wij = mul2(wx2[i], wy2[j]);
-#pragma unroll
-            for (int k = 0; k < 3; k++) {
-              const float2 w = mul2(wij, wz2[k]);
-              const F4 N = k == 0 ? T : (k == 1 ? f4_sub(T, c2) : f4_fma(m2, c2, T));  // ... - k c2
-              acc[i * 9 + j * 3 + k] = f4_fma(w, N, acc[i * 9 + j * 3 + k]);
-            }
-          }
-        }
-      }
+      // ---- 3: accumulate my half of my cell's stencil in registers.  A warp iterates as long as its fullest cell has
+      // particles; in a developed flow (cells hold 0..30 particles) that is the kernel's cost.  Tried and dropped:
+      // capping the loop and adding the excess particles with one lane per stencil node (the serialised excess pass
+      // costs more than the idle tail), re-assigning cells to threads per tile so that warp 0 owns the fuller cells, and
+      // software-pipelining the row fetch: the kernel is latency-bound, an early warp's issue slots are not what it lacks.
+      const int i0 = s_start[own], i1 = s_start[own + 1];
+      if (half == 0)
+        p2g_accumulate<0>(acc, s_rows, s_order, i0, i1, P, fbx, fby, fbz);
+      else
+        p2g_accumulate<1>(acc, s_rows, s_order, i0, i1, P, fbx, fby, fbz);
       vbase += s_start[64];
       __syncthreads();  // rows / order / hist are reused by the next chunk
     }
-    // ---- 4: both warps flush at once, warp 0 into s_arena, warp 1 into a second arena laid over the
-    // row staging area (free after the last chunk's barrier; zeroed by warp 1 itself, so a __syncwarp
-    // is all it needs).  The store below sums the two in a fixed order: still bit-reproducible.
+    // ---- 4: cells 0-31 flush into s_arena, cells 32-63 into a second arena laid over the row staging area (free after
+    // the last chunk's barrier; zeroed by warp 1 itself, so a __syncwarp is all it needs).  Warps 0-1 flush steps
+    // [0, 14), then warps 2-3 flush [14, 27): every node receives its adds in ascending step order, as from one thread
+    // holding the whole stencil.  The store below sums the two arenas in a fixed order: still bit-reproducible.
     float (*ar1)[AR_SIZE] = reinterpret_cast<float (*)[AR_SIZE]>(&s_rows[0][0]);
     {
-      if (warp == 1) {
-        for (int n = lane; n < 4 * AR_SIZE; n += 32) (&ar1[0][0])[n] = 0.f;
-        __syncwarp();
-      }
-      float (*ar)[AR_SIZE] = warp == 0 ? s_arena : ar1;
+      float (*ar)[AR_SIZE] = (warp & 1) ? ar1 : s_arena;
       const int nb = cx * AR_SX + cy * AR_SY + cz;
-#pragma unroll
-      for (int i = 0; i < 3; i++)
-#pragma unroll
-        for (int j = 0; j < 3; j++)
-#pragma unroll
-          for (int k = 0; k < 3; k++) {
-            const int node = nb + i * AR_SX + j * AR_SY + k;
-            const F4 &a = acc[i * 9 + j * 3 + k];
-            ar[0][node] += a.lo.x;
-            ar[1][node] += a.lo.y;
-            ar[2][node] += a.hi.x;
-            ar[3][node] += a.hi.y;
-            __syncwarp();
-          }
+      if (half == 0) {
+        if (warp == 1) {
+          for (int n = lane; n < 4 * AR_SIZE; n += 32) (&ar1[0][0])[n] = 0.f;
+          __syncwarp();
+        }
+        p2g_flush<0>(acc, ar, nb);
+      }
+      __syncthreads();
+      if (half == 1) p2g_flush<1>(acc, ar, nb);
     }
     __syncthreads();
     float4 *out = V.arena + (size_t)slot * ARENA;
