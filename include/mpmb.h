@@ -182,6 +182,25 @@ int mpmb_upload_aos(MpmbHandle h, int64_t n, const void *pool, int64_t pool_slot
  * particles within 7 cells of a face are not created (src/mpm.cpp:129-132).  Replaces the resident set.           */
 int mpmb_seed_lattice(MpmbHandle h, const int32_t lo_cell[3], const int32_t hi_cell[3], float vol, float mass, float jitter,
                       uint32_t seed, int32_t group, const float v0[3], int64_t *n_seeded);
+/* Appends n particles to the resident set (MPM<3>::add_particles' push onto `particles`, src/mpm.cpp:147; ids from
+ * ParticleAllocator::particle_counter, src/particle_allocator.h:72).  Fields as mpmb_upload_particles (F, b, scalar,
+ * group may be NULL).  Resident particles keep their rows' state, ids and CPIC colours; the new ones get ids
+ * id_base + id_span .. + n - 1, where id_span is the end of the ids handed out so far (n of an upload, the lattice range
+ * of mpmb_seed_lattice, plus every earlier append); *first_id (may be NULL) receives the first, also for n == 0, which
+ * changes nothing.  The same rule as an upload drops particles that are not finite or whose stencil leaves the node grid
+ * (they still consume their ids).  The storage needs the resident rows plus n: with capacity == 0 it grows (by at least
+ * half) keeping the resident rows; a configured capacity that is too small returns MPMB_ERR_CAPACITY and changes
+ * nothing.  Ids past 2^28 return MPMB_ERR_CAPACITY.  The whole set is ordered again, as after an upload, so the next
+ * substep is not replayed from a graph.  After an append the index vector of an earlier mpmb_upload_aos does not cover
+ * the new ids: mpmb_download_aos then reports MPMB_ERR_INVALID (the new particles are not written anywhere) and the
+ * AoS caller must upload again.  Between substeps; world == 1 (else MPMB_ERR_STATE).                                    */
+int mpmb_append_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
+                          const float *mass, const float *vol, const float *scalar, const int32_t *group, int64_t *first_id);
+/* delete_particles_inside_level_set (src/mpm.cpp:959-973): removes every live particle whose level set value, trilinear
+ * in the node phi of the current level set at x / dx (clamped to the node grid, node values capped at 1e20), is < 0.
+ * Survivors keep their ids and state; *n_deleted receives the number removed.  No level set: deletes none.  Between
+ * substeps; world == 1 (else MPMB_ERR_STATE).                                                                           */
+int mpmb_delete_inside_levelset(MpmbHandle h, int64_t *n_deleted);
 /* Number of live particles, counted on the device (4 bytes cross the bus; synchronises).
  * Reference: particles.size().                                                                    */
 int mpmb_num_particles(MpmbHandle h, int64_t *n);

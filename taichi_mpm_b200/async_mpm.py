@@ -104,6 +104,8 @@ class AsyncMPM(MPM):
         if kwargs.get("type") == "rigid":
             raise ValueError("AsyncMPM with rigid bodies is not supported")
         before = None if self._host is None else len(self._host["x"])
+        # the pools own the particles and advance() uploads them itself, so _n_uploaded stays 0: MPM.add_particles never
+        # appends on the device here, it always leaves the new particles in self._host
         ret = super().add_particles(**kwargs)
         h = self._host
         lo = 0 if before is None else before

@@ -284,7 +284,9 @@ __global__ void k_iota(uint32_t *a, int n) {
   if (i < n) a[i] = (uint32_t)i;
 }
 
-__device__ __forceinline__ void pack_one(View &V, const Params &P, int i, uint32_t id_base, float3 x, float3 v, Mat3 F, Mat3 b, float mass, float vol, float ps,
+// one particle into storage row `row` with id `id` (an upload: row = upload index, id = id_base + upload index; an append:
+// the rows after the resident ones and the ids after the ones handed out so far)
+__device__ __forceinline__ void pack_one(View &V, const Params &P, int row, uint32_t id, float3 x, float3 v, Mat3 F, Mat3 b, float mass, float vol, float ps,
                                          int g, uint32_t *keys) {
   // a hole is encoded by the sign of the mass and the group by 4 tag bits: reject what cannot be represented
   if (g < 0 || g >= MPMB_MAX_GROUPS || !(mass > 0.f)) {
@@ -295,13 +297,13 @@ __device__ __forceinline__ void pack_one(View &V, const Params &P, int i, uint32
   Mat3 force, A;
   calculate_force(P.mats[g], F, ps, vol, force);
   make_affine(force, b, mass, -4.0f * P.inv_dx * P.dt, A);
-  store_particle(V.q, (size_t)i, x, mass, v, A, F, ps, vol, ((uint32_t)g << TAG_ID_BITS) | (id_base + (uint32_t)i), b);
-  keys[i] = make_key(P, x.x, x.y, x.z);
+  store_particle(V.q, (size_t)row, x, mass, v, A, F, ps, vol, ((uint32_t)g << TAG_ID_BITS) | id, b);
+  keys[row] = make_key(P, x.x, x.y, x.z);
 }
 
-// Field-wise host arrays (staged on the device) -> q streams.
+// Field-wise host arrays (staged on the device) -> q streams: particle i into row row0 + i with id id0 + i.
 __global__ void k_pack_particles(View V, Params P, int n, const float *x, const float *v, const float *F, const float *b,
-                                 const float *mass, const float *vol, const float *scalar, const int *group, uint32_t *keys, uint32_t id_base) {
+                                 const float *mass, const float *vol, const float *scalar, const int *group, uint32_t *keys, int row0, uint32_t id0) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   Mat3 f, bb;
@@ -319,7 +321,7 @@ __global__ void k_pack_particles(View V, Params P, int n, const float *x, const 
   }
   float3 xx = make_float3(x[3 * (size_t)i], x[3 * (size_t)i + 1], x[3 * (size_t)i + 2]);
   float3 vv = make_float3(v[3 * (size_t)i], v[3 * (size_t)i + 1], v[3 * (size_t)i + 2]);
-  pack_one(V, P, i, id_base, xx, vv, f, bb, mass[i], vol[i], ps, g, keys);
+  pack_one(V, P, row0 + i, id0 + (uint32_t)i, xx, vv, f, bb, mass[i], vol[i], ps, g, keys);
 }
 
 // Reference AoS slots (staged on the device) -> q streams.
@@ -342,7 +344,7 @@ __global__ void k_pack_aos(View V, Params P, int n, const unsigned char *pool, c
   int g = group ? group[i] : 0;
   float vol = *(const float *)(s + L.off_vol);
   float ps = L.off_scalar >= 0 ? *(const float *)(s + L.off_scalar) : 0.f;
-  pack_one(V, P, i, id_base, make_float3(pos[0], pos[1], pos[2]), make_float3(vm[0], vm[1], vm[2]), f, bb, vm[3], vol, ps, g, keys);
+  pack_one(V, P, i, id_base + (uint32_t)i, make_float3(pos[0], pos[1], pos[2]), make_float3(vm[0], vm[1], vm[2]), f, bb, vm[3], vol, ps, g, keys);
 }
 
 // q streams -> field-wise arrays, compacting live particles (storage order).
@@ -390,6 +392,45 @@ __global__ void k_alive_flags(const uint32_t *keys, int n, uint32_t special_min,
 __global__ void k_fill_u32(uint32_t *a, int n, uint32_t v) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) a[i] = v;
+}
+
+// delete_particles_inside_level_set (src/mpm.cpp:959-973): phi at X = x / dx, trilinear in the node phi (clamped to
+// [0, nnode - 1 - 1e-9], node values capped at 1e20), in double as LevelSet.sample in mpm.py computes it.  A live row
+// with phi < 0 gets the dead key (the next ordering drops it); the killed rows are counted into cnt->n_live.
+__global__ void __launch_bounds__(256) k_delete_inside(View V, Params P, int n, uint32_t special_min, uint32_t key_dead) {
+  typedef cub::BlockReduce<int, 256> Red;
+  __shared__ typename Red::TempStorage tmp;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  int killed = 0;
+  if (i < n && V.keys[i] < special_min) {
+    const float4 q0 = V.q[0][i];
+    const double xs[3] = {(double)q0.x, (double)q0.y, (double)q0.z};
+    int i0[3];
+    double f[3];
+#pragma unroll
+    for (int a = 0; a < 3; a++) {
+      const double X = fmin(fmax(xs[a] / (double)P.dx, 0.0), (double)(P.nnode[a] - 1) - 1e-9);
+      i0[a] = (int)floor(X);
+      f[a] = X - (double)i0[a];
+    }
+    double phi = 0.0;
+#pragma unroll
+    for (int a = 0; a < 2; a++)
+#pragma unroll
+      for (int b = 0; b < 2; b++)
+#pragma unroll
+        for (int c = 0; c < 2; c++) {
+          const double w = (a ? f[0] : 1.0 - f[0]) * (b ? f[1] : 1.0 - f[1]) * (c ? f[2] : 1.0 - f[2]);
+          const float s = V.sdf4[((size_t)(i0[0] + a) * P.nnode[1] + (i0[1] + b)) * P.nnode[2] + (i0[2] + c)].w;
+          phi += w * (double)fminf(s, 1e20f);
+        }
+    if (phi < 0.0) {
+      V.keys[i] = key_dead;
+      killed = 1;
+    }
+  }
+  killed = Red(tmp).Sum(killed);
+  if (threadIdx.x == 0 && killed) atomicAdd(&V.cnt->n_live, killed);
 }
 
 // ------------------------------------------------------------------------------ device-side seeding
@@ -2668,18 +2709,34 @@ static int ensure_capacity(MpmbEngine *h, int64_t n) {
   return MPMB_OK;
 }
 
-static int rigid_reserve_ids(MpmbEngine *h, int64_t n_ids);
-static int finish_upload(MpmbEngine *h, int64_t n) {
-  // Fresh storage in upload order: no runs yet, every particle is an "arrival" of its tile.  The
-  // one radix sort of the engine's life (per upload) groups the rows by tile; the ordinary
-  // ordering scan then lays out the first runs.
-  h->id_span = std::max<int64_t>(h->id_span_pending, n);
-  h->id_span_pending = 0;
-  if (h->rigid_on) {  // new particles start with MPMParticle::states = 0 (mpmb_set_particle_states overrides)
-    int rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap));
-    if (rc != MPMB_OK) return rc;
-    CUDA_TRY(h, cudaMemsetAsync(h->R.p_states, 0, sizeof(uint32_t) * h->R.id_cap, h->stream));
+// Room for `need` rows that keeps rows [0, n_keep) of the current storage (an append onto a resident set).  With a
+// configured capacity that is too small nothing changes; otherwise the buffers grow by at least half, so that a source
+// that appends every frame reallocates rarely.
+static int grow_keeping_rows(MpmbEngine *h, int64_t need, int n_keep) {
+  if (need <= h->cap) return MPMB_OK;
+  if (h->cfg.capacity > 0)
+    return fail(h, MPMB_ERR_CAPACITY, "%lld particle rows exceed the configured capacity %lld", (long long)need, (long long)h->cap);
+  const int64_t want = std::max<int64_t>(need, std::min<int64_t>(h->cap + h->cap / 2, (1ll << 30) - 1));
+  float4 *old_q[N_Q];
+  uint32_t *old_keys = h->keys[h->cur];
+  for (int k = 0; k < N_Q; k++) { old_q[k] = h->q[h->cur][k]; h->q[h->cur][k] = nullptr; }
+  h->keys[h->cur] = nullptr;
+  int rc = alloc_particles(h, want);   // frees everything else (scratch, the other buffer) and resets the graphs
+  if (rc == MPMB_OK && n_keep > 0) {
+    for (int k = 0; k < N_Q; k++)
+      CUDA_TRY(h, cudaMemcpyAsync(h->q[h->cur][k], old_q[k], sizeof(float4) * n_keep, cudaMemcpyDeviceToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->keys[h->cur], old_keys, sizeof(uint32_t) * n_keep, cudaMemcpyDeviceToDevice, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   }
+  for (int k = 0; k < N_Q; k++) cudaFree(old_q[k]);
+  cudaFree(old_keys);
+  return rc;
+}
+
+// Orders rows [0, n_rows) of the current storage from scratch: no runs yet, every live row is an "arrival" of its tile.
+// One radix sort groups the rows by tile (dead keys sort past every tile, so rows killed since the last ordering drop
+// out here); the ordinary ordering scan then lays out the first runs.  The next substep runs outside the graph.
+static int reorder_from_scratch(MpmbEngine *h, int64_t n_rows) {
   View V = make_view(h);
   const size_t dense = sizeof(int) * (size_t)h->ntot;
   CUDA_TRY(h, cudaMemsetAsync(h->run_begin[h->ord], 0, dense, h->stream));
@@ -2687,12 +2744,12 @@ static int finish_upload(MpmbEngine *h, int64_t n) {
   CUDA_TRY(h, cudaMemsetAsync(h->stay[h->ord], 0, dense, h->stream));
   CUDA_TRY(h, cudaMemsetAsync(h->arr_cnt, 0, dense, h->stream));
   Counters c{};
-  c.n_store = (int)n;
+  c.n_store = (int)n_rows;
   CUDA_TRY(h, cudaMemcpyAsync(h->cnt, &c, sizeof(int) * 3, cudaMemcpyHostToDevice, h->stream));          // n_store, n_tiles, n_ghost
   CUDA_TRY(h, cudaMemsetAsync(&h->cnt->n_movers, 0, sizeof(int) * 3, h->stream));                          // n_movers, n_movers_next, n_alive
-  if (n > 0) {
-    cub::DeviceRadixSort::SortPairs(h->cub_temp, h->cub_bytes, h->keys[h->cur], h->keys_sorted, h->iota, h->arrivals_sorted, (int)n, 0, h->key_bits, h->stream);
-    k_count_sorted<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(V, h->keys_sorted, (int)n, h->ntot);
+  if (n_rows > 0) {
+    cub::DeviceRadixSort::SortPairs(h->cub_temp, h->cub_bytes, h->keys[h->cur], h->keys_sorted, h->iota, h->arrivals_sorted, (int)n_rows, 0, h->key_bits, h->stream);
+    k_count_sorted<<<(unsigned)((n_rows + 255) / 256), 256, 0, h->stream>>>(V, h->keys_sorted, (int)n_rows, h->ntot);
     h->launches++;
   }
   h->fresh = true;
@@ -2702,15 +2759,22 @@ static int finish_upload(MpmbEngine *h, int64_t n) {
   return MPMB_OK;
 }
 
-int mpmb_upload_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
-                          const float *mass, const float *vol, const float *scalar, const int32_t *group) {
-  CHECK_HANDLE(h);
-  if (n < 0 || (n > 0 && (!x || !v || !mass || !vol))) return fail(h, MPMB_ERR_INVALID, "x, v, mass, vol are required");
-  if ((int64_t)h->id_base + n > (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_CAPACITY, "particle ids exceed 2^%d", TAG_ID_BITS);
-  h->aos_host_pool = nullptr;
-  int rc = ensure_capacity(h, n);
-  if (rc != MPMB_OK) return rc;
-  if (n == 0) return finish_upload(h, 0);
+static int rigid_reserve_ids(MpmbEngine *h, int64_t n_ids);
+// A new resident set of n rows (upload, seeding): its id span, fresh rigid colours, then the ordering.
+static int finish_upload(MpmbEngine *h, int64_t n) {
+  h->id_span = std::max<int64_t>(h->id_span_pending, n);
+  h->id_span_pending = 0;
+  if (h->rigid_on) {  // new particles start with MPMParticle::states = 0 (mpmb_set_particle_states overrides)
+    int rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap));
+    if (rc != MPMB_OK) return rc;
+    CUDA_TRY(h, cudaMemsetAsync(h->R.p_states, 0, sizeof(uint32_t) * h->R.id_cap, h->stream));
+  }
+  return reorder_from_scratch(h, n);
+}
+
+// Stages n field-wise particles on the device and packs them into rows row0.. with ids id0.. of the current storage.
+static int pack_fields(MpmbEngine *h, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
+                       const float *vol, const float *scalar, const int32_t *group, int row0, uint32_t id0) {
   // stage the field arrays on the device (one allocation)
   size_t fl = (size_t)n * (3 + 3 + (F ? 9 : 0) + (b ? 9 : 0) + 1 + 1 + (scalar ? 1 : 0)) + (group ? (size_t)n : 0);
   float *stage = nullptr;
@@ -2734,12 +2798,77 @@ int mpmb_upload_particles(MpmbHandle h, int64_t n, const float *x, const float *
         *ds = put(scalar, n);
   int *dg = (int *)put(group, n);
   View V = make_view(h);
-  k_pack_particles<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, dx_, dv, dF, db, dm, dvol, ds, dg, h->keys[h->cur], h->id_base);
+  k_pack_particles<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, dx_, dv, dF, db, dm, dvol, ds, dg, h->keys[h->cur], row0, id0);
   h->launches++;
   cudaError_t e = cudaStreamSynchronize(h->stream);
   CUDA_TRY(h, e);
   CUDA_TRY(h, cudaGetLastError());
+  return MPMB_OK;
+}
+
+int mpmb_upload_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
+                          const float *mass, const float *vol, const float *scalar, const int32_t *group) {
+  CHECK_HANDLE(h);
+  if (n < 0 || (n > 0 && (!x || !v || !mass || !vol))) return fail(h, MPMB_ERR_INVALID, "x, v, mass, vol are required");
+  if ((int64_t)h->id_base + n > (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_CAPACITY, "particle ids exceed 2^%d", TAG_ID_BITS);
+  h->aos_host_pool = nullptr;
+  int rc = ensure_capacity(h, n);
+  if (rc != MPMB_OK) return rc;
+  if (n > 0 && (rc = pack_fields(h, n, x, v, F, b, mass, vol, scalar, group, 0, h->id_base)) != MPMB_OK) return rc;
   return finish_upload(h, n);
+}
+
+// Edits of the resident set between substeps (single-GPU engines): the rows already there keep their state, ids and
+// CPIC colours; the whole set is ordered again from scratch, as after an upload.
+static int edit_allowed(MpmbEngine *h, const char *what) {
+  if (h->cfg.world > 1) return fail(h, MPMB_ERR_STATE, "%s is implemented for single-GPU engines (world == 1)", what);
+  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "%s runs between substeps, not inside one", what);
+  return MPMB_OK;
+}
+
+int mpmb_append_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
+                          const float *mass, const float *vol, const float *scalar, const int32_t *group, int64_t *first_id) {
+  CHECK_HANDLE(h);
+  if (n < 0 || (n > 0 && (!x || !v || !mass || !vol))) return fail(h, MPMB_ERR_INVALID, "x, v, mass, vol are required");
+  int rc = edit_allowed(h, "append");
+  if (rc != MPMB_OK) return rc;
+  const int64_t id0 = h->id_span;
+  if ((int64_t)h->id_base + id0 + n > (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_CAPACITY, "particle ids exceed 2^%d", TAG_ID_BITS);
+  if (first_id) *first_id = (int64_t)h->id_base + id0;
+  if (n == 0) return MPMB_OK;
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  int ns = 0;
+  if ((rc = read_n_store(h, &ns)) != MPMB_OK) return rc;
+  if ((rc = grow_keeping_rows(h, (int64_t)ns + n, ns)) != MPMB_OK) return rc;
+  h->aos_host_pool = nullptr;   // the AoS index vector does not cover the new ids: mpmb_download_aos needs a new upload
+  if ((rc = pack_fields(h, n, x, v, F, b, mass, vol, scalar, group, ns, h->id_base + (uint32_t)id0)) != MPMB_OK) return rc;
+  h->id_span = id0 + n;
+  if (h->rigid_on && (rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap))) != MPMB_OK) return rc;   // keeps the colours
+  return reorder_from_scratch(h, (int64_t)ns + n);
+}
+
+int mpmb_delete_inside_levelset(MpmbHandle h, int64_t *n_deleted) {
+  CHECK_HANDLE(h);
+  if (!n_deleted) return fail(h, MPMB_ERR_INVALID, "null argument");
+  *n_deleted = 0;
+  int rc = edit_allowed(h, "delete_inside_levelset");
+  if (rc != MPMB_OK) return rc;
+  h->aos_host_pool = nullptr;
+  if (!h->P.has_sdf || h->cap == 0) return MPMB_OK;
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  int ns = 0;
+  if ((rc = read_n_store(h, &ns)) != MPMB_OK) return rc;
+  if (ns == 0) return MPMB_OK;
+  CUDA_TRY(h, cudaMemsetAsync(&h->cnt->n_live, 0, sizeof(int), h->stream));
+  View V = make_view(h);
+  k_delete_inside<<<(unsigned)((ns + 255) / 256), 256, 0, h->stream>>>(V, h->P, ns, h->special_min, h->key_dead);
+  h->launches++;
+  int killed = 0;
+  CUDA_TRY(h, cudaMemcpyAsync(&killed, &h->cnt->n_live, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  *n_deleted = killed;
+  return killed > 0 ? reorder_from_scratch(h, ns) : MPMB_OK;
 }
 
 // flags / exclusive prefix scratch for n items (grow-only) and the CUB scan over them

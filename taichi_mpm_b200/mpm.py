@@ -157,6 +157,8 @@ class MPM:
         self._host = None         # pending host-side particle set (dict of arrays)
         self._dirty = False
         self._n_uploaded = 0
+        self._id_base = 0         # the engine's id base (set by 'load')
+        self._id_span = 0         # ids handed out since the last upload: [id_base, id_base + _id_span)
 
     # ---- level set
     def create_levelset(self):
@@ -215,6 +217,12 @@ class MPM:
         st = scenes.make_state(x, mass, vol, kind, group, kwargs.get("initial_velocity", (0.0, 0.0, 0.0)))
         if kind == scenes.MAT_VISCO and "tau" in kwargs:                         # visco_tau, src/particles.cpp:62
             st["ps"][:] = np.float32(kwargs["tau"])
+        if self._host is None and self._n_uploaded > 0 and hasattr(self.engine, "append"):
+            # particles are resident and no host copy is pending: append on the device (mpm.cpp:147), the resident
+            # particles keep their ids and state, the new ones are numbered after every id handed out so far
+            first = self.engine.append(st["x"], st["v"], st["mass"], st["vol"], st["F"], st["b"], st["ps"], st["group"])
+            self._id_span = max(self._id_span, int(first) - self._id_base + len(st["x"]))
+            return ""
         cur = self._pull_host()
         if cur is None:
             self._host = st
@@ -314,6 +322,7 @@ class MPM:
             h = self._host
             self.engine.upload(h["x"], h["v"], h["mass"], h["vol"], h["F"], h["b"], h["ps"], h["group"])
             self._n_uploaded = len(h["x"])
+            self._id_span = len(h["x"])     # an upload numbers its particles id_base + 0..n-1
             self._dirty = False
             self._host = None
 
@@ -412,7 +421,8 @@ class MPM:
         return fn
 
     def _id_range(self):
-        return max(int(self._n_uploaded), 1)
+        # ids lie in [id_base, id_base + id span): the last upload plus every device append since
+        return max(int(self._id_span), 1)
 
     def general_action(self, **kwargs):
         """The actions of MPM<dim>::general_action (src/mpm.cpp:920-976) that concern the accelerated
@@ -451,6 +461,9 @@ class MPM:
             return ""
         if action == "delete_particles_inside_level_set":                      # mpm.cpp:958-972
             ls = getattr(self, "_levelset", None)
+            if ls is not None and self._host is None and self._n_uploaded > 0 and hasattr(self.engine, "delete_inside_levelset"):
+                self.engine.delete_inside_levelset()     # on the device: the survivors keep their ids and state
+                return ""
             p = self.get_particles()
             if ls is None or len(p["x"]) == 0:
                 return ""
@@ -504,5 +517,6 @@ class MPM:
         ids = ids[order]
         base = int(ids[0]) if len(ids) and np.array_equal(ids - ids[0], np.arange(len(ids), dtype=ids.dtype)) else 0
         self.engine.set_id_base(base)
+        self._id_base = base
         self._host = h
         self._push()
