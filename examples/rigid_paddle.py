@@ -3,8 +3,9 @@
 
     python examples/rigid_paddle.py [frames] [res]
 
-The colour field, gather_cdf and the coupled transfers run on the device; the paddle's motion is host code (a Python callable
-where the reference wraps one in tc.function13)."""
+The colour field, gather_cdf, the coupled transfers and the paddle's advance run on the device, a whole frame per engine call;
+the paddle's motion is a Python callable (where the reference wraps one in tc.function13), evaluated on the host once per frame
+into the table of poses the device follows."""
 import sys
 
 import numpy as np

@@ -261,13 +261,16 @@ int mpmb_download_grid(MpmbHandle h, int32_t which, float *dense4);
 /* Two-way coupling with rigid bodies as the reference's optimized path does it (SURVEY §8f row 2).  On the device:
  * update_rigid_page_map (src/mpm.cpp:1026-1076), rasterize_rigid_boundary and gather_cdf (src/rigid_transfer.cpp:18-113,
  * 120-274) and the block_op_rigid branches of rasterize_optimized / resample_optimized (src/transfer.cpp:367-463, 706-835),
- * selected per 4x4x8-node page exactly as block_op_switch does.  On the host, as in the reference: the bodies themselves
- * (RigidBody: integration, scripted motion, rigid-rigid collisions, articulation — src/mpm_rigid_body.cpp:252-330 call into
- * the reference's un-vendored core for these).  Per substep the host hands over poses and velocities and reads the
- * velocities back:
- *     mpmb_set_rigid_state -> mpmb_substep(h, 1) -> mpmb_get_rigid_state -> host: advect_rigid_bodies
- * (mpmb_substep(h, n > 1) keeps the pose fixed over the n substeps.)  CUDA-graph replay is off while bodies are present.
- * Single-GPU engines only (world == 1).
+ * selected per 4x4x8-node page exactly as block_op_switch does.  The bodies themselves (RigidBody: integration, scripted
+ * motion, rigid-rigid collisions, articulation — src/mpm_rigid_body.cpp:252-330 call into the reference's un-vendored core for
+ * these) are advanced in one of two ways:
+ *   - by the host (the default): per substep the host hands over poses and velocities and reads the velocities back,
+ *         mpmb_set_rigid_state -> mpmb_substep(h, 1) -> mpmb_get_rigid_state -> host: advect_rigid_bodies
+ *     (mpmb_substep(h, n > 1) keeps the pose fixed over the n substeps; no CUDA-graph replay);
+ *   - on the device, after mpmb_set_rigid_motion: every substep ends with advect_rigid_bodies (and, if asked for,
+ *     rigid_body_levelset_collision) on an fp64 master state per body, scripted parts taken from a table the host uploads
+ *     with mpmb_set_rigid_script.  mpmb_substep(h, n) then runs n whole coupled substeps and replays CUDA graphs.
+ * Rigid-rigid collisions (rigidify) and articulation are not implemented.  Single-GPU engines only (world == 1).
  * What the device assumes of the core's RigidBody (it cannot be read here; SURVEY appendix C):
  *   get_velocity_at(p) = velocity + angular_velocity x (p - position);
  *   apply_tmp_impulse(j, p): tmp_velocity += inv_mass j, tmp_angular_velocity += inv_inertia ((p - position) x j);
@@ -291,11 +294,47 @@ typedef struct MpmbRigidBody {
 int mpmb_set_rigid_samples(MpmbHandle h, int32_t n_bodies, int64_t n_samples, const float *offset3, const float *tri9,
                            const int32_t *rigid_id);
 /* `penalty` (src/mpm.cpp:35, default 0) and `pushing_force` (src/mpm.cpp:40, default 20000).                          */
+/* (mpmb_set_rigid_samples switches device advection off: the motion records describe one set of bodies.)               */
 int mpmb_set_rigid_coupling(MpmbHandle h, float penalty, float pushing_force);
-/* Poses and velocities of all n_bodies bodies (entry 0 ignored) for the next substep(s).                              */
+/* Poses and velocities of all n_bodies bodies (entry 0 ignored) for the next substep(s).  With device advection on it also
+ * restarts the fp64 master states from these (fp32) values.                                                           */
 int mpmb_set_rigid_state(MpmbHandle h, int32_t n_bodies, const MpmbRigidBody *bodies);
-/* The same records with velocity / angular_velocity as the two transfers left them (synchronises).                    */
+/* The same records (synchronises).  Host-advanced bodies: velocity / angular_velocity as the two transfers of the last
+ * substep left them, the pose as set.  Device-advanced bodies: the advanced pose and velocities (fp32 copies of the master
+ * state) and the world-space inverse inertia of that pose.                                                            */
 int mpmb_get_rigid_state(MpmbHandle h, int32_t n_bodies, MpmbRigidBody *bodies);
+/* Device advection (advect_rigid_bodies, src/mpm_rigid_body.cpp:273-287), one record per body (entry 0 ignored: the
+ * background body is never advanced).  After the second transfer of every substep, per body in fp64:
+ *   [levelset_collision != 0 and a level set is set: rigid_body_levelset_collision (src/mpm_rigid_body.cpp:347-384) — phi
+ *    trilinear in the node phi at every boundary sample, its central-difference gradient (eps 0.25 grid units) normalised,
+ *    normal + Coulomb friction impulses (frictions[0]) with restitution applied sample after sample in sample order;
+ *    bodies with zero inverse mass and inertia are skipped]
+ *   enforce the rotation axis; free position: v *= exp(-linear_damping dt), x += v dt; scripted position: x, v of the script
+ *   entry; free rotation: w *= exp(-angular_damping dt), R = exp([w dt]x) R; scripted rotation: R, w of the entry; gravity
+ *   impulse v += g mass dt inv_mass (inv_mass = 0 for a scripted position, else 1 / mass); enforce the axis again;
+ *   inverse inertia = R inv_inertia_body R^T.
+ * The master states start from the current records (mpmb_set_rigid_state, before or after this call).  Velocities entering a
+ * substep's advance are the fp32 values the transfers produced, as a host reading them back sees them.  Requires
+ * mpmb_set_rigid_samples first (else MPMB_ERR_STATE); n_bodies must match (else MPMB_ERR_INVALID), fields finite and a free
+ * body's mass positive (else MPMB_ERR_INVALID).  n_bodies == 0 switches device advection off (host-advanced contract).
+ * Resets the script (no entries left).  The level-set collision runs after the transfers of a substep, not between the grid
+ * normalisation and the grid boundary condition as in the reference (src/mpm.cpp:535-538).                            */
+typedef struct MpmbRigidMotion {
+  float mass;
+  float inv_inertia_body[9];   /* body frame, column-major; all 0 = scripted / infinite inertia                      */
+  float rotation_axis[3];      /* enforce_angular_velocity_parallel_to when max |axis| > 0.1                        */
+  float linear_damping, angular_damping, restitution;
+  int32_t scripted_position, scripted_rotation;
+  int32_t reserved[4];
+} MpmbRigidMotion;
+int mpmb_set_rigid_motion(MpmbHandle h, int32_t n_bodies, const MpmbRigidMotion *motion, int32_t levelset_collision);
+/* Script table of the scripted parts: poses[n_substeps][n_bodies][18] = position (3), rotation (9, column-major), velocity
+ * (3), angular velocity (3) at the END of substep k; only the scripted parts of an entry are read.  Resets the cursor;
+ * every device advance consumes one entry.  When a scripted body is present and fewer than nsub entries are left,
+ * mpmb_substep(h, nsub) returns MPMB_ERR_STATE and enqueues nothing (mpmb_resample likewise with none left).  Needs
+ * mpmb_set_rigid_motion first (else MPMB_ERR_STATE); n_substeps < 0, a NULL table or non-finite scripted parts:
+ * MPMB_ERR_INVALID.  The table is copied (synchronises).                                                               */
+int mpmb_set_rigid_script(MpmbHandle h, int32_t n_substeps, const double *poses);
 /* MPMParticle::states (src/particles.h) by particle id - id_base: set (default 0 for uploaded particles) / read together
  * with boundary_normal, boundary_distance and near_boundary_ of the last substep.  Any pointer may be NULL.            */
 int mpmb_set_particle_states(MpmbHandle h, int64_t n, const uint32_t *states);

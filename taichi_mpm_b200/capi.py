@@ -27,7 +27,8 @@ EXPORTS = [
     "mpmb_resample_part", "mpmb_download_grid",
     "mpmb_set_profiling", "mpmb_get_profile", "mpmb_get_counters", "mpmb_get_ordering_stats",
     "mpmb_halo_bytes", "mpmb_halo_pack", "mpmb_halo_unpack", "mpmb_migrate_bytes", "mpmb_migrate_pack", "mpmb_migrate_unpack",
-    "mpmb_set_rigid_samples", "mpmb_set_rigid_coupling", "mpmb_set_rigid_state", "mpmb_get_rigid_state", "mpmb_set_particle_states",
+    "mpmb_set_rigid_samples", "mpmb_set_rigid_coupling", "mpmb_set_rigid_state", "mpmb_get_rigid_state", "mpmb_set_rigid_motion",
+    "mpmb_set_rigid_script", "mpmb_set_particle_states",
     "mpmb_get_particle_cdf", "mpmb_download_cdf",
     "mpmb_xchg_buffer", "mpmb_xchg_ipc_handle", "mpmb_xchg_connect", "mpmb_halo_send", "mpmb_halo_recv", "mpmb_migrate_send", "mpmb_migrate_recv",
 ]
@@ -69,6 +70,15 @@ class MpmbShape(C.Structure):
 class MpmbRigidBody(C.Structure):
     _fields_ = [("position", C.c_float * 3), ("rot", C.c_float * 9), ("velocity", C.c_float * 3), ("angular_velocity", C.c_float * 3),
                 ("inv_mass", C.c_float), ("inv_inertia", C.c_float * 9), ("frictions", C.c_float * 2)]
+
+
+class MpmbRigidMotion(C.Structure):
+    _fields_ = [("mass", C.c_float), ("inv_inertia_body", C.c_float * 9), ("rotation_axis", C.c_float * 3), ("linear_damping", C.c_float),
+                ("angular_damping", C.c_float), ("restitution", C.c_float), ("scripted_position", C.c_int32), ("scripted_rotation", C.c_int32),
+                ("reserved", C.c_int32 * 4)]
+
+
+RIGID_SCRIPT_STRIDE = 18   # position, rotation (column-major), velocity, angular velocity per body and substep
 
 
 SHAPE_PLANE, SHAPE_SPHERE, SHAPE_CUBOID = range(3)
@@ -340,7 +350,32 @@ class Engine:
         arr = (MpmbRigidBody * n_bodies)()
         self._check(self.L.mpmb_get_rigid_state(self.h, C.c_int32(n_bodies), arr))
         return dict(velocity=np.array([list(a.velocity) for a in arr], np.float32), angular_velocity=np.array([list(a.angular_velocity) for a in arr], np.float32),
-                    position=np.array([list(a.position) for a in arr], np.float32))
+                    position=np.array([list(a.position) for a in arr], np.float32),
+                    rotation=np.array([np.reshape(list(a.rot), (3, 3)).T for a in arr], np.float32))
+
+    def set_rigid_motion(self, motion, levelset_collision=False):
+        """Device advection of the bodies (mpmb_set_rigid_motion).  motion: one dict per body, row 0 = the background body
+        (ignored), with mass, inv_inertia_body (3x3, body frame), rotation_axis, linear_damping, angular_damping, restitution,
+        scripted_position, scripted_rotation; missing keys are 0.  An empty list switches device advection off."""
+        nb = len(motion)
+        arr = (MpmbRigidMotion * max(nb, 1))()
+        for b, m in enumerate(motion):
+            arr[b].mass = float(m.get("mass", 0.0))
+            arr[b].inv_inertia_body[:] = [float(v) for v in np.asarray(m.get("inv_inertia_body", np.zeros((3, 3))), np.float64).T.reshape(9)]
+            arr[b].rotation_axis[:] = [float(v) for v in m.get("rotation_axis", (0.0, 0.0, 0.0))]
+            arr[b].linear_damping = float(m.get("linear_damping", 0.0))
+            arr[b].angular_damping = float(m.get("angular_damping", 0.0))
+            arr[b].restitution = float(m.get("restitution", 0.0))
+            arr[b].scripted_position = int(bool(m.get("scripted_position", False)))
+            arr[b].scripted_rotation = int(bool(m.get("scripted_rotation", False)))
+        self._check(self.L.mpmb_set_rigid_motion(self.h, C.c_int32(nb), arr, C.c_int32(int(bool(levelset_collision)))))
+
+    def set_rigid_script(self, poses):
+        """poses[n_substeps][n_bodies][18] (float64): position, rotation (3x3 flattened column-major), velocity, angular
+        velocity at the end of each substep; only the scripted parts are read."""
+        poses = np.ascontiguousarray(poses, np.float64)
+        n = poses.shape[0] if poses.ndim == 3 else 0
+        self._check(self.L.mpmb_set_rigid_script(self.h, C.c_int32(n), _ptr(poses)))
 
     def set_particle_states(self, states):
         st = np.ascontiguousarray(states, np.uint32)

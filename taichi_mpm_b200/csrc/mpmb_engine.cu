@@ -394,9 +394,33 @@ __global__ void k_fill_u32(uint32_t *a, int n, uint32_t v) {
   if (i < n) a[i] = v;
 }
 
-// delete_particles_inside_level_set (src/mpm.cpp:959-973): phi at X = x / dx, trilinear in the node phi (clamped to
-// [0, nnode - 1 - 1e-9], node values capped at 1e20), in double as LevelSet.sample in mpm.py computes it.  A live row
-// with phi < 0 gets the dead key (the next ordering drops it); the killed rows are counted into cnt->n_live.
+// LevelSet.sample (mpm.py): phi at X (grid units), trilinear in the node phi (X clamped to [0, nnode - 1 - 1e-9], node
+// values capped at 1e20), in double
+__device__ __forceinline__ double sdf_phi_trilinear(const float4 *sdf4, const Params &P, const double Xg[3]) {
+  int i0[3];
+  double f[3];
+#pragma unroll
+  for (int a = 0; a < 3; a++) {
+    const double X = fmin(fmax(Xg[a], 0.0), (double)(P.nnode[a] - 1) - 1e-9);
+    i0[a] = (int)floor(X);
+    f[a] = X - (double)i0[a];
+  }
+  double phi = 0.0;
+#pragma unroll
+  for (int a = 0; a < 2; a++)
+#pragma unroll
+    for (int b = 0; b < 2; b++)
+#pragma unroll
+      for (int c = 0; c < 2; c++) {
+        const double w = (a ? f[0] : 1.0 - f[0]) * (b ? f[1] : 1.0 - f[1]) * (c ? f[2] : 1.0 - f[2]);
+        const float s = sdf4[((size_t)(i0[0] + a) * P.nnode[1] + (i0[1] + b)) * P.nnode[2] + (i0[2] + c)].w;
+        phi += w * (double)fminf(s, 1e20f);
+      }
+  return phi;
+}
+
+// delete_particles_inside_level_set (src/mpm.cpp:959-973): phi at X = x / dx (sdf_phi_trilinear).  A live row with phi < 0
+// gets the dead key (the next ordering drops it); the killed rows are counted into cnt->n_live.
 __global__ void __launch_bounds__(256) k_delete_inside(View V, Params P, int n, uint32_t special_min, uint32_t key_dead) {
   typedef cub::BlockReduce<int, 256> Red;
   __shared__ typename Red::TempStorage tmp;
@@ -404,26 +428,8 @@ __global__ void __launch_bounds__(256) k_delete_inside(View V, Params P, int n, 
   int killed = 0;
   if (i < n && V.keys[i] < special_min) {
     const float4 q0 = V.q[0][i];
-    const double xs[3] = {(double)q0.x, (double)q0.y, (double)q0.z};
-    int i0[3];
-    double f[3];
-#pragma unroll
-    for (int a = 0; a < 3; a++) {
-      const double X = fmin(fmax(xs[a] / (double)P.dx, 0.0), (double)(P.nnode[a] - 1) - 1e-9);
-      i0[a] = (int)floor(X);
-      f[a] = X - (double)i0[a];
-    }
-    double phi = 0.0;
-#pragma unroll
-    for (int a = 0; a < 2; a++)
-#pragma unroll
-      for (int b = 0; b < 2; b++)
-#pragma unroll
-        for (int c = 0; c < 2; c++) {
-          const double w = (a ? f[0] : 1.0 - f[0]) * (b ? f[1] : 1.0 - f[1]) * (c ? f[2] : 1.0 - f[2]);
-          const float s = V.sdf4[((size_t)(i0[0] + a) * P.nnode[1] + (i0[1] + b)) * P.nnode[2] + (i0[2] + c)].w;
-          phi += w * (double)fminf(s, 1e20f);
-        }
+    const double X[3] = {(double)q0.x / (double)P.dx, (double)q0.y / (double)P.dx, (double)q0.z / (double)P.dx};
+    const double phi = sdf_phi_trilinear(V.sdf4, P, X);
     if (phi < 0.0) {
       V.keys[i] = key_dead;
       killed = 1;
@@ -1355,9 +1361,11 @@ __global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4
 // Replaces, for scenes with rigid bodies: update_rigid_page_map (src/mpm.cpp:1026-1076), rasterize_rigid_boundary and
 // gather_cdf (src/rigid_transfer.cpp:18-113, 120-274) and the block_op_rigid branches of rasterize_optimized /
 // resample_optimized (src/transfer.cpp:367-463, 706-835).  The rigid bodies themselves (RigidBody, its integrator, the
-// rigid-rigid solver, articulation) belong to the reference's un-vendored core and stay on the host: the engine takes poses and
-// velocities (mpmb_set_rigid_state), applies the impulses of both transfers as apply_tmp_impulse / apply_tmp_velocity would
-// (assumptions stated in include/mpmb.h) and hands the velocities back (mpmb_get_rigid_state).
+// rigid-rigid solver, articulation) belong to the reference's un-vendored core.  By default the host advances them: the engine
+// takes poses and velocities (mpmb_set_rigid_state), applies the impulses of both transfers as apply_tmp_impulse /
+// apply_tmp_velocity would (assumptions stated in include/mpmb.h) and hands the velocities back (mpmb_get_rigid_state).  With
+// mpmb_set_rigid_motion the engine advances scripted and free bodies itself (k_rigid_contacts, k_rigid_advance below); the
+// rigid-rigid solver and articulation are not built.
 // Layout: RigidBoundaryParticles are NOT MPM particles here but a sample list (anchor offset + untransformed triangle + body);
 // node colour data is two dense node arrays (a 64-bit key (distance bits, body) taken with atomicMin, the tags with atomicOr),
 // cleared sample by sample; particle colour state is kept by particle id.  Tiles whose 4x4x8 page is a rigid page are
@@ -1388,7 +1396,7 @@ struct RigidView {
   float4 *p_cdf;                   // (boundary_normal, boundary_distance) of this substep
   uint32_t *p_mark;                // (epoch << 1) | near_boundary_: p_cdf / near of a particle count only if its mark carries THIS substep's
                                    // epoch — gather_cdf then touches only the particles of rigid pages (no 8 M scattered zero-writes)
-  uint32_t epoch;
+  uint32_t *epoch;                 // device word, advanced by k_cdf_clear once per substep (a graph replays it correctly)
   uint32_t id_base;
   int id_cap;
   float penalty, pushing_force;
@@ -1443,9 +1451,13 @@ __device__ __forceinline__ float3 friction_project_rel(float3 v, float3 base, fl
 }
 __device__ __forceinline__ int pack_base(int bx, int by, int bz) { return (bx << 20) | (by << 10) | bz; }   // node coordinates < 1024
 
-// nodes of the previous rasterisation back to "no boundary"
+// nodes of the previous rasterisation back to "no boundary"; thread 0 opens the substep's epoch (0 is never current)
 __global__ void k_cdf_clear(RigidView R, Params P) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s == 0) {
+    uint32_t e = (*R.epoch + 1u) & 0x7fffffffu;
+    *R.epoch = e == 0u ? 1u : e;
+  }
   if (s >= R.n_samples) return;
   const int pb = R.s_base[s];
   if (pb < 0) return;
@@ -1542,8 +1554,9 @@ __global__ void __launch_bounds__(128) k_gather_cdf(View V, Params P, RigidView 
   }
   const uint32_t id = (__float_as_uint(V.q[6][row].w) & TAG_ID_MASK) - R.id_base;
   if (id >= (uint32_t)R.id_cap) { atomicOr(&V.cnt->error, DEVERR_BAD_INPUT); return; }
+  const uint32_t epoch = *R.epoch;
   R.p_cdf[id] = make_float4(0.f, 0.f, 0.f, 0.f);
-  R.p_mark[id] = R.epoch << 1;
+  R.p_mark[id] = epoch << 1;
   int bx, by, bz;
   float rx, ry, rz;
   base_rel(q0.x, P.inv_dx, bx, rx);
@@ -1614,7 +1627,7 @@ __global__ void __launch_bounds__(128) k_gather_cdf(View V, Params P, RigidView 
     }
     float sol[4];
     for (int r = 3; r >= 0; r--) { float sum = A[r][4]; for (int c = r + 1; c < 4; c++) sum -= A[r][c] * sol[c]; sol[r] = sum / A[r][r]; }
-    R.p_mark[id] = (R.epoch << 1) | 1u;
+    R.p_mark[id] = (epoch << 1) | 1u;
     const float l2 = sol[0] * sol[0] + sol[1] * sol[1] + sol[2] * sol[2];
     float4 o = make_float4(0.f, 0.f, 0.f, sol[3] * P.dx);
     if (l2 > 1e-4f) { const float il = 1.0f / sqrtf(l2); o.x = sol[0] * il; o.y = sol[1] * il; o.z = sol[2] * il; }
@@ -1638,6 +1651,7 @@ __global__ void __launch_bounds__(128) k_p2g_rigid(View V, Params P, RigidView R
   __shared__ float s_acc[RIGID_MAX][6];
   const int tid = threadIdx.x;
   const int n_tiles = V.cnt->n_tiles;
+  const uint32_t epoch = *R.epoch;
     for (int slot = blockIdx.x; slot < n_tiles; slot += gridDim.x) {
     if (!R.tile_flag[slot]) continue;
     const TileMeta tm = V.meta[slot];
@@ -1662,7 +1676,7 @@ __global__ void __launch_bounds__(128) k_p2g_rigid(View V, Params P, RigidView R
       const float mass = fabsf(a0.w);
       const uint32_t id = (__float_as_uint(V.q[6][row].w) & TAG_ID_MASK) - R.id_base;
       const uint32_t pst = id < (uint32_t)R.id_cap ? R.p_states[id] : 0u;
-      const bool fresh = id < (uint32_t)R.id_cap && (R.p_mark[id] >> 1) == R.epoch;   // gather_cdf saw this particle in this substep
+      const bool fresh = id < (uint32_t)R.id_cap && (R.p_mark[id] >> 1) == epoch;   // gather_cdf saw this particle in this substep
       const float4 pc = fresh ? R.p_cdf[id] : make_float4(0.f, 0.f, 0.f, 0.f);
       float3 v = make_float3(a1.x, a1.y, a1.z);
       if (P.particle_gravity) { v.x += P.gdt[0]; v.y += P.gdt[1]; v.z += P.gdt[2]; }
@@ -1733,6 +1747,168 @@ __global__ void k_rigid_apply(RigidView R) {
   for (int k = 0; k < 6; k++) B.acc[k] = 0.f;
 }
 
+// Bodies advanced on the device (mpmb_set_rigid_motion): advect_rigid_bodies (src/mpm_rigid_body.cpp:273-287) and
+// rigid_body_levelset_collision (:347-384) with the arithmetic of HostRigidBody.advect / levelset_collision
+// (taichi_mpm_b200/rigid.py) step for step, in fp64 on a master state per body; RigidDev gets the fp32 copy the transfers read.
+struct RigidMaster {
+  double pos[3], rot[9], vel[3], ang[3];   // rot column-major
+  double mass, inv_mass, inv_inertia_body[9], axis[3], lin_damp, ang_damp, restitution;
+  int scripted_pos, scripted_rot;
+};
+constexpr int SCRIPT_STRIDE = 18;          // script entry of one body: position, rotation, velocity, angular velocity
+constexpr int CONTACT_STRIDE = 7;          // contact of one boundary sample: world position, phi, unit gradient of phi
+struct MotionView {
+  RigidMaster *m;                          // [RIGID_MAX]
+  const double *script;                    // [entry][n_bodies][SCRIPT_STRIDE]
+  int *cursor;                             // next script entry (device word: replayed graphs advance it)
+  const int *s_order;                      // sample indices grouped by body, in sample order within a body
+  int s_begin[RIGID_MAX + 1];              // body b owns s_order[s_begin[b] .. s_begin[b + 1])
+  double *contact;                         // [sample][CONTACT_STRIDE]: world position, phi, unit gradient of phi
+  int collide;                             // the level-set collision runs in this substep (asked for and a level set is set)
+};
+
+__device__ __forceinline__ bool motion_collides(const RigidMaster &B) {   // levelset_collision skips fully scripted bodies
+  if (B.inv_mass != 0.0) return true;
+  for (int k = 0; k < 9; k++) if (B.inv_inertia_body[k] != 0.0) return true;
+  return false;
+}
+// R * A * R^T, all column-major
+__device__ __forceinline__ void rot_conj(const double *R, const double *A, double *out) {
+  double T[9];
+  for (int c = 0; c < 3; c++)
+    for (int r = 0; r < 3; r++) T[c * 3 + r] = R[r] * A[c * 3] + R[3 + r] * A[c * 3 + 1] + R[6 + r] * A[c * 3 + 2];
+  for (int c = 0; c < 3; c++)
+    for (int r = 0; r < 3; r++) out[c * 3 + r] = T[r] * R[c] + T[3 + r] * R[3 + c] + T[6 + r] * R[6 + c];
+}
+__device__ __forceinline__ void mat3_vec(const double *M, const double *v, double *out) {
+  for (int r = 0; r < 3; r++) out[r] = M[r] * v[0] + M[3 + r] * v[1] + M[6 + r] * v[2];
+}
+__device__ __forceinline__ void cross3(const double *a, const double *b, double *out) {
+  out[0] = a[1] * b[2] - a[2] * b[1]; out[1] = a[2] * b[0] - a[0] * b[2]; out[2] = a[0] * b[1] - a[1] * b[0];
+}
+__device__ __forceinline__ double dot3(const double *a, const double *b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+__device__ __forceinline__ void enforce_axis(RigidMaster &B) {   // enforce_angular_velocity_parallel_to
+  if (fmax(fabs(B.axis[0]), fmax(fabs(B.axis[1]), fabs(B.axis[2]))) > 0.1) {
+    const double l = sqrt(dot3(B.axis, B.axis));
+    const double a[3] = {B.axis[0] / l, B.axis[1] / l, B.axis[2] / l};
+    const double p = dot3(a, B.ang);
+    for (int k = 0; k < 3; k++) B.ang[k] = a[k] * p;
+  }
+}
+
+// phi and its normalised central-difference gradient (eps = 0.25 grid units) at every boundary sample of a colliding body
+__global__ void k_rigid_contacts(RigidView R, MotionView M, Params P, const float4 *sdf4) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= R.n_samples) return;
+  const RigidMaster &B = M.m[R.s_rigid[s]];
+  if (!motion_collides(B)) return;
+  const float *o = R.s_offset + 3 * s;
+  double *c = M.contact + CONTACT_STRIDE * (size_t)s;
+  double X[3];
+  for (int r = 0; r < 3; r++) {
+    c[r] = B.pos[r] + (B.rot[r] * (double)o[0] + B.rot[3 + r] * (double)o[1] + B.rot[6 + r] * (double)o[2]);
+    X[r] = c[r] / (double)P.dx;
+  }
+  c[3] = sdf_phi_trilinear(sdf4, P, X);
+  const double eps = 0.25;
+  double g[3];
+  for (int a = 0; a < 3; a++) {
+    double Xp[3] = {X[0], X[1], X[2]}, Xm[3] = {X[0], X[1], X[2]};
+    Xp[a] += eps;
+    Xm[a] -= eps;
+    g[a] = (sdf_phi_trilinear(sdf4, P, Xp) - sdf_phi_trilinear(sdf4, P, Xm)) / (2 * eps);
+  }
+  const double n = fmax(sqrt(dot3(g, g)), 1e-12);
+  for (int a = 0; a < 3; a++) c[4 + a] = g[a] / n;
+}
+
+// one thread per body: the level-set impulses in sample order (the reference's loop is order dependent), then the advance
+__global__ void k_rigid_advance(RigidView R, MotionView M, Params P, float3 gravity) {
+  const int b = threadIdx.x;
+  const int entry = *M.cursor;
+  __syncthreads();
+  if (b == 0) *M.cursor = entry + 1;
+  if (b < 1 || b >= R.n_bodies) return;   // body 0 is the background body
+  RigidMaster &B = M.m[b];
+  RigidDev &D = R.bodies[b];
+  const double dt = (double)P.dt;
+  for (int k = 0; k < 3; k++) { B.vel[k] = (double)D.vel[k]; B.ang[k] = (double)D.ang[k]; }   // what the transfers left
+  if (M.collide && motion_collides(B)) {
+    double Iw[9];
+    rot_conj(B.rot, B.inv_inertia_body, Iw);
+    const double f0 = (double)D.fric[0];
+    auto contribution = [&](const double *r0, const double *n) {   // 1/m + n . ((I^-1 (r0 x n)) x r0)
+      double t[3], u[3], w[3];
+      cross3(r0, n, t); mat3_vec(Iw, t, u); cross3(u, r0, w);
+      return B.inv_mass + dot3(n, w);
+    };
+    auto velocity_at = [&](const double *r0, double *v) { double t[3]; cross3(B.ang, r0, t); for (int k = 0; k < 3; k++) v[k] = B.vel[k] + t[k]; };
+    auto apply_impulse = [&](const double *j, const double *r0) {
+      double t[3], u[3];
+      cross3(r0, j, t); mat3_vec(Iw, t, u);
+      for (int k = 0; k < 3; k++) { B.vel[k] += B.inv_mass * j[k]; B.ang[k] += u[k]; }
+    };
+    for (int i = M.s_begin[b]; i < M.s_begin[b + 1]; i++) {
+      const double *c = M.contact + CONTACT_STRIDE * (size_t)M.s_order[i];
+      if (!(c[3] < 0.0)) continue;
+      const double r0[3] = {c[0] - B.pos[0], c[1] - B.pos[1], c[2] - B.pos[2]};
+      const double *g = c + 4;
+      double v[3];
+      velocity_at(r0, v);
+      const double J = -((1.0 + B.restitution) * dot3(g, v)) / contribution(r0, g);
+      if (J < 0.0) continue;
+      const double jn[3] = {J * g[0], J * g[1], J * g[2]};
+      apply_impulse(jn, r0);
+      velocity_at(r0, v);
+      const double vn = dot3(g, v);
+      double tao[3] = {v[0] - g[0] * vn, v[1] - g[1] * vn, v[2] - g[2] * vn};
+      if (fmax(fabs(tao[0]), fmax(fabs(tao[1]), fabs(tao[2]))) > 1e-7) {
+        const double l = sqrt(dot3(tao, tao));
+        for (int k = 0; k < 3; k++) tao[k] /= l;
+        const double j = fmin(fmax(-dot3(v, tao) / contribution(r0, tao), -f0 * J), f0 * J);
+        const double jt[3] = {j * tao[0], j * tao[1], j * tao[2]};
+        apply_impulse(jt, r0);
+      }
+    }
+  }
+  enforce_axis(B);
+  const double *T = M.script ? M.script + ((size_t)entry * R.n_bodies + b) * SCRIPT_STRIDE : nullptr;
+  if (B.scripted_pos) {
+    for (int k = 0; k < 3; k++) { B.pos[k] = T[k]; B.vel[k] = T[12 + k]; }
+  } else {
+    const double d = exp(-B.lin_damp * dt);
+    for (int k = 0; k < 3; k++) { B.vel[k] *= d; B.pos[k] = B.pos[k] + B.vel[k] * dt; }
+  }
+  if (B.scripted_rot) {
+    for (int k = 0; k < 9; k++) B.rot[k] = T[3 + k];
+    for (int k = 0; k < 3; k++) B.ang[k] = T[15 + k];
+  } else {
+    const double d = exp(-B.ang_damp * dt);
+    for (int k = 0; k < 3; k++) B.ang[k] *= d;
+    const double w[3] = {B.ang[0] * dt, B.ang[1] * dt, B.ang[2] * dt};
+    const double a = sqrt(dot3(w, w));
+    if (a >= 1e-12) {   // exponential map: I + sin(a) K + (1 - cos(a)) K^2, K = [w / a]x
+      const double k0 = w[0] / a, k1 = w[1] / a, k2 = w[2] / a;
+      const double K[9] = {0, k2, -k1, -k2, 0, k0, k1, -k0, 0};   // column-major
+      double K2[9], E[9], Rn[9];
+      for (int c = 0; c < 3; c++)
+        for (int r = 0; r < 3; r++) K2[c * 3 + r] = K[r] * K[c * 3] + K[3 + r] * K[c * 3 + 1] + K[6 + r] * K[c * 3 + 2];
+      const double sa = sin(a), ca = 1.0 - cos(a);
+      for (int k = 0; k < 9; k++) E[k] = (k % 4 == 0 ? 1.0 : 0.0) + sa * K[k] + ca * K2[k];
+      for (int c = 0; c < 3; c++)
+        for (int r = 0; r < 3; r++) Rn[c * 3 + r] = E[r] * B.rot[c * 3] + E[3 + r] * B.rot[c * 3 + 1] + E[6 + r] * B.rot[c * 3 + 2];
+      for (int k = 0; k < 9; k++) B.rot[k] = Rn[k];
+    }
+  }
+  const double gv[3] = {(double)gravity.x, (double)gravity.y, (double)gravity.z};
+  for (int k = 0; k < 3; k++) B.vel[k] = B.vel[k] + gv[k] * (B.mass * dt) * B.inv_mass;   // apply_impulse(g m dt, position)
+  enforce_axis(B);
+  double Iw[9];
+  rot_conj(B.rot, B.inv_inertia_body, Iw);
+  for (int k = 0; k < 3; k++) { D.pos[k] = (float)B.pos[k]; D.vel[k] = (float)B.vel[k]; D.ang[k] = (float)B.ang[k]; }
+  for (int k = 0; k < 9; k++) { D.rot[k] = (float)B.rot[k]; D.inv_inertia[k] = (float)Iw[k]; }
+}
+
 // block_op_rigid of resample_optimized (src/transfer.cpp:706-835) + what k_g2p does for the ordering (output rows, keys,
 // movers, stay counts), for the tiles of rigid pages.  Launched BEFORE k_g2p, which commits the substep.
 __global__ void __launch_bounds__(128) k_g2p_rigid(View V, Params P, RigidView R, const float4 *vel) {
@@ -1743,6 +1919,7 @@ __global__ void __launch_bounds__(128) k_g2p_rigid(View V, Params P, RigidView R
   const int tid = threadIdx.x;
   const int n_tiles = V.cnt->n_tiles;
   const float scale = -4.0f * P.inv_dx * P.dt;
+  const uint32_t epoch = *R.epoch;
   for (int slot = blockIdx.x; slot < n_tiles; slot += gridDim.x) {
     if (!R.tile_flag[slot]) continue;
     const TileMeta tm = V.meta[slot];
@@ -1770,7 +1947,7 @@ __global__ void __launch_bounds__(128) k_g2p_rigid(View V, Params P, RigidView R
       const bool known = id < (uint32_t)R.id_cap;
       const uint32_t pst = known ? R.p_states[id] : 0u;
       const uint32_t mark = known ? R.p_mark[id] : 0u;
-      const bool fresh = known && (mark >> 1) == R.epoch;   // gather_cdf saw this particle in this substep
+      const bool fresh = known && (mark >> 1) == epoch;   // gather_cdf saw this particle in this substep
       const float4 pc = fresh ? R.p_cdf[id] : make_float4(0.f, 0.f, 0.f, 0.f);
       const bool near = fresh && (mark & 1u);
       const float3 bn = make_float3(pc.x, pc.y, pc.z);
@@ -2273,6 +2450,17 @@ struct MpmbEngine {
   float *rs_offset = nullptr, *rs_tri = nullptr;
   int *rs_rigid = nullptr;
   size_t rigid_nodes = 0;
+  // bodies advanced on the device (mpmb_set_rigid_motion): master states, script table, contacts
+  bool motion_on = false;
+  bool motion_scripted = false;        // some body follows the script table
+  bool motion_collide = false;         // the level-set collision was asked for (it runs while a level set is set)
+  MotionView M{};
+  RigidMaster h_master[RIGID_MAX] = {};  // host image: motion parameters (+ the state last written by the host)
+  double *script = nullptr;
+  size_t script_cap = 0;               // doubles
+  int64_t script_left = 0;             // entries not yet consumed (host-side count of the device cursor)
+  int *s_order = nullptr;
+  double *contact = nullptr;
   int64_t id_span_pending = 0;
   int64_t id_span = 0;   // ids of the resident particles lie in [id_base, id_base + id_span): uploads number 0..n-1, the seeded
                          // lattice numbers by lattice index (gaps where the boundary band is skipped)
@@ -2562,6 +2750,7 @@ int mpmb_destroy(MpmbHandle h) {
   if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
   cudaFree(h->R.bodies); cudaFree(h->rs_offset); cudaFree(h->rs_tri); cudaFree(h->rs_rigid); cudaFree(h->R.s_base); cudaFree(h->R.node_key);
   cudaFree(h->R.node_tags); cudaFree(h->R.page); cudaFree(h->R.tile_flag); cudaFree(h->R.p_states); cudaFree(h->R.p_cdf); cudaFree(h->R.p_mark);
+  cudaFree(h->R.epoch); cudaFree(h->M.m); cudaFree(h->M.cursor); cudaFree(h->s_order); cudaFree(h->contact); cudaFree(h->script);
 
   delete h;
   return MPMB_OK;
@@ -2638,6 +2827,7 @@ int mpmb_set_delta_t(MpmbHandle h, float dt) {
 int mpmb_set_id_base(MpmbHandle h, int64_t base) {
   CHECK_HANDLE(h);
   if (base < 0 || base >= (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_INVALID, "id base %lld outside [0, 2^%d)", (long long)base, TAG_ID_BITS);
+  if ((uint32_t)base != h->id_base) graph_reset(h);   // the captured rigid kernels take id_base by value
   h->id_base = (uint32_t)base;
   return MPMB_OK;
 }
@@ -3221,6 +3411,7 @@ static int rigid_reserve_ids(MpmbEngine *h, int64_t n_ids) {
   cudaFree(h->R.p_states); cudaFree(h->R.p_cdf); cudaFree(h->R.p_mark);
   h->R.p_states = st; h->R.p_cdf = cdf; h->R.p_mark = nr;
   h->R.id_cap = (int)cap;
+  graph_reset(h);   // the captured rigid kernels hold the freed arrays and the old id_cap
   return MPMB_OK;
 }
 
@@ -3229,8 +3420,6 @@ static int rigid_prepare(MpmbEngine *h, const View &V, int *nl) {
   RigidView &R = h->R;
   R.id_base = h->id_base;
   if (!R.p_states || R.id_cap < h->id_span) { int rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap)); if (rc != MPMB_OK) return rc; }
-  R.epoch = (R.epoch + 1u) & 0x7fffffffu;
-  if (R.epoch == 0u) R.epoch = 1u;
   const int ns = R.n_samples, sb = (ns + 127) / 128;
   k_cdf_clear<<<sb, 128, 0, h->stream>>>(R, h->P);
   CUDA_TRY(h, cudaMemsetAsync(R.page, 0, (size_t)R.nb[0] * R.nb[1] * R.nb[2], h->stream));
@@ -3244,7 +3433,7 @@ static int rigid_prepare(MpmbEngine *h, const View &V, int *nl) {
 int mpmb_set_rigid_samples(MpmbHandle h, int32_t n_bodies, int64_t n_samples, const float *offset3, const float *tri9, const int32_t *rigid_id) {
   CHECK_HANDLE(h);
   if (h->cfg.world > 1) return fail(h, MPMB_ERR_STATE, "rigid coupling is implemented for single-GPU engines (world == 1)");
-  if (n_samples == 0) { h->rigid_on = false; graph_reset(h); return MPMB_OK; }
+  if (n_samples == 0) { h->rigid_on = false; h->motion_on = false; graph_reset(h); return MPMB_OK; }
   if (n_bodies < 2 || n_bodies > RIGID_MAX || n_samples < 0 || n_samples > (1 << 24) || !offset3 || !tri9 || !rigid_id)
     return fail(h, MPMB_ERR_INVALID, "need 2..%d bodies (entry 0 is the background body) and their boundary samples", RIGID_MAX);
   if (h->P.nnode[0] > 1023 || h->P.nnode[1] > 1023 || h->P.nnode[2] > 1023) return fail(h, MPMB_ERR_INVALID, "rigid coupling supports grids up to 1022 cells per axis");
@@ -3267,6 +3456,26 @@ int mpmb_set_rigid_samples(MpmbHandle h, int32_t n_bodies, int64_t n_samples, co
   if (!R.bodies) {
     CUDA_TRY(h, cudaMalloc(&R.bodies, sizeof(RigidDev) * RIGID_MAX));
     CUDA_TRY(h, cudaMemsetAsync(R.bodies, 0, sizeof(RigidDev) * RIGID_MAX, h->stream));
+    CUDA_TRY(h, cudaMalloc(&R.epoch, sizeof(uint32_t)));
+    CUDA_TRY(h, cudaMemsetAsync(R.epoch, 0, sizeof(uint32_t), h->stream));
+    CUDA_TRY(h, cudaMalloc(&h->M.m, sizeof(RigidMaster) * RIGID_MAX));
+    CUDA_TRY(h, cudaMalloc(&h->M.cursor, sizeof(int)));
+    CUDA_TRY(h, cudaMemsetAsync(h->M.cursor, 0, sizeof(int), h->stream));
+  }
+  {  // per-body sample lists for the level-set collision (samples need not be grouped by body)
+    std::vector<int> order((size_t)n_samples);
+    int cnt[RIGID_MAX + 1] = {};
+    for (int64_t s = 0; s < n_samples; s++) cnt[rigid_id[s] + 1]++;
+    for (int b = 0; b < RIGID_MAX; b++) cnt[b + 1] += cnt[b];
+    for (int b = 0; b <= RIGID_MAX; b++) h->M.s_begin[b] = cnt[b];
+    for (int64_t s = 0; s < n_samples; s++) order[(size_t)cnt[rigid_id[s]]++] = (int)s;
+    cudaFree(h->s_order); cudaFree(h->contact);   // contacts: allocated by mpmb_set_rigid_motion when the collision is asked for
+    h->s_order = nullptr; h->contact = nullptr;
+    CUDA_TRY(h, cudaMalloc(&h->s_order, sizeof(int) * n_samples));
+    CUDA_TRY(h, cudaMemcpyAsync(h->s_order, order.data(), sizeof(int) * n_samples, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));   // `order` lives on this stack frame
+    h->M.s_order = h->s_order;
+    h->M.contact = h->contact;
   }
   const size_t nn = (size_t)h->P.nnode[0] * h->P.nnode[1] * h->P.nnode[2];
   if (!R.node_key) {
@@ -3283,8 +3492,9 @@ int mpmb_set_rigid_samples(MpmbHandle h, int32_t n_bodies, int64_t n_samples, co
   if (R.pushing_force == 0.f && R.penalty == 0.f) R.pushing_force = 20000.0f;   // src/mpm.cpp:35,40 defaults
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   h->rigid_on = true;
-  // poses change between substeps: the host drives every substep, so mpmb_substep does not replay graphs while bodies are present
-  // (use_graph itself keeps what the configuration asked for: switching the coupling off brings graph replay back)
+  h->motion_on = false;   // motion records describe a set of bodies: mpmb_set_rigid_motion follows the samples
+  // poses change between substeps: unless the device advances the bodies (mpmb_set_rigid_motion) the host drives every substep,
+  // and mpmb_substep does not replay graphs (use_graph itself keeps what the configuration asked for)
   graph_reset(h);
   return MPMB_OK;
 }
@@ -3293,6 +3503,7 @@ int mpmb_set_rigid_coupling(MpmbHandle h, float penalty, float pushing_force) {
   CHECK_HANDLE(h);
   h->R.penalty = penalty;
   h->R.pushing_force = pushing_force;
+  graph_reset(h);   // both are kernel arguments
   return MPMB_OK;
 }
 
@@ -3311,6 +3522,14 @@ int mpmb_set_rigid_state(MpmbHandle h, int32_t n_bodies, const MpmbRigidBody *bo
     d.fric[0] = s.frictions[0]; d.fric[1] = s.frictions[1];
   }
   CUDA_TRY(h, cudaMemcpyAsync(h->R.bodies, dev, sizeof(RigidDev) * RIGID_MAX, cudaMemcpyHostToDevice, h->stream));
+  if (h->motion_on) {   // the master states restart from the given records
+    for (int b = 0; b < n_bodies; b++) {
+      RigidMaster &m = h->h_master[b];
+      for (int k = 0; k < 3; k++) { m.pos[k] = dev[b].pos[k]; m.vel[k] = dev[b].vel[k]; m.ang[k] = dev[b].ang[k]; }
+      for (int k = 0; k < 9; k++) m.rot[k] = dev[b].rot[k];
+    }
+    CUDA_TRY(h, cudaMemcpyAsync(h->M.m, h->h_master, sizeof(RigidMaster) * RIGID_MAX, cudaMemcpyHostToDevice, h->stream));
+  }
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));   // `dev` lives on this stack frame
   return MPMB_OK;
 }
@@ -3334,6 +3553,98 @@ int mpmb_get_rigid_state(MpmbHandle h, int32_t n_bodies, MpmbRigidBody *bodies) 
   return MPMB_OK;
 }
 
+int mpmb_set_rigid_motion(MpmbHandle h, int32_t n_bodies, const MpmbRigidMotion *motion, int32_t levelset_collision) {
+  CHECK_HANDLE(h);
+  if (n_bodies == 0) { h->motion_on = false; graph_reset(h); return MPMB_OK; }
+  if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies: call mpmb_set_rigid_samples first");
+  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "rigid motion changes between substeps, not inside one");
+  if (n_bodies != h->R.n_bodies || !motion) return fail(h, MPMB_ERR_INVALID, "expected %d motion records", h->R.n_bodies);
+  bool scripted = false;
+  for (int b = 1; b < n_bodies; b++) {
+    const MpmbRigidMotion &m = motion[b];
+    bool ok = std::isfinite(m.mass) && std::isfinite(m.linear_damping) && std::isfinite(m.angular_damping) && std::isfinite(m.restitution);
+    for (int k = 0; k < 9; k++) ok = ok && std::isfinite(m.inv_inertia_body[k]);
+    for (int k = 0; k < 3; k++) ok = ok && std::isfinite(m.rotation_axis[k]);
+    if (!ok) return fail(h, MPMB_ERR_INVALID, "motion record of body %d is not finite", b);
+    if (!m.scripted_position && !(m.mass > 0.f)) return fail(h, MPMB_ERR_INVALID, "body %d: a free body needs a positive mass", b);
+    scripted = scripted || m.scripted_position || m.scripted_rotation;
+  }
+  RigidDev dev[RIGID_MAX];   // the master states start from the current records
+  CUDA_TRY(h, cudaMemcpyAsync(dev, h->R.bodies, sizeof(RigidDev) * RIGID_MAX, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  memset(h->h_master, 0, sizeof(h->h_master));
+  for (int b = 1; b < n_bodies; b++) {
+    const MpmbRigidMotion &s = motion[b];
+    RigidMaster &m = h->h_master[b];
+    for (int k = 0; k < 3; k++) { m.pos[k] = dev[b].pos[k]; m.vel[k] = dev[b].vel[k]; m.ang[k] = dev[b].ang[k]; m.axis[k] = s.rotation_axis[k]; }
+    for (int k = 0; k < 9; k++) { m.rot[k] = dev[b].rot[k]; m.inv_inertia_body[k] = s.inv_inertia_body[k]; }
+    m.mass = s.mass;
+    m.inv_mass = s.scripted_position ? 0.0 : 1.0 / (double)s.mass;   // set_infinity_mass (src/mpm_rigid_body.cpp:198-200)
+    m.lin_damp = s.linear_damping; m.ang_damp = s.angular_damping; m.restitution = s.restitution;
+    m.scripted_pos = s.scripted_position != 0;
+    m.scripted_rot = s.scripted_rotation != 0;
+  }
+  CUDA_TRY(h, cudaMemcpyAsync(h->M.m, h->h_master, sizeof(RigidMaster) * RIGID_MAX, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->M.cursor, 0, sizeof(int), h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (levelset_collision && !h->contact) {
+    CUDA_TRY(h, cudaMalloc(&h->contact, sizeof(double) * CONTACT_STRIDE * h->R.n_samples));
+    h->M.contact = h->contact;
+  }
+  h->script_left = 0;
+  h->motion_scripted = scripted;
+  h->motion_collide = levelset_collision != 0;
+  h->motion_on = true;
+  graph_reset(h);
+  return MPMB_OK;
+}
+
+int mpmb_set_rigid_script(MpmbHandle h, int32_t n_substeps, const double *poses) {
+  CHECK_HANDLE(h);
+  if (!h->rigid_on || !h->motion_on) return fail(h, MPMB_ERR_STATE, "no device-advanced bodies: call mpmb_set_rigid_motion first");
+  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "the script changes between substeps, not inside one");
+  if (n_substeps < 0 || (n_substeps > 0 && !poses)) return fail(h, MPMB_ERR_INVALID, "need n_substeps >= 0 and a table");
+  const int nb = h->R.n_bodies;
+  const size_t n = (size_t)n_substeps * nb * SCRIPT_STRIDE;
+  for (int64_t e = 0; e < n_substeps; e++)   // only the scripted parts are read
+    for (int b = 1; b < nb; b++) {
+      const double *p = poses + ((size_t)e * nb + b) * SCRIPT_STRIDE;
+      bool ok = true;
+      if (h->h_master[b].scripted_pos) for (int k : {0, 1, 2, 12, 13, 14}) ok = ok && std::isfinite(p[k]);
+      if (h->h_master[b].scripted_rot) for (int k = 3; k < 12; k++) ok = ok && std::isfinite(p[k]);
+      if (h->h_master[b].scripted_rot) for (int k = 15; k < 18; k++) ok = ok && std::isfinite(p[k]);
+      if (!ok) return fail(h, MPMB_ERR_INVALID, "script entry %lld of body %d is not finite", (long long)e, b);
+    }
+  if (n > h->script_cap) {   // geometric growth: a fixed frame length allocates once (and keeps the captured graphs)
+    const size_t cap = std::max(n, 2 * h->script_cap);
+    cudaFree(h->script);
+    h->script = nullptr;
+    h->script_cap = 0;
+    CUDA_TRY(h, cudaMalloc(&h->script, sizeof(double) * cap));
+    h->script_cap = cap;
+    h->M.script = h->script;
+    graph_reset(h);
+  }
+  if (n) CUDA_TRY(h, cudaMemcpyAsync(h->script, poses, sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->M.cursor, 0, sizeof(int), h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));   // the caller owns `poses`
+  h->script_left = n_substeps;
+  return MPMB_OK;
+}
+
+// after the second apic_b-velocity transfer of a substep: level-set impulses, then the advance (one script entry)
+static void launch_rigid_motion(MpmbEngine *h) {
+  MotionView M = h->M;   // without a level set there are no contacts: the advance must not read the buffer
+  M.collide = h->motion_collide && h->P.has_sdf;   // (changing the level set resets the captured graphs)
+  if (M.collide) {
+    k_rigid_contacts<<<(h->R.n_samples + 127) / 128, 128, 0, h->stream>>>(h->R, M, h->P, h->sdf4);
+    h->launches++;
+  }
+  k_rigid_advance<<<1, 32, 0, h->stream>>>(h->R, M, h->P, make_float3(h->cfg.gravity[0], h->cfg.gravity[1], h->cfg.gravity[2]));
+  h->launches++;
+  if (h->motion_scripted) h->script_left--;
+}
+
 int mpmb_set_particle_states(MpmbHandle h, int64_t n, const uint32_t *states) {
   CHECK_HANDLE(h);
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies");
@@ -3351,12 +3662,14 @@ int mpmb_get_particle_cdf(MpmbHandle h, int64_t n, uint32_t *states, float *norm
   if (n < 0 || n > h->R.id_cap) return fail(h, MPMB_ERR_INVALID, "n exceeds the %d particle ids tracked", h->R.id_cap);
   std::vector<float4> cdf((size_t)n);
   std::vector<uint32_t> mark((size_t)n);
+  uint32_t epoch = 0;
+  CUDA_TRY(h, cudaMemcpyAsync(&epoch, h->R.epoch, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
   if (states) CUDA_TRY(h, cudaMemcpyAsync(states, h->R.p_states, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaMemcpyAsync(mark.data(), h->R.p_mark, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaMemcpyAsync(cdf.data(), h->R.p_cdf, sizeof(float4) * n, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   for (int64_t i = 0; i < n; i++) {   // particles gather_cdf did not see in the last substep: distance 0, normal 0, not near (138-146)
-    const bool fresh = (mark[i] >> 1) == h->R.epoch;
+    const bool fresh = (mark[i] >> 1) == epoch;
     if (normal3) { normal3[3 * i] = fresh ? cdf[i].x : 0.f; normal3[3 * i + 1] = fresh ? cdf[i].y : 0.f; normal3[3 * i + 2] = fresh ? cdf[i].z : 0.f; }
     if (distance) distance[i] = fresh ? cdf[i].w : 0.f;
     if (near_boundary) near_boundary[i] = (fresh && (mark[i] & 1u)) ? 1 : 0;
@@ -3452,6 +3765,8 @@ static void launch_g2p(MpmbEngine *h, const View &V, int part, int commit, bool 
 int mpmb_resample(MpmbHandle h) {
   CHECK_HANDLE(h);
   if (h->stage != 2) return fail(h, MPMB_ERR_STATE, "resample must follow rasterize");
+  const bool motion = h->rigid_on && h->motion_on;
+  if (motion && h->motion_scripted && h->script_left < 1) return fail(h, MPMB_ERR_STATE, "the rigid script has no entry left for this substep");
   View V = make_view(h);
   prof_begin(h, 4);
   if (h->cap > 0) k_grid<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, h->vel, 0);
@@ -3468,6 +3783,7 @@ int mpmb_resample(MpmbHandle h) {
       h->launches += 1;
     }
   }
+  if (motion) launch_rigid_motion(h);                    // advect_rigid_bodies (src/mpm_rigid_body.cpp:273-287)
   h->launches += 2;
   prof_end(h, 1);
   CUDA_TRY(h, cudaGetLastError());
@@ -3551,6 +3867,7 @@ static int graph_capture_pair(MpmbEngine *h, bool peers) {
   cudaStream_t user = h->stream;
   const int64_t l0 = h->launches;
   const int cur0 = h->cur, ord0 = h->ord, mov0 = h->mov, x0 = h->xstep;
+  const int64_t left0 = h->script_left;
   h->stream = h->cap_stream;
   cudaGraph_t g = nullptr;
   cudaError_t e = cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeThreadLocal);
@@ -3567,12 +3884,12 @@ static int graph_capture_pair(MpmbEngine *h, bool peers) {
     cudaGetLastError();
     h->graph_exec[par] = nullptr;
     h->use_graph = false;
-    h->cur = cur0; h->ord = ord0; h->mov = mov0; h->xstep = x0; h->stage = 0; h->launches = l0;   // nothing has run
+    h->cur = cur0; h->ord = ord0; h->mov = mov0; h->xstep = x0; h->stage = 0; h->launches = l0; h->script_left = left0;   // nothing has run
     h->sticky_cuda = false;
     return MPMB_OK;
   }
   h->graph_launches = (int)(h->launches - l0);
-  h->cur = cur0; h->ord = ord0; h->mov = mov0; h->xstep = x0; h->launches = l0;   // the caller's launch accounts for them
+  h->cur = cur0; h->ord = ord0; h->mov = mov0; h->xstep = x0; h->launches = l0; h->script_left = left0;   // the caller's launch accounts for them
   return MPMB_OK;
 }
 
@@ -3581,13 +3898,20 @@ int mpmb_substep(MpmbHandle h, int32_t nsub) {
   const bool peers = peers_connected(h);
   if (h->cfg.world > 1 && !peers) return fail(h, MPMB_ERR_STATE, "z-slab run: connect the peers (mpmb_xchg_connect) or drive the stages and move the buffers yourself");
   int s = 0, rc;
+  if (nsub > 0 && h->rigid_on && h->motion_on && h->motion_scripted && h->script_left < nsub)
+    return fail(h, MPMB_ERR_STATE, "the rigid script has %lld entries left, %d substeps asked", (long long)h->script_left, nsub);
+  // the by-id colour arrays cover every id before any capture: allocating them inside one would end graph replay for good
+  if (nsub > 0 && h->rigid_on && h->cap > 0 && (!h->R.p_states || h->R.id_cap < h->id_span) &&
+      (rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap))) != MPMB_OK)
+    return rc;
   // the first substep after an upload takes the radix-sorted arrival lists (a different ordering launch): never in a graph
   if (h->fresh && nsub > 0) {
     if ((rc = substep_once(h, peers, nsub > 1)) != MPMB_OK) return rc;
     s = 1;
   }
-  // pairs of intermediate substeps through the captured graph; the last substep (it stores apic_b) always runs directly
-  while (h->use_graph && !h->rigid_on && !h->profiling && h->cap > 0 && h->stage == 0 && nsub - s >= 3) {
+  // pairs of intermediate substeps through the captured graph; the last substep (it stores apic_b) always runs directly.
+  // Rigid scenes replay too when the device advances the bodies (their per-substep state lives in device memory).
+  while (h->use_graph && (!h->rigid_on || h->motion_on) && !h->profiling && h->cap > 0 && h->stage == 0 && nsub - s >= 3) {
     const int par = h->cur;
     if (!h->graph_exec[par]) {
       if ((rc = graph_capture_pair(h, peers)) != MPMB_OK) return rc;
@@ -3595,6 +3919,7 @@ int mpmb_substep(MpmbHandle h, int32_t nsub) {
     }
     CUDA_TRY(h, cudaGraphLaunch(h->graph_exec[par], h->stream));
     h->launches += h->graph_launches;
+    if (h->rigid_on && h->motion_on && h->motion_scripted) h->script_left -= 2;
     h->xstep += 2;   // cur / ord / mov flip twice: unchanged
     s += 2;
   }

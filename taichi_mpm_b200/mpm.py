@@ -14,7 +14,7 @@ reference tree by scripts/async/async_mpm.py:17-300) and the `MPM<3>` plugin beh
 
 Everything numerical happens in libmpmb.so (capi.Engine); this file is glue: kwargs -> MpmbConfig,
 registered particle type names -> material groups, level-set planes -> the engine's dense SDF.
-Only the fast path of the reference is mirrored (optimized=True, no rigid bodies, static level set).
+Only the fast path of the reference is mirrored (optimized=True, static level set); rigid bodies are advanced on the device.
 """
 import os
 
@@ -143,6 +143,7 @@ class MPM:
         self.rigid_body_levelset_collision = bool(kwargs.get("rigid_body_levelset_collision", False))   # mpm.cpp:535-538
         self.rigids = []          # HostRigidBody per add_particles(type='rigid'); engine body id = index + 1 (rigids[0] of the
         self._rigid_dirty = False  # reference is the background body, mpm.cpp:72-74)
+        self._rigid_seen = None   # body states at the last read-back (a difference is a user edit, pushed before the next step)
         self.engine = capi.Engine(self.res, self.delta_x, self.base_delta_t, self.gravity, self.particle_gravity,
                                   self.clean_boundary, device=int(kwargs.get("device", 0)), capacity=int(kwargs.get("capacity", 0)))
         self.current_t = np.float32(0.0)
@@ -267,45 +268,51 @@ class MPM:
     def _rigid_records(self):
         return rigid_mod.engine_records(self.rigids, self.delta_x, self.penalty, self.pushing_force)
 
-    def _substeps_with_rigid(self, n):
-        """The reference's substep() with bodies (src/mpm.cpp:452-575): transfers at the current pose, then
-        advect_rigid_bodies — one engine substep per pose."""
+    def _rigid_substeps(self, n):
+        """n substeps of the reference's substep() with bodies (src/mpm.cpp:452-575) in one engine call: the transfers at the
+        current pose, then on the device the level-set collision (if enabled) and advect_rigid_bodies.  Scripted parts follow a
+        table evaluated here in fp64 at the float32 clock sequence of step().  The bodies are uploaded when the set changed and
+        their state only after a user edit (the device keeps an fp64 master state); one read-back per call puts the advanced
+        state into the HostRigidBody objects.  The level-set collision follows the transfers of a substep, where in the reference
+        it sits between the grid normalisation and the boundary condition (src/mpm.cpp:535-538).  Returns the clock after."""
         h = np.float32(self.base_delta_t)
         t = np.float32(self.current_t)
+        if self._rigid_dirty:
+            self.engine.set_rigid(self._rigid_records())            # boundary samples of every body + coupling constants + state
+            self.engine.set_rigid_motion([{}] + [b.motion_record() for b in self.rigids], self.rigid_body_levelset_collision)
+            self._rigid_dirty = False
+        elif self._rigid_edited():
+            self.engine.set_rigid_state(rigid_mod.state_records(self.rigids))
+        clocks = []
         for _ in range(n):
-            rec = self._rigid_records()
-            if self._rigid_dirty:
-                self.engine.set_rigid(rec)            # boundary samples of every body + coupling constants + state
-                self._rigid_dirty = False
-            else:
-                self.engine.set_rigid_state(rec)
-            self.engine.substep(1)
-            rs = self.engine.get_rigid_state(len(self.rigids) + 1)
-            for k, b in enumerate(self.rigids):
-                b.velocity = rs["velocity"][k + 1].astype(np.float64)
-                b.angular_velocity = rs["angular_velocity"][k + 1].astype(np.float64)
-            if self.rigid_body_levelset_collision and getattr(self, "_levelset", None) is not None:
-                # in the reference this sits between the grid normalisation and the boundary condition of the same substep
-                # (src/mpm.cpp:535-538); here the transfers of a substep are one engine call, so it follows them
-                self._rigid_levelset_collision(rec)
-            for b in self.rigids:
-                b.advect(float(t), float(h), self.gravity)
+            clocks.append(float(t) + float(h))                      # HostRigidBody.advect(t, h) evaluates its functions at t + h
             t = np.float32(t + h)
+        scripted = [b.pos_func is not None or b.rot_func is not None for b in self.rigids]
+        table = None
+        if any(scripted):
+            table = np.zeros((n, len(self.rigids) + 1, capi.RIGID_SCRIPT_STRIDE))
+            for k, b in enumerate(self.rigids):
+                if scripted[k]:
+                    table[:, k + 1] = b.script_poses(clocks, float(h))
+            self.engine.set_rigid_script(table)
+        self.engine.substep(n)
+        rs = self.engine.get_rigid_state(len(self.rigids) + 1)
+        for k, b in enumerate(self.rigids):
+            b.velocity = rs["velocity"][k + 1].astype(np.float64)
+            b.angular_velocity = rs["angular_velocity"][k + 1].astype(np.float64)
+            # scripted parts keep the table's fp64 pose (the device holds the same): the next table differences against it
+            b.position = table[-1, k + 1, 0:3].copy() if b.pos_func else rs["position"][k + 1].astype(np.float64)
+            b.rotation = table[-1, k + 1, 3:12].reshape(3, 3).T.copy() if b.rot_func else rs["rotation"][k + 1].astype(np.float64)
+        self._rigid_seen = [(b.position.copy(), b.rotation.copy(), b.velocity.copy(), b.angular_velocity.copy()) for b in self.rigids]
         return t
 
-    def _rigid_levelset_collision(self, rec):
-        ls = self._levelset
-        for k, b in enumerate(self.rigids):
-            sel = rec["sample_rigid"] == k + 1
-            if not sel.any():
-                continue
-            world = b.position + rec["sample_offset"][sel].astype(np.float64) @ b.rotation.T
-            X = world / self.delta_x
-            phi = ls.sample(X)
-            eps = 0.25
-            grad = np.stack([(ls.sample(X + e) - ls.sample(X - e)) / (2 * eps) for e in np.eye(3) * eps], 1)   # get_spatial_gradient
-            nrm = np.linalg.norm(grad, axis=1, keepdims=True)
-            b.levelset_collision(world, phi, grad / np.maximum(nrm, 1e-12))
+    def _rigid_edited(self):
+        """Whether the user changed a body's pose or velocities since the last read-back."""
+        seen = self._rigid_seen
+        if seen is None or len(seen) != len(self.rigids):
+            return True
+        return any(not (np.array_equal(b.position, p) and np.array_equal(b.rotation, r) and np.array_equal(b.velocity, v) and
+                        np.array_equal(b.angular_velocity, w)) for b, (p, r, v, w) in zip(self.rigids, seen))
 
     def _pull_host(self):
         """Host copy of the resident particles (download -> mutate -> upload contract, SURVEY §8b)."""
@@ -330,7 +337,7 @@ class MPM:
     def substep(self):
         self._push()
         if self.rigids:
-            self.current_t = self._substeps_with_rigid(1)
+            self.current_t = self._rigid_substeps(1)
         else:
             self.engine.substep(1)
             self.current_t = np.float32(self.current_t + np.float32(self.base_delta_t))   # src/mpm.cpp:573, float
@@ -356,7 +363,7 @@ class MPM:
             # "Times of particle updating" (src/mpm.cpp:436,449) = particles.size() per substep: the engine sums the
             # particles every ordering bins (exact when particles are deleted inside the frame); see update_counter
             if self.rigids:
-                self._substeps_with_rigid(n)
+                self._rigid_substeps(n)
             else:
                 self.engine.substep(n)
             self.current_t = t

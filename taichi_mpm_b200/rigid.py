@@ -60,6 +60,15 @@ def mass_properties(tris, density, codimensional):
     return float(mass), com, inertia
 
 
+def _incremental_angular_velocity(new, old, dt):
+    """Angular velocity that turns `old` into `new` over dt (axis-angle of the incremental rotation new old^T)."""
+    d = new @ old.T
+    ang = math.acos(max(-1.0, min(1.0, (np.trace(d) - 1) / 2)))
+    axis = np.array([d[2, 1] - d[1, 2], d[0, 2] - d[2, 0], d[1, 0] - d[0, 1]])
+    nrm = np.linalg.norm(axis)
+    return (axis / nrm * ang / dt) if nrm > 1e-12 else np.zeros(3)
+
+
 def _expmap(w):
     """Rotation matrix exp([w]x)."""
     a = float(np.linalg.norm(w))
@@ -141,6 +150,31 @@ class HostRigidBody:
             hits += 1
         return hits
 
+    def motion_record(self):
+        """This body's capi.Engine.set_rigid_motion record (device advection)."""
+        return dict(mass=self.mass, inv_inertia_body=self.inv_inertia_body, rotation_axis=self.rotation_axis, linear_damping=self.linear_damping,
+                    angular_damping=self.angular_damping, restitution=self.restitution, scripted_position=self.pos_func is not None,
+                    scripted_rotation=self.rot_func is not None)
+
+    def script_poses(self, clocks, dt):
+        """Script entries [n, 18] (position, rotation column-major, velocity, angular velocity) of the substeps whose scripted
+        functions are evaluated at `clocks` (each substep's start time + dt), in fp64 as advect computes them: the velocity is the
+        finite difference of positions, the angular velocity that of the incremental rotation.  Free parts are 0; the body is not
+        changed."""
+        out = np.zeros((len(clocks), 18))
+        pos, rot = self.position, self.rotation
+        for k, tc in enumerate(clocks):
+            if self.pos_func:
+                new = np.asarray(self.pos_func(tc), np.float64)
+                out[k, 12:15] = (new - pos) / dt
+                out[k, 0:3] = pos = new
+            if self.rot_func:
+                new = scenes.euler_rotation(self.rot_func(tc))
+                out[k, 15:18] = _incremental_angular_velocity(new, rot, dt)
+                out[k, 3:12] = new.T.reshape(9)
+                rot = new
+        return out
+
     def advect(self, t, dt, gravity):
         """advect_rigid_bodies for this body (src/mpm_rigid_body.cpp:254-267): axis constraint, advance, gravity impulse."""
         self._enforce_axis()
@@ -153,17 +187,29 @@ class HostRigidBody:
             self.position = self.position + self.velocity * dt
         if self.rot_func:
             new = scenes.euler_rotation(self.rot_func(t + dt))
-            d = new @ self.rotation.T                                                          # incremental rotation over dt
-            ang = math.acos(max(-1.0, min(1.0, (np.trace(d) - 1) / 2)))
-            axis = np.array([d[2, 1] - d[1, 2], d[0, 2] - d[2, 0], d[1, 0] - d[0, 1]])
-            nrm = np.linalg.norm(axis)
-            self.angular_velocity = (axis / nrm * ang / dt) if nrm > 1e-12 else np.zeros(3)
+            self.angular_velocity = _incremental_angular_velocity(new, self.rotation, dt)
             self.rotation = new
         else:
             self.angular_velocity *= math.exp(-self.angular_damping * dt)
             self.rotation = _expmap(self.angular_velocity * dt) @ self.rotation
         self.velocity = self.velocity + np.asarray(gravity, np.float64) * (self.mass * dt) * self.inv_mass   # apply_impulse(g m dt, position)
         self._enforce_axis()
+
+
+def state_records(bodies):
+    """The state rows of engine_records without the boundary samples (capi.Engine.set_rigid_state; row 0 = the background body)."""
+    nr = len(bodies) + 1
+    r = dict(position=np.zeros((nr, 3), np.float32), rot=np.tile(np.eye(3, dtype=np.float32).reshape(9), (nr, 1)), velocity=np.zeros((nr, 3), np.float32),
+             angular_velocity=np.zeros((nr, 3), np.float32), inv_mass=np.zeros(nr, np.float32), inv_inertia=np.zeros((nr, 9), np.float32),
+             frictions=np.zeros((nr, 2), np.float32))
+    for k, b in enumerate(bodies):
+        i = k + 1
+        r["position"][i], r["velocity"][i], r["angular_velocity"][i] = b.position, b.velocity, b.angular_velocity
+        r["rot"][i] = np.asarray(b.rotation, np.float32).T.reshape(9)
+        r["inv_mass"][i] = b.inv_mass
+        r["inv_inertia"][i] = np.asarray(b.inv_inertia_world(), np.float32).T.reshape(9)
+        r["frictions"][i] = b.frictions
+    return r
 
 
 def engine_records(bodies, dx, penalty, pushing_force):
