@@ -3,8 +3,9 @@ a finer time level than the rest:
 
     python examples/async_snow.py [steps]
 
-The scheduler (per-block power-of-two time levels, backup pools) is host code; every substep it schedules runs on the device with
-the level's step (mpmb_set_delta_t)."""
+The scheduler (per-block power-of-two time levels, neighbour masks) is host code; the particle and backup pools live on the
+device, and every advance it schedules (gather, pool edits and one substep with the level's step) runs there without moving a
+particle record across the bus."""
 import sys
 
 sys.path.insert(0, __import__("os").path.dirname(__import__("os").path.dirname(__import__("os").path.abspath(__file__))))

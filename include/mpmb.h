@@ -343,6 +343,48 @@ int mpmb_get_particle_cdf(MpmbHandle h, int64_t n, uint32_t *states, float *norm
  * (tags | (rigid id + 1) << 24) and GridState::distance (world units).                                                 */
 int mpmb_download_cdf(MpmbHandle h, uint32_t *node_states, float *node_distance);
 
+/* ------------------------------------------------------------------------------ AsyncMPM pools */
+/* The particle_pool and backup_pool of the reference's AsyncMPM<3> (src/async/async_mpm.h:85-117), kept on the device so that
+ * the block scheduler (host code: levels, neighbour masks, the step loop) moves no particle record across the bus.  A record
+ * is x, v, F, b, mass, vol, scalar, group, id and the linear index of its 4x4x8-node scheduler block,
+ *   base = int(x * inv_dx - 0.5) (fp32, the HOST's inv_dx), block (base_x >> 2, base_y >> 2, base_z >> 3),
+ *   linear (bx * nb1 + by) * nb2 + bz.
+ * Each advance gathers a particle set from the pools and runs one ordinary substep on it (src/async/async_mpm.cpp:256-373):
+ * the engine's resident set is replaced by every advance.  Single-GPU engines without rigid samples, between substeps (else
+ * MPMB_ERR_STATE); every call but mpmb_async_init needs a preceding mpmb_async_init (else MPMB_ERR_STATE).                */
+enum { MPMB_ASYNC_SMALLER = 1, MPMB_ASYNC_EQUAL = 2, MPMB_ASYNC_LARGER = 4, MPMB_ASYNC_SWAP = 8, MPMB_ASYNC_CLEAR = 16 };
+/* nb = scheduler blocks per axis (each in [1, 4096]); inv_dx = the host's float32(1 / dx).  Empties both pools.           */
+int mpmb_async_init(MpmbHandle h, const int32_t nb[3], float inv_dx);
+/* Appends n records to pool `which` (0 particle_pool, 1 backup_pool) in order; their blocks are computed from x.  Every
+ * array is required.  A record whose block lies outside the nb grid: MPMB_ERR_INVALID and the pool is unchanged.         */
+int mpmb_async_add(MpmbHandle h, int32_t which, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
+                   const float *vol, const float *scalar, const int32_t *group, const uint32_t *id);
+/* One pass over the particle pool (the backup pool is not read): the occupied blocks in ascending linear index into block[],
+ * *n_blocks their number (MPMB_ERR_CAPACITY if more than cap).  With with_limits also, per block, min(0.1, allowed_dt) over
+ * its particles starting from 0.1 and max |v|^2 starting from 1e-16 (update_dt_limits, src/async/async_mpm.cpp:100-112);
+ * |v|^2 = (vx vx + vy vy) + vz vz rounded per operation, allowed_dt = MPMParticle::get_allowed_dt of snow, water, sand,
+ * elastic, von_mises and visco; a NaN makes the block's value NaN.  A pool particle of a type without a limit (linear,
+ * jelly) returns MPMB_ERR_INVALID (the reference stops, :112-124).  min_dt / max_v2 may be NULL without limits.          */
+int mpmb_async_block_limits(MpmbHandle h, int32_t with_limits, int64_t cap, int64_t *n_blocks, int32_t *block, float *min_dt, float *max_v2);
+/* AsyncMPM::advance for one time level: flags[nb0 * nb1 * nb2] are the MPMB_ASYNC_* bits of every block, dt the level's step.
+ *  1. gather: pool entries of SMALLER blocks, then pool entries of EQUAL blocks, then backup entries of LARGER blocks, each
+ *     part stably ordered by the block's SPGrid page index; the first copy of every id is kept; gather index k is engine id k;
+ *  2. backup <- backup[not SWAP] ++ pool[SWAP], pool <- pool[not SWAP];
+ *  3. if the set is not empty: the step becomes dt (as mpmb_set_delta_t), the set replaces the resident particles and one
+ *     substep runs; the survivors' blocks are computed from their new x;
+ *  4. backup <- backup[not CLEAR];
+ *  5. in gather order, survivors whose new block is EQUAL are appended to the pool, those whose new block is CLEAR and not
+ *     EQUAL to the backup; the others are dropped.
+ * *n_gathered receives the size of the set (the reference's update_counter increment).  All pool edits are stable.  A
+ * configured capacity below the set: MPMB_ERR_CAPACITY, both pools unchanged.  NULL flags: MPMB_ERR_INVALID.             */
+int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_gathered);
+/* Records in the pools (either pointer may be NULL).                                                                      */
+int mpmb_async_size(MpmbHandle h, int64_t *n_pool, int64_t *n_backup);
+/* Copies pool `which` out in pool order, any array may be NULL; *n_out receives its size (MPMB_ERR_CAPACITY and nothing
+ * written if it exceeds cap).  Synchronises.                                                                              */
+int mpmb_async_download(MpmbHandle h, int32_t which, int64_t cap, int64_t *n_out, uint32_t *id, int32_t *block, float *x, float *v, float *F,
+                        float *b, float *mass, float *vol, float *scalar, int32_t *group);
+
 /* ------------------------------------------------------------------------------ profiling */
 #define MPMB_N_STAGES 5 /* 0 sort+tiles, 1 P2G, 2 G2P, 3 exchange pack/unpack, 4 grid update */
 /* When enabled, CUDA events bracket every stage on the engine's stream.                          */

@@ -3,16 +3,20 @@
 The reference's AsyncMPM<dim> derives from MPM<dim>; per 4x4x8-node block it keeps a time-step level (a power-of-two multiple of
 `unit_delta_t`, from the block's strength and CFL limits), a pool of particle records and a backup pool of frozen copies, and for
 every level whose turn it is it gathers a particle set, sets base_delta_t and calls MPM<dim>::substep().  That substep is the
-engine's; the scheduler around it is restated here with numpy (vectorised over blocks, pools are flat record arrays labelled
-with their block) and drives ONE engine through `mpmb_set_delta_t` + upload / substep / download per advance.  Functional, not
-fast: every advance moves its particle set across the bus (DESIGN.md §8/§9).
+engine's; the scheduler around it (time levels, neighbour masks, the step loop: work per block) is restated here with numpy,
+vectorised over blocks.  The pools (work per particle) live on the device: the engine keeps both as record arrays labelled with
+their block (mpmb_async_*), reduces the pool to per-block limits for update_dt_limits and runs each advance — gather, pool
+edits, the substep — without moving a particle record across the bus (DESIGN.md §8 row 3).  Records added before the first
+step() are staged in `pool` / `backup` and move into the engine then.  An engine without those calls (the CPU suite's
+stand-in) gets the same pools as numpy record arrays here, gathered and uploaded per advance: the reference the device pools
+are tested against bit for bit.
 
 Citations are lines of src/async/async_mpm.cpp unless a file is named.  What cannot be reproduced bit for bit: the reference
 takes 1/sqrt(max |v|^2) with `_mm_rsqrt_ss` (:78-80), a 12-bit hardware approximation; the exact reciprocal square root is used
 here, which can move a block's CFL limit across an integer — and so its level — only when the limit sits within 2e-4 of one."""
 import numpy as np
 
-from . import scenes
+from . import capi, scenes
 from .mpm import MPM
 
 
@@ -76,8 +80,11 @@ class AsyncMPM(MPM):
         self.backup_t = np.zeros(shape, np.int64)
         self.current_t_int = 0
         self.min_delta_t_int = self.max_delta_t_int = 1
-        self.pool = None       # particle_pool: dict of record arrays + "block" [n,3]
+        self.pool = None       # particle_pool: dict of record arrays + "block" [n,3] (host pools, or staged before the first step)
         self.backup = None     # backup_pool
+        self._next_id = 0
+        self._device_pools = hasattr(self.engine, "async_advance")   # the engine keeps the pools (mpmb_async_*)
+        self._on_device = False    # the staged records have moved into the engine's pools (first step)
         self.step_counter = 0
         self._async_updates = 0
 
@@ -110,15 +117,42 @@ class AsyncMPM(MPM):
         h = self._host
         lo = 0 if before is None else before
         rec = {k: np.ascontiguousarray(h[k][lo:]) for k in ("x", "v", "F", "b", "mass", "vol", "ps", "group")}
-        n0 = 0 if self.pool is None else int(self._next_id)
+        n0 = int(self._next_id)
         rec["id"] = np.arange(n0, n0 + len(rec["x"]), dtype=np.int64)
         self._next_id = n0 + len(rec["x"])
         rec["block"] = self._block_of(rec["x"])
-        self.pool = self._cat(self.pool, rec)
-        if self.backup is None:
-            self.backup = self._empty_like(rec)
+        if self._on_device:
+            self.engine.async_add(0, rec)                                  # the engine computes the same blocks from x
+        else:
+            self.pool = self._cat(self.pool, rec)
+            if self.backup is None:
+                self.backup = self._empty_like(rec)
         self._host, self._dirty = None, False                              # this->particles.clear() (:75): the pools own the particles
         return ret
+
+    def _pools_to_device(self):
+        """First step with an engine that keeps the pools: the records staged by add_particles move into them."""
+        if not self._device_pools or self._on_device:
+            return
+        self.engine.async_init(self.nb, np.float32(1.0 / self.delta_x))
+        for which, rec in ((0, self.pool), (1, self.backup)):
+            if rec is not None and len(rec["id"]):
+                self.engine.async_add(which, rec)
+        self.pool = self.backup = None
+        self._on_device = True
+
+    def pools(self):
+        """(particle_pool, backup_pool) as host record dicts in pool order (read from the device pools if the engine keeps them)."""
+        if not self._on_device:
+            return self.pool, self.backup
+        out = []
+        for which in (0, 1):
+            d = self.engine.async_download(which)
+            blk = np.stack(np.unravel_index(d.pop("block"), self.nb), 1).astype(np.int32)
+            d["id"] = d["id"].astype(np.int64)
+            d["block"] = blk
+            out.append(d)
+        return tuple(out)
 
     # ---- update_dt_limits (:90-254)
     def _neighbour_levels(self):
@@ -134,28 +168,61 @@ class AsyncMPM(MPM):
                     if (i, j, k) != (1, 1, 1):
                         yield (i - 1, j - 1, k - 1), pad_l[i:i + nx, j:j + ny, k:k + nz], pad_e[i:i + nx, j:j + ny, k:k + nz]
 
+    def _pool_scan(self, t):
+        """The pass over the particle pool: its occupied blocks, and a function returning per block (flat) min(0.1, allowed_dt)
+        and max |v|^2 (:100-112).  Device pools: one mpmb_async_block_limits call, with the limits whenever some block's level
+        is aligned to the clock (only such a block can be due)."""
+        nblk = int(np.prod(self.nb))
+        if self._on_device:
+            aligned = (t & (self.level - 1)) == 0
+            try:
+                blk, mn, mx = self.engine.async_block_limits(bool(aligned.any()))
+            except capi.MpmbError as e:
+                if e.code != -1:
+                    raise
+                blk, _, _ = self.engine.async_block_limits(False)      # a type without a limit matters only if a block is due
+                if aligned.reshape(-1)[blk].any():
+                    raise ValueError("particle type without a time-step limit (jelly / linear return 0: the reference stops, :112-124)") from e
+                mn = mx = None
+            nonempty = np.zeros(nblk, bool)
+            nonempty[blk] = True
+
+            def limits():
+                min_adt = np.full(nblk, np.float32(0.1))
+                max_v2 = np.full(nblk, np.float32(1e-16))
+                min_adt[blk], max_v2[blk] = mn, mx
+                return min_adt, max_v2
+            return nonempty.reshape(self.nb), limits
+        p = self.pool
+        nonempty = np.zeros(self.nb, bool)
+        if p is None or len(p["id"]) == 0:
+            return nonempty, None
+        blk = p["block"]
+        nonempty[blk[:, 0], blk[:, 1], blk[:, 2]] = True
+
+        def limits():
+            lin = (blk[:, 0] * self.nb[1] + blk[:, 1]) * self.nb[2] + blk[:, 2]
+            adt = np.full(len(lin), 0.1, np.float32)
+            for g, (kind, prm) in enumerate(self._groups):
+                m = p["group"] == g
+                if m.any():
+                    adt[m] = np.minimum(np.float32(0.1), allowed_dt(kind, prm, p["F"][m], p["ps"][m], p["mass"][m], p["vol"][m], p["v"][m], self.delta_x))
+            v2 = (p["v"].astype(np.float32) ** 2).sum(1)
+            min_adt = np.full(nblk, np.float32(0.1))
+            max_v2 = np.full(nblk, np.float32(1e-16))
+            np.minimum.at(min_adt, lin, adt)
+            np.maximum.at(max_v2, lin, v2)
+            return min_adt, max_v2
+        return nonempty, limits
+
     def update_dt_limits(self):
         t = self.current_t_int
         inv_unit = np.float32(1.0) / np.float32(self.unit_delta_t)
-        p = self.pool
-        nonempty = np.zeros(self.nb, bool)
-        if p is not None and len(p["id"]):
-            blk = p["block"]
-            nonempty[blk[:, 0], blk[:, 1], blk[:, 2]] = True
+        nonempty, limits = self._pool_scan(t)
+        if nonempty.any():
             due = nonempty & ((t & (self.level - 1)) == 0)                  # :95-96
             if due.any():
-                lin = (blk[:, 0] * self.nb[1] + blk[:, 1]) * self.nb[2] + blk[:, 2]
-                adt = np.full(len(lin), 0.1, np.float32)
-                for g, (kind, prm) in enumerate(self._groups):
-                    m = p["group"] == g
-                    if m.any():
-                        adt[m] = np.minimum(np.float32(0.1), allowed_dt(kind, prm, p["F"][m], p["ps"][m], p["mass"][m], p["vol"][m], p["v"][m], self.delta_x))
-                v2 = (p["v"].astype(np.float32) ** 2).sum(1)
-                nblk = int(np.prod(self.nb))
-                min_adt = np.full(nblk, np.float32(0.1))
-                max_v2 = np.full(nblk, np.float32(1e-16))
-                np.minimum.at(min_adt, lin, adt)
-                np.maximum.at(max_v2, lin, v2)
+                min_adt, max_v2 = limits()
                 sdl = (np.float32(self.strength_dt_mul) * min_adt * inv_unit).astype(np.int64).reshape(self.nb)          # :110
                 cdl = (np.float32(self.cfl_dt_mul) * np.float32(self.delta_x) * inv_unit * (np.float32(1.0) / np.sqrt(max_v2))).astype(np.int64).reshape(self.nb)   # :111-112
                 tmp = np.minimum(np.minimum(cdl, sdl), self.max_units)
@@ -231,6 +298,24 @@ class AsyncMPM(MPM):
         larger = self._larger.get(lg, np.zeros(self.nb, bool))
         equal = self.level == limit
         has_copied = smaller | larger                                       # :262-268, :300-310
+        swap = equal & (self.particle_t == t)                               # backup_current_dt_limit (:318-326)
+        drop = has_copied & (self.level > limit) & (self.local_min == t + limit)
+        clear_b = drop & ~equal                                             # :331-343
+        dt = float(np.float32(self.unit_delta_t) * np.float32(limit))       # :407-409
+        if self._on_device:
+            flags = (smaller * capi.ASYNC_SMALLER | equal * capi.ASYNC_EQUAL | larger * capi.ASYNC_LARGER | swap * capi.ASYNC_SWAP |
+                     clear_b * capi.ASYNC_CLEAR).astype(np.uint8)
+            n = self.engine.async_advance(flags, dt)                        # gather, pool edits and the substep, on the device
+        else:
+            n = self._advance_host(smaller, equal, larger, swap, clear_b, dt)
+        self._async_updates += n                                            # update_counter += particles.size() (:328)
+        # update backup_t and particle_t (:318-343)
+        self.backup_t = np.where(swap, t, self.backup_t)
+        self.particle_t = np.where(equal, t + limit, self.particle_t)
+        self.backup_t = np.where(clear_b, t + limit, self.backup_t)
+
+    def _advance_host(self, smaller, equal, larger, swap, clear_b, dt):
+        """The pool work of one advance on host pools; returns the size of the gathered set."""
         parts = [self._select(self.pool, smaller), self._select(self.pool, equal), self._select(self.backup, larger)]
         g = None
         for q in parts:                                                     # gather order: smaller neighbours, this level, larger neighbours' backups
@@ -241,7 +326,6 @@ class AsyncMPM(MPM):
             _, first = np.unique(g["id"], return_index=True)
             g = {k: v[np.sort(first)] for k, v in g.items()}
         # backup_current_dt_limit (:318-326): the level's pools become their blocks' backups
-        swap = equal & (self.particle_t == t)
         if self.pool is not None and len(self.pool["id"]):
             pb = self.pool["block"]
             mv = swap[pb[:, 0], pb[:, 1], pb[:, 2]]
@@ -249,12 +333,9 @@ class AsyncMPM(MPM):
             keep_b = ~swap[bb[:, 0], bb[:, 1], bb[:, 2]] if len(bb) else np.zeros(0, bool)
             self.backup = self._cat({k: v[keep_b] for k, v in self.backup.items()}, {k: v[mv] for k, v in self.pool.items()})
             self.pool = {k: v[~mv] for k, v in self.pool.items()}
-        self.backup_t = np.where(swap, t, self.backup_t)
         n = 0 if g is None else len(g["id"])
-        self._async_updates += n                                            # update_counter += particles.size() (:328)
         out = None
         if n:
-            dt = float(np.float32(self.unit_delta_t) * np.float32(limit))   # :407-409
             self.engine.set_delta_t(dt)
             self.engine.upload(g["x"], g["v"], g["mass"], g["vol"], g["F"], g["b"], g["ps"], g["group"].astype(np.int32))
             self.engine.substep(1)                                          # MPM<dim>::substep() (:329)
@@ -262,14 +343,9 @@ class AsyncMPM(MPM):
             k = d["id"].astype(np.int64)                                    # upload index of the survivors
             out = dict(x=d["x"], v=d["v"], F=d["F"], b=d["b"], mass=d["mass"], vol=d["vol"], ps=d["ps"], group=g["group"][k], id=g["id"][k])
             out["block"] = self._block_of(out["x"])
-        # update backup_t and particle_t (:331-343)
-        drop = has_copied & (self.level > limit) & (self.local_min == t + limit)
-        self.particle_t = np.where(equal, t + limit, self.particle_t)
-        clear_b = drop & ~equal
-        if len(self.backup["id"]):
+        if len(self.backup["id"]):                                          # blocks whose backups were consumed (:331-343)
             bb = self.backup["block"]
             self.backup = {k: v[~clear_b[bb[:, 0], bb[:, 1], bb[:, 2]]] for k, v in self.backup.items()}
-        self.backup_t = np.where(clear_b, t + limit, self.backup_t)
         # update backup_pool and particle_pool (:345-370)
         if out is not None and len(out["id"]):
             ob = out["block"]
@@ -277,12 +353,14 @@ class AsyncMPM(MPM):
             to_backup = (~to_pool) & clear_b[ob[:, 0], ob[:, 1], ob[:, 2]]
             self.pool = self._cat(self.pool, {k: v[to_pool] for k, v in out.items()})
             self.backup = self._cat(self.backup, {k: v[to_backup] for k, v in out.items()})
+        return n
 
     # ---- step (:375-421)
     def step(self, dt):
         if dt < 0:
             raise ValueError("AsyncMPM.step needs dt >= 0 here")
         self.request_t = np.float32(self.request_t + np.float32(dt))
+        self._pools_to_device()
         while True:
             self.update_dt_limits()
             delta = self.max_delta_t_int
@@ -307,7 +385,7 @@ class AsyncMPM(MPM):
 
     def get_particles(self):
         """The particles of the pools by id (every live particle's current record is the LAST one a pool received for its id)."""
-        p = self.pool
+        p = self.pools()[0]
         if p is None or len(p["id"]) == 0:
             return {k: np.zeros((0,) + s, np.float32) for k, s in (("x", (3,)), ("v", (3,)), ("F", (9,)), ("b", (9,)), ("mass", ()), ("vol", ()), ("ps", ()))}
         o = np.argsort(self._offset[p["block"][:, 0], p["block"][:, 1], p["block"][:, 2]], kind="stable")
@@ -318,7 +396,8 @@ class AsyncMPM(MPM):
         return {k: v[sel] for k, v in q.items() if k != "block"}
 
     def num_particles(self):
-        return 0 if self.pool is None else len(np.unique(self.pool["id"]))
+        p = self.pool if not self._on_device else self.engine.async_download(0, ("id",))
+        return 0 if p is None else len(np.unique(p["id"]))
 
     def visualize(self):
         """The frame dump of MPM.visualize from the pools (the engine only ever holds the particle set of the last advance)."""
@@ -341,7 +420,7 @@ class AsyncMPM(MPM):
         return super().general_action(**kwargs)
 
     def scheduler_stats(self):
-        p = self.pool
+        p = self.pools()[0]
         ne = np.zeros(self.nb, bool)
         if p is not None and len(p["id"]):
             ne[p["block"][:, 0], p["block"][:, 1], p["block"][:, 2]] = True

@@ -31,7 +31,9 @@ EXPORTS = [
     "mpmb_set_rigid_script", "mpmb_set_particle_states",
     "mpmb_get_particle_cdf", "mpmb_download_cdf",
     "mpmb_xchg_buffer", "mpmb_xchg_ipc_handle", "mpmb_xchg_connect", "mpmb_halo_send", "mpmb_halo_recv", "mpmb_migrate_send", "mpmb_migrate_recv",
+    "mpmb_async_init", "mpmb_async_add", "mpmb_async_block_limits", "mpmb_async_advance", "mpmb_async_size", "mpmb_async_download",
 ]
+ASYNC_SMALLER, ASYNC_EQUAL, ASYNC_LARGER, ASYNC_SWAP, ASYNC_CLEAR = 1, 2, 4, 8, 16   # per-block flags of mpmb_async_advance
 
 
 class MpmbConfig(C.Structure):
@@ -313,6 +315,59 @@ class Engine:
         if sort_by_id:
             o = np.argsort(out["id"], kind="stable")
             out = {k: a[o] for k, a in out.items()}
+        return out
+
+    # --- AsyncMPM pools (mpmb_async_*): which = 0 particle pool, 1 backup pool
+    def async_init(self, nb, inv_dx):
+        """Empties both pools; nb = scheduler blocks per axis, inv_dx = the host's float32(1 / dx)."""
+        self._async_nb = tuple(int(n) for n in nb)
+        self._check(self.L.mpmb_async_init(self.h, (C.c_int32 * 3)(*self._async_nb), C.c_float(float(inv_dx))))
+
+    def async_add(self, which, rec):
+        """Appends records dict(x, v, F, b, mass, vol, ps, group, id) to a pool; their blocks come from x."""
+        x = _f32(rec["x"]).reshape(-1, 3)
+        n = len(x)
+        v, F, b = _f32(rec["v"], (n, 3)), _f32(rec["F"], (n, 9)), _f32(rec["b"], (n, 9))
+        mass, vol, ps = _f32(rec["mass"], (n,)), _f32(rec["vol"], (n,)), _f32(rec["ps"], (n,))
+        group = np.ascontiguousarray(rec["group"], np.int32).reshape(n)
+        ids = np.ascontiguousarray(rec["id"], np.uint32).reshape(n)
+        self._check(self.L.mpmb_async_add(self.h, C.c_int32(which), C.c_int64(n), _ptr(x), _ptr(v), _ptr(F), _ptr(b), _ptr(mass), _ptr(vol),
+                                          _ptr(ps), _ptr(group), _ptr(ids)))
+
+    def async_block_limits(self, with_limits):
+        """Occupied blocks of the particle pool (linear indices, ascending) and, with limits, their min(0.1, allowed_dt) and
+        max |v|^2 (else None): (block, min_dt, max_v2)."""
+        cap = int(np.prod(self._async_nb))
+        blk = np.empty(cap, np.int32)
+        mn = np.empty(cap, np.float32) if with_limits else None
+        mx = np.empty(cap, np.float32) if with_limits else None
+        n = C.c_int64(0)
+        self._check(self.L.mpmb_async_block_limits(self.h, C.c_int32(int(bool(with_limits))), C.c_int64(cap), C.byref(n), _ptr(blk), _ptr(mn), _ptr(mx)))
+        k = n.value
+        return blk[:k], None if mn is None else mn[:k], None if mx is None else mx[:k]
+
+    def async_advance(self, flags, dt):
+        """One AsyncMPM advance; flags = uint8 ASYNC_* bits per block (C order of the block grid).  Returns the gathered count."""
+        fl = np.ascontiguousarray(flags, np.uint8).reshape(-1)
+        assert fl.size == int(np.prod(self._async_nb))
+        n = C.c_int64(0)
+        self._check(self.L.mpmb_async_advance(self.h, _ptr(fl), C.c_float(float(dt)), C.byref(n)))
+        return n.value
+
+    def async_size(self):
+        a, b = C.c_int64(0), C.c_int64(0)
+        self._check(self.L.mpmb_async_size(self.h, C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+    def async_download(self, which, fields=("id", "block", "x", "v", "F", "b", "mass", "vol", "ps", "group")):
+        """A pool in pool order: dict of the asked fields (id uint32, block = linear block index int32)."""
+        n = self.async_size()[which]
+        shape = dict(id=((), np.uint32), block=((), np.int32), x=((3,), np.float32), v=((3,), np.float32), F=((9,), np.float32),
+                     b=((9,), np.float32), mass=((), np.float32), vol=((), np.float32), ps=((), np.float32), group=((), np.int32))
+        out = {k: np.empty((n,) + shape[k][0], shape[k][1]) for k in fields}
+        got = C.c_int64(0)
+        self._check(self.L.mpmb_async_download(self.h, C.c_int32(which), C.c_int64(n), C.byref(got), *[_ptr(out.get(k)) for k in (
+            "id", "block", "x", "v", "F", "b", "mass", "vol", "ps", "group")]))
         return out
 
     # --- hot path

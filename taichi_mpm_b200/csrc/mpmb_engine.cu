@@ -2369,6 +2369,220 @@ __global__ void k_migrate_commit(Counters *c, const int *hdr, int cap, int cap_p
   c->n_movers += n;
 }
 
+// ------------------------------------------------------------------------------ AsyncMPM pools (mpmb_async_*)
+// One pool of AsyncMPM particle records, SoA: x[3n] v[3n] F[9n] b[9n] mass vol scalar group id block (the linear index of
+// the record's 4x4x8-node scheduler block).
+struct ARec {
+  float *x, *v, *F, *b, *mass, *vol, *scalar;
+  int *group;
+  uint32_t *id;
+  int *block;
+};
+constexpr int AREC_WORDS = 30;  // 4-byte words per record
+enum { ASYNC_SMALLER = MPMB_ASYNC_SMALLER, ASYNC_EQUAL = MPMB_ASYNC_EQUAL, ASYNC_LARGER = MPMB_ASYNC_LARGER, ASYNC_SWAP = MPMB_ASYNC_SWAP,
+       ASYNC_CLEAR = MPMB_ASYNC_CLEAR };
+
+__device__ __forceinline__ void arec_copy(const ARec &d, size_t j, const ARec &s, size_t i) {
+#pragma unroll
+  for (int k = 0; k < 3; k++) { d.x[3 * j + k] = s.x[3 * i + k]; d.v[3 * j + k] = s.v[3 * i + k]; }
+#pragma unroll
+  for (int k = 0; k < 9; k++) { d.F[9 * j + k] = s.F[9 * i + k]; d.b[9 * j + k] = s.b[9 * i + k]; }
+  d.mass[j] = s.mass[i]; d.vol[j] = s.vol[i]; d.scalar[j] = s.scalar[i];
+  d.group[j] = s.group[i]; d.id[j] = s.id[i]; d.block[j] = s.block[i];
+}
+
+// The scheduler block of a position, in the host scheduler's fp32 arithmetic with ITS 1/dx: base = int(x * inv_dx - 0.5),
+// block = (base_x >> 2, base_y >> 2, base_z >> 3), linear (bx * nb1 + by) * nb2 + bz.  A block outside the grid counts in *bad.
+__global__ void k_async_blocks(const float *x, int n, float inv_dx, int nb0, int nb1, int nb2, int *block, int *bad) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int c[3];
+#pragma unroll
+  for (int a = 0; a < 3; a++) c[a] = (int)__fsub_rn(__fmul_rn(x[3 * (size_t)i + a], inv_dx), 0.5f);
+  const int bx = c[0] >> 2, by = c[1] >> 2, bz = c[2] >> 3;
+  const bool ok = bx >= 0 && by >= 0 && bz >= 0 && bx < nb0 && by < nb1 && bz < nb2;
+  block[i] = ok ? (bx * nb1 + by) * nb2 + bz : 0;
+  if (!ok) atomicAdd(bad, 1);
+}
+
+// MPMParticle::get_allowed_dt of the registered types (src/particles.cpp:136-153, 254-281, 480-494, 649-668, 734-753,
+// 814-833) in the operation order of async_mpm.allowed_dt: fp32 with explicit rounding (no FMA contraction), the
+// determinant and the transcendental functions in fp64 rounded once.  Types without a limit (linear, jelly) return -1.
+__device__ __forceinline__ float async_allowed_dt(const Material &M, const float *F, float ps, float mass, float vol, float v2, float dx) {
+  const double d = (double)F[0] * ((double)F[4] * F[8] - (double)F[5] * F[7]) - (double)F[1] * ((double)F[3] * F[8] - (double)F[5] * F[6]) +
+                   (double)F[2] * ((double)F[3] * F[7] - (double)F[4] * F[6]);
+  float J = (float)d;
+  const float u = sqrtf(v2);
+  const float rho0 = mass / vol;
+  float c;
+  if (M.kind == MAT_SNOW) {
+    J = __fmul_rn(J, ps);
+    const float hh = (float)exp((double)__fmul_rn(M.p[2], __fsub_rn(1.0f, ps)));
+    const float mu = __fmul_rn(M.p[0], hh), lam = __fmul_rn(M.p[1], hh);
+    c = sqrtf(__fadd_rn(lam, __fmul_rn(2.0f, mu)) / (rho0 / J));
+  } else if (M.kind == MAT_WATER) {
+    c = sqrtf(__fmul_rn(M.p[0], M.p[1]) / (float)pow((double)ps, (double)__fsub_rn(M.p[1], 1.0f)));
+  } else if (M.kind == MAT_SAND || M.kind == MAT_VON_MISES || M.kind == MAT_ELASTIC || M.kind == MAT_VISCO) {
+    const float mu = M.p[0], lam = M.p[1];
+    const float K = __fadd_rn(__fmul_rn(2.0f, mu) / 3.0f, lam);
+    const float c2 = __fadd_rn(__fmul_rn(4.0f, mu) / __fmul_rn(3.0f, rho0 / J), __fmul_rn(K, __fsub_rn(1.0f, (float)log((double)J))) / rho0);
+    c = sqrtf(c2 != c2 ? c2 : fmaxf(c2, 1e-20f));  // np.maximum keeps a NaN
+  } else {
+    return -1.0f;
+  }
+  return dx / __fadd_rn(c, u);
+}
+
+// One pass over the particle pool: per block an occupied bit (1), and with limits min(0.1, allowed_dt) and max |v|^2 as
+// the bits of non-negative floats read as signed integers (ordered like the floats), a NaN as a flag bit (2: the limit,
+// 4: |v|^2).  A type without a limit sets *bad.
+__global__ void __launch_bounds__(256) k_async_limits(ARec R, int n, Params P, int with_limits, uint32_t *bflag, int *bmin, int *bmax, int *bad) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int blk = R.block[i];
+  if (!with_limits) {
+    if (bflag[blk] == 0u) atomicOr(&bflag[blk], 1u);
+    return;
+  }
+  const float vx = R.v[3 * (size_t)i], vy = R.v[3 * (size_t)i + 1], vz = R.v[3 * (size_t)i + 2];
+  const float v2 = __fadd_rn(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy)), __fmul_rn(vz, vz));
+  const int g = min(max(R.group[i], 0), MPMB_MAX_GROUPS - 1);
+  float adt = async_allowed_dt(P.mats[g], R.F + 9 * (size_t)i, R.scalar[i], R.mass[i], R.vol[i], v2, P.dx);
+  if (adt == -1.0f) { atomicAdd(bad, 1); return; }
+  unsigned f = 1u;
+  if (adt != adt) f |= 2u;
+  else atomicMin(&bmin[blk], __float_as_int(fminf(0.1f, adt)));
+  if (v2 != v2) f |= 4u;
+  else atomicMax(&bmax[blk], __float_as_int(v2));
+  atomicOr(&bflag[blk], f);
+}
+
+__global__ void k_async_occupied(const uint32_t *bflag, int nblk, int *flags) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < nblk) flags[i] = (int)(bflag[i] & 1u);
+}
+
+// the occupied blocks in block order, with their limits
+__global__ void k_async_block_out(const uint32_t *bflag, const int *bmin, const int *bmax, int nblk, const int *prefix, int *ob, float *omin,
+                                  float *omax) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nblk || !(bflag[i] & 1u)) return;
+  const int o = prefix[i];
+  ob[o] = i;
+  omin[o] = (bflag[i] & 2u) ? __uint_as_float(0x7fc00000u) : __int_as_float(bmin[i]);
+  omax[o] = (bflag[i] & 4u) ? __uint_as_float(0x7fc00000u) : __int_as_float(bmax[i]);
+}
+
+// candidates of a gather: [0, np) pool entries of SMALLER blocks, [np, 2np) pool entries of EQUAL blocks, [2np, 2np + nbk)
+// backup entries of LARGER blocks
+__device__ __forceinline__ int async_cand_part(int c, int np, int &src) {
+  if (c < np) { src = c; return 0; }
+  if (c < 2 * np) { src = c - np; return 1; }
+  src = c - 2 * np;
+  return 2;
+}
+
+__global__ void k_async_cand_flags(const int *pblock, int np, const int *bblock, int nbk, const uint8_t *bfl, int *flags) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= 2 * np + nbk) return;
+  int s;
+  const int part = async_cand_part(c, np, s);
+  const int want = part == 0 ? ASYNC_SMALLER : part == 1 ? ASYNC_EQUAL : ASYNC_LARGER;
+  flags[c] = (bfl[part == 2 ? bblock[s] : pblock[s]] & want) ? 1 : 0;
+}
+
+// SPGrid's page index of a block (async_mpm._morton): coordinate bits interleaved y, x, z from the least significant
+__device__ __forceinline__ unsigned long long async_morton(int bx, int by, int bz) {
+  unsigned long long m = 0;
+#pragma unroll
+  for (int i = 0; i < 12; i++)
+    m |= ((unsigned long long)((by >> i) & 1) << (3 * i)) | ((unsigned long long)((bx >> i) & 1) << (3 * i + 1)) |
+         ((unsigned long long)((bz >> i) & 1) << (3 * i + 2));
+  return m;
+}
+
+// the flagged candidates in candidate order with the sort key (part, morton of the block)
+__global__ void k_async_cand_keys(const int *pblock, int np, const int *bblock, int nbk, const int *flags, const int *prefix, int nb1, int nb2,
+                                  unsigned long long *key, uint32_t *cand) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= 2 * np + nbk || !flags[c]) return;
+  int s;
+  const int part = async_cand_part(c, np, s);
+  const int blk = part == 2 ? bblock[s] : pblock[s];
+  const int bz = blk % nb2, by = (blk / nb2) % nb1, bx = blk / (nb1 * nb2);
+  const int o = prefix[c];
+  key[o] = ((unsigned long long)part << 36) | async_morton(bx, by, bz);
+  cand[o] = (uint32_t)c;
+}
+
+__global__ void k_async_cand_ids(const uint32_t *cand, int nc, const uint32_t *pid, int np, const uint32_t *bid, uint32_t *ids, uint32_t *pos) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= nc) return;
+  int s;
+  const int part = async_cand_part((int)cand[k], np, s);
+  ids[k] = part == 2 ? bid[s] : pid[s];
+  pos[k] = (uint32_t)k;
+}
+
+// sorted by id (stable: ascending gather position within an id): the first entry of every id is the copy that is kept
+__global__ void k_async_first(const uint32_t *ids_sorted, const uint32_t *pos_sorted, int nc, int *keep) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < nc) keep[pos_sorted[j]] = (j == 0 || ids_sorted[j] != ids_sorted[j - 1]) ? 1 : 0;
+}
+
+__global__ void k_async_gather(const uint32_t *cand, int nc, const int *keep, const int *prefix, ARec Pp, int np, ARec Bp, ARec G) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= nc || !keep[k]) return;
+  int s;
+  const int part = async_cand_part((int)cand[k], np, s);
+  arec_copy(G, (size_t)prefix[k], part == 2 ? Bp : Pp, (size_t)s);
+}
+
+__global__ void k_async_rec_flags(const int *block, int n, const uint8_t *bfl, int bit, int *flags) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) flags[i] = (bfl[block[i]] & bit) ? 1 : 0;
+}
+
+// stable partition: flagged records to dA[offA + rank among the flagged], the others to dB[offB + rank among the others];
+// a side whose has* is 0 is dropped
+__global__ void k_async_split(ARec src, int n, const int *flags, const int *prefix, ARec dA, int offA, int hasA, ARec dB, int offB, int hasB) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (flags[i]) {
+    if (hasA) arec_copy(dA, (size_t)offA + prefix[i], src, (size_t)i);
+  } else if (hasB) {
+    arec_copy(dB, (size_t)offB + (i - prefix[i]), src, (size_t)i);
+  }
+}
+
+// survivors of a substep: row of every gather index (-1: deleted)
+__global__ void k_async_rank(const uint32_t *sid, int ns, int *rowk) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < ns) rowk[sid[r]] = r;
+}
+
+// in gather order: survivors whose new block is EQUAL (to_backup = 0), or CLEAR and not EQUAL (to_backup = 1)
+__global__ void k_async_route_flags(const int *rowk, int ng, const int *sblock, const uint8_t *bfl, int to_backup, int *flags) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= ng) return;
+  const int r = rowk[k];
+  int f = 0;
+  if (r >= 0) {
+    const uint8_t b = bfl[sblock[r]];
+    f = to_backup ? (!(b & ASYNC_EQUAL) && (b & ASYNC_CLEAR)) : ((b & ASYNC_EQUAL) != 0);
+  }
+  flags[k] = f;
+}
+
+// the survivor of gather index k appended to a pool, with the particle id of its gathered record (the engine numbered it k)
+__global__ void k_async_route(const int *rowk, int ng, const int *flags, const int *prefix, ARec S, const uint32_t *gid, ARec D, int off) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= ng || !flags[k]) return;
+  const size_t o = (size_t)off + prefix[k];
+  arec_copy(D, o, S, (size_t)rowk[k]);
+  D.id[o] = gid[k];
+}
+
 }  // namespace mpmb
 
 // =====================================================================================
@@ -2465,6 +2679,34 @@ struct MpmbEngine {
   int64_t id_span = 0;   // ids of the resident particles lie in [id_base, id_base + id_span): uploads number 0..n-1, the seeded
                          // lattice numbers by lattice index (gaps where the boundary band is skipped)
 
+  // AsyncMPM pools (mpmb_async_*): [0] particle_pool, [1] backup_pool, each double-buffered for the stable edits
+  struct APool {
+    void *buf[2] = {};
+    ARec r[2] = {};
+    int cur = 0;
+    int64_t n = 0, cap = 0;
+  };
+  bool async_on = false;
+  int anb[3] = {};
+  int nblk = 0;
+  float a_inv_dx = 0.f;
+  APool apool[2];
+  uint8_t *a_bfl = nullptr;                                         // [nblk] MPMB_ASYNC_* flags of the current advance
+  uint32_t *a_bflag = nullptr;                                      // [nblk] block reductions of mpmb_async_block_limits
+  int *a_bmin = nullptr, *a_bmax = nullptr;
+  int *a_blk = nullptr;                                             // [nblk] compacted block list
+  float *a_lim = nullptr;                                           // [2 nblk] compacted min_dt, max_v2
+  int *a_bad = nullptr;
+  void *a_gbuf = nullptr, *a_sbuf = nullptr;                        // gathered set / survivors (record layout)
+  ARec a_G{}, a_S{};
+  int64_t a_gcap = 0, a_scap = 0;
+  unsigned long long *a_key[2] = {};                                // gather: candidate keys, candidate / id / position lists
+  uint32_t *a_u[4] = {};
+  int *a_rowk = nullptr;
+  int64_t a_ccap = 0;
+  void *a_cub = nullptr;
+  size_t a_cub_bytes = 0;
+
   bool profiling = false;
   struct Ev { cudaEvent_t a, b; int stage; };
   std::vector<Ev> events;
@@ -2474,6 +2716,32 @@ struct MpmbEngine {
 };
 
 static thread_local std::string g_create_error;
+
+// fields of `cap` records laid out one after another in one allocation of AREC_WORDS * cap words
+static ARec arec_layout(void *buf, int64_t cap) {
+  float *w = (float *)buf;
+  const size_t c = (size_t)cap;
+  ARec r;
+  r.x = w; r.v = w + 3 * c; r.F = w + 6 * c; r.b = w + 15 * c; r.mass = w + 24 * c; r.vol = w + 25 * c; r.scalar = w + 26 * c;
+  r.group = (int *)(w + 27 * c); r.id = (uint32_t *)(w + 28 * c); r.block = (int *)(w + 29 * c);
+  return r;
+}
+
+static void async_free(MpmbEngine *h) {
+  for (auto &p : h->apool) {
+    for (int b = 0; b < 2; b++) { cudaFree(p.buf[b]); p.buf[b] = nullptr; }
+    p.n = p.cap = 0;
+    p.cur = 0;
+  }
+  cudaFree(h->a_bfl); cudaFree(h->a_bflag); cudaFree(h->a_bmin); cudaFree(h->a_bmax); cudaFree(h->a_blk); cudaFree(h->a_lim); cudaFree(h->a_bad);
+  cudaFree(h->a_gbuf); cudaFree(h->a_sbuf); cudaFree(h->a_key[0]); cudaFree(h->a_key[1]); cudaFree(h->a_rowk); cudaFree(h->a_cub);
+  for (auto &u : h->a_u) { cudaFree(u); u = nullptr; }
+  h->a_bfl = nullptr; h->a_bflag = nullptr; h->a_bmin = h->a_bmax = nullptr; h->a_blk = nullptr; h->a_lim = nullptr; h->a_bad = nullptr;
+  h->a_gbuf = h->a_sbuf = nullptr; h->a_key[0] = h->a_key[1] = nullptr; h->a_rowk = nullptr; h->a_cub = nullptr;
+  h->a_gcap = h->a_scap = h->a_ccap = 0;
+  h->a_cub_bytes = 0;
+  h->async_on = false;
+}
 
 static int fail(MpmbEngine *h, int code, const char *fmt, ...) {
   char buf[512];
@@ -2751,6 +3019,7 @@ int mpmb_destroy(MpmbHandle h) {
   cudaFree(h->R.bodies); cudaFree(h->rs_offset); cudaFree(h->rs_tri); cudaFree(h->rs_rigid); cudaFree(h->R.s_base); cudaFree(h->R.node_key);
   cudaFree(h->R.node_tags); cudaFree(h->R.page); cudaFree(h->R.tile_flag); cudaFree(h->R.p_states); cudaFree(h->R.p_cdf); cudaFree(h->R.p_mark);
   cudaFree(h->R.epoch); cudaFree(h->M.m); cudaFree(h->M.cursor); cudaFree(h->s_order); cudaFree(h->contact); cudaFree(h->script);
+  async_free(h);
 
   delete h;
   return MPMB_OK;
@@ -2798,15 +3067,21 @@ int mpmb_set_material(MpmbHandle h, int32_t group, int32_t kind, const float *pa
   return MPMB_OK;
 }
 
-int mpmb_set_delta_t(MpmbHandle h, float dt) {
-  CHECK_HANDLE(h);
-  if (!(dt > 0.f) || !std::isfinite(dt)) return fail(h, MPMB_ERR_INVALID, "delta_t must be positive and finite");
-  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "delta_t changes between substeps, not inside one");
-  if (dt == h->P.dt) return MPMB_OK;
+// the step of the following substeps (dt and the gravity kick it scales); returns whether it changed
+static bool apply_delta_t(MpmbEngine *h, float dt) {
+  if (dt == h->P.dt) return false;
   h->cfg.dt = dt;
   h->P.dt = dt;
   for (int d = 0; d < 3; d++) h->P.gdt[d] = h->cfg.gravity[d] * dt;
   graph_reset(h);
+  return true;
+}
+
+int mpmb_set_delta_t(MpmbHandle h, float dt) {
+  CHECK_HANDLE(h);
+  if (!(dt > 0.f) || !std::isfinite(dt)) return fail(h, MPMB_ERR_INVALID, "delta_t must be positive and finite");
+  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "delta_t changes between substeps, not inside one");
+  if (!apply_delta_t(h, dt)) return MPMB_OK;
   // resident particles: the affine matrix cached for the next rasterize carries the old dt (stress * (-4 dt / dx))
   if (h->cap > 0) {
     int ns = 0;
@@ -2962,6 +3237,19 @@ static int finish_upload(MpmbEngine *h, int64_t n) {
   return reorder_from_scratch(h, n);
 }
 
+// Packs n field-wise particles held in DEVICE arrays into rows row0.. with ids id0.. of the current storage (F, b, scalar,
+// group may be NULL).  The one packing path of uploads, appends and AsyncMPM advances.
+static int pack_rows(MpmbEngine *h, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
+                     const float *vol, const float *scalar, const int *group, int row0, uint32_t id0) {
+  View V = make_view(h);
+  k_pack_particles<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, x, v, F, b, mass, vol, scalar, group, h->keys[h->cur], row0, id0);
+  h->launches++;
+  cudaError_t e = cudaStreamSynchronize(h->stream);
+  CUDA_TRY(h, e);
+  CUDA_TRY(h, cudaGetLastError());
+  return MPMB_OK;
+}
+
 // Stages n field-wise particles on the device and packs them into rows row0.. with ids id0.. of the current storage.
 static int pack_fields(MpmbEngine *h, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
                        const float *vol, const float *scalar, const int32_t *group, int row0, uint32_t id0) {
@@ -2987,13 +3275,7 @@ static int pack_fields(MpmbEngine *h, int64_t n, const float *x, const float *v,
   float *dx_ = put(x, 3 * n), *dv = put(v, 3 * n), *dF = put(F, 9 * n), *db = put(b, 9 * n), *dm = put(mass, n), *dvol = put(vol, n),
         *ds = put(scalar, n);
   int *dg = (int *)put(group, n);
-  View V = make_view(h);
-  k_pack_particles<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, dx_, dv, dF, db, dm, dvol, ds, dg, h->keys[h->cur], row0, id0);
-  h->launches++;
-  cudaError_t e = cudaStreamSynchronize(h->stream);
-  CUDA_TRY(h, e);
-  CUDA_TRY(h, cudaGetLastError());
-  return MPMB_OK;
+  return pack_rows(h, n, dx_, dv, dF, db, dm, dvol, ds, dg, row0, id0);
 }
 
 int mpmb_upload_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
@@ -3248,6 +3530,24 @@ int mpmb_get_update_count(MpmbHandle h, int64_t *updates) {
   return MPMB_OK;
 }
 
+// The live rows among the n rows of the current storage: alive flags and their exclusive prefix (scan_a / scan_b), *alive
+// their number.  Followed by unpack_live: the one unpacking path of downloads and AsyncMPM advances.
+static int live_prefix(MpmbEngine *h, int n, int64_t *alive) {
+  int rc, total = 0;
+  if ((rc = scan_reserve(h, (size_t)n)) != MPMB_OK) return rc;
+  k_alive_flags<<<(n + 255) / 256, 256, 0, h->stream>>>(h->keys[h->cur], n, h->special_min, h->scan_a);
+  if ((rc = scan_flags(h, (size_t)n, &total)) != MPMB_OK) return rc;
+  *alive = total;
+  return MPMB_OK;
+}
+
+// The live rows, compacted in storage order, into DEVICE arrays (any may be NULL); id = the engine's particle id.
+static void unpack_live(MpmbEngine *h, int n, uint32_t *id, float *x, float *v, float *F, float *b, float *mass, float *vol, float *scalar, int *group) {
+  View V = make_view(h);
+  k_unpack_particles<<<(n + 127) / 128, 128, 0, h->stream>>>(V, h->keys[h->cur], n, h->special_min, id, x, v, F, b, mass, vol, scalar, group, h->scan_b);
+  h->launches += 2;
+}
+
 int mpmb_download_particles(MpmbHandle h, int64_t cap, int64_t *n_out, uint32_t *id, float *x, float *v, float *F, float *b,
                             float *mass, float *vol, float *scalar, int32_t *group) {
   CHECK_HANDLE(h);
@@ -3258,25 +3558,9 @@ int mpmb_download_particles(MpmbHandle h, int64_t cap, int64_t *n_out, uint32_t 
   if ((rc = read_n_store(h, &n)) != MPMB_OK) return rc;
   *n_out = 0;
   if (n == 0 || h->cap == 0) return MPMB_OK;
-  // exclusive prefix of the alive flags (CUB scan)
-  int *flags = nullptr, *prefix = nullptr;
-  CUDA_TRY(h, cudaMalloc(&flags, sizeof(int) * n));
-  CUDA_TRY(h, cudaMalloc(&prefix, sizeof(int) * (n + 1)));
-  k_alive_flags<<<(n + 255) / 256, 256, 0, h->stream>>>(h->keys[h->cur], n, h->special_min, flags);
-  void *tmp = nullptr;
-  size_t tmp_bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flags, prefix, n, h->stream);
-  CUDA_TRY(h, cudaMalloc(&tmp, tmp_bytes));
-  cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flags, prefix, n, h->stream);
-  int last_flag = 0, last_prefix = 0;
-  CUDA_TRY(h, cudaMemcpyAsync(&last_flag, flags + n - 1, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(&last_prefix, prefix + n - 1, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  const int64_t alive = (int64_t)last_flag + last_prefix;
-  if (alive > cap) {
-    cudaFree(flags); cudaFree(prefix); cudaFree(tmp);
-    return fail(h, MPMB_ERR_CAPACITY, "%lld live particles do not fit in the %lld rows provided", (long long)alive, (long long)cap);
-  }
+  int64_t alive = 0;
+  if ((rc = live_prefix(h, n, &alive)) != MPMB_OK) return rc;
+  if (alive > cap) return fail(h, MPMB_ERR_CAPACITY, "%lld live particles do not fit in the %lld rows provided", (long long)alive, (long long)cap);
   size_t fl = (size_t)alive * ((x ? 3 : 0) + (v ? 3 : 0) + (F ? 9 : 0) + (b ? 9 : 0) + (mass ? 1 : 0) + (vol ? 1 : 0) + (scalar ? 1 : 0) +
                                (id ? 1 : 0) + (group ? 1 : 0));
   float *stage = nullptr;
@@ -3298,16 +3582,13 @@ int mpmb_download_particles(MpmbHandle h, int64_t cap, int64_t *n_out, uint32_t 
   float *dx_ = take(x, 3), *dv = take(v, 3), *dF = take(F, 9), *db = take(b, 9), *dm = take(mass, 1), *dvol = take(vol, 1), *ds = take(scalar, 1);
   uint32_t *did = (uint32_t *)take(id, 1);
   int *dg = (int *)take(group, 1);
-  View V = make_view(h);
-  k_unpack_particles<<<(n + 127) / 128, 128, 0, h->stream>>>(V, h->keys[h->cur], n, h->special_min, did, dx_, dv, dF, db, dm, dvol, ds, dg, prefix);
-  h->launches += 2;
+  unpack_live(h, n, did, dx_, dv, dF, db, dm, dvol, ds, dg);
   auto get = [&](void *dst, const void *src, size_t per) {
     if (dst) cudaMemcpyAsync(dst, src, per * alive * sizeof(float), cudaMemcpyDeviceToHost, h->stream);
   };
   get(x, dx_, 3); get(v, dv, 3); get(F, dF, 9); get(b, db, 9); get(mass, dm, 1); get(vol, dvol, 1); get(scalar, ds, 1);
   get(id, did, 1); get(group, dg, 1);
   cudaError_t e = cudaStreamSynchronize(h->stream);
-  cudaFree(flags); cudaFree(prefix); cudaFree(tmp);
   CUDA_TRY(h, e);
   CUDA_TRY(h, cudaGetLastError());
   *n_out = alive;
@@ -4262,6 +4543,344 @@ int mpmb_migrate_recv(MpmbHandle h, int32_t face) {
   if (h->cfg.world <= 1 || face < 0 || face > 1 || !h->tx[1][face]) return fail(h, MPMB_ERR_STATE, "no connected peer through face %d", face);
   if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "migrate_recv must follow resample");
   return xchg_migrate_launch(h, 0, 1 << face);
+}
+
+}  // extern "C"
+
+// =====================================================================================
+// AsyncMPM pools (mpmb_async_*, SURVEY §8f row 3): the particle records live on the device, the scheduler on the host
+// =====================================================================================
+static int async_check(MpmbEngine *h, bool need_init) {
+  if (need_init && !h->async_on) return fail(h, MPMB_ERR_STATE, "mpmb_async_init has not been called");
+  if (h->cfg.world > 1) return fail(h, MPMB_ERR_STATE, "AsyncMPM pools are implemented for single-GPU engines (world == 1)");
+  if (h->rigid_on) return fail(h, MPMB_ERR_STATE, "AsyncMPM pools do not support rigid bodies");
+  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "AsyncMPM pools are edited between substeps, not inside one");
+  return MPMB_OK;
+}
+
+// room for `need` records in both buffers of a pool, keeping the current records (grows by at least half, as
+// grow_keeping_rows does for the resident set)
+static int apool_reserve(MpmbEngine *h, MpmbEngine::APool &p, int64_t need) {
+  if (need <= p.cap) return MPMB_OK;
+  const int64_t want = std::max<int64_t>(need, p.cap + p.cap / 2);
+  void *nb[2] = {};
+  for (int b = 0; b < 2; b++) {
+    cudaError_t e = cudaMalloc(&nb[b], sizeof(float) * AREC_WORDS * (size_t)want);
+    if (e != cudaSuccess) {
+      cudaFree(nb[0]);
+      h->sticky_cuda = true;
+      return fail(h, MPMB_ERR_CUDA, "cudaMalloc of an AsyncMPM pool failed: %s", cudaGetErrorString(e));
+    }
+  }
+  ARec n0 = arec_layout(nb[0], want);
+  const ARec &o = p.r[p.cur];
+  const size_t n = (size_t)p.n;
+  if (n > 0) {
+    const struct { void *d; const void *s; size_t w; } cp[] = {{n0.x, o.x, 3}, {n0.v, o.v, 3}, {n0.F, o.F, 9}, {n0.b, o.b, 9}, {n0.mass, o.mass, 1},
+                                                              {n0.vol, o.vol, 1}, {n0.scalar, o.scalar, 1}, {n0.group, o.group, 1}, {n0.id, o.id, 1},
+                                                              {n0.block, o.block, 1}};
+    for (const auto &c : cp) CUDA_TRY(h, cudaMemcpyAsync(c.d, c.s, 4 * c.w * n, cudaMemcpyDeviceToDevice, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  for (int b = 0; b < 2; b++) cudaFree(p.buf[b]);
+  p.buf[0] = nb[0];
+  p.buf[1] = nb[1];
+  p.r[0] = n0;
+  p.r[1] = arec_layout(nb[1], want);
+  p.cur = 0;
+  p.cap = want;
+  return MPMB_OK;
+}
+
+static unsigned nblocks(int64_t n) { return (unsigned)((n + 255) / 256); }
+
+// pool <- pool[records of blocks without `bit`]; with `to` the others are appended to that pool, in order.  Stable.
+static int apool_split(MpmbEngine *h, MpmbEngine::APool &p, int bit, MpmbEngine::APool *to) {
+  const int n = (int)p.n;
+  if (n == 0) return MPMB_OK;
+  int rc, moved = 0;
+  if ((rc = scan_reserve(h, (size_t)n)) != MPMB_OK) return rc;
+  k_async_rec_flags<<<nblocks(n), 256, 0, h->stream>>>(p.r[p.cur].block, n, h->a_bfl, bit, h->scan_a);
+  h->launches++;
+  if ((rc = scan_flags(h, (size_t)n, &moved)) != MPMB_OK) return rc;
+  if (moved == 0) return MPMB_OK;
+  if (to && (rc = apool_reserve(h, *to, to->n + moved)) != MPMB_OK) return rc;
+  k_async_split<<<nblocks(n), 256, 0, h->stream>>>(p.r[p.cur], n, h->scan_a, h->scan_b, to ? to->r[to->cur] : ARec{}, to ? (int)to->n : 0, to ? 1 : 0,
+                                                    p.r[p.cur ^ 1], 0, 1);
+  h->launches++;
+  CUDA_TRY(h, cudaGetLastError());
+  p.cur ^= 1;
+  p.n = n - moved;
+  if (to) to->n += moved;
+  return MPMB_OK;
+}
+
+extern "C" {
+
+int mpmb_async_init(MpmbHandle h, const int32_t nb[3], float inv_dx) {
+  CHECK_HANDLE(h);
+  int rc = async_check(h, false);
+  if (rc != MPMB_OK) return rc;
+  if (!nb) return fail(h, MPMB_ERR_INVALID, "null argument");
+  for (int d = 0; d < 3; d++)
+    if (nb[d] < 1 || nb[d] > 4096) return fail(h, MPMB_ERR_INVALID, "nb[%d] = %d outside [1, 4096]", d, nb[d]);
+  if (!(inv_dx > 0.f) || !std::isfinite(inv_dx)) return fail(h, MPMB_ERR_INVALID, "inv_dx must be positive and finite");
+  const int64_t nblk = (int64_t)nb[0] * nb[1] * nb[2];
+  if (nblk >= (1ll << 30)) return fail(h, MPMB_ERR_INVALID, "too many scheduler blocks");
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  async_free(h);
+  for (int d = 0; d < 3; d++) h->anb[d] = nb[d];
+  h->nblk = (int)nblk;
+  h->a_inv_dx = inv_dx;
+  CUDA_TRY(h, cudaMalloc(&h->a_bfl, (size_t)nblk));
+  CUDA_TRY(h, cudaMalloc(&h->a_bflag, sizeof(uint32_t) * nblk));
+  CUDA_TRY(h, cudaMalloc(&h->a_bmin, sizeof(int) * nblk));
+  CUDA_TRY(h, cudaMalloc(&h->a_bmax, sizeof(int) * nblk));
+  CUDA_TRY(h, cudaMalloc(&h->a_blk, sizeof(int) * nblk));
+  CUDA_TRY(h, cudaMalloc(&h->a_lim, sizeof(float) * 2 * nblk));
+  CUDA_TRY(h, cudaMalloc(&h->a_bad, sizeof(int)));
+  for (auto &p : h->apool)
+    if ((rc = apool_reserve(h, p, 1024)) != MPMB_OK) return rc;
+  h->async_on = true;
+  return MPMB_OK;
+}
+
+int mpmb_async_add(MpmbHandle h, int32_t which, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
+                   const float *vol, const float *scalar, const int32_t *group, const uint32_t *id) {
+  CHECK_HANDLE(h);
+  int rc = async_check(h, true);
+  if (rc != MPMB_OK) return rc;
+  if (which < 0 || which > 1) return fail(h, MPMB_ERR_INVALID, "which = %d: 0 (particle pool) or 1 (backup pool)", which);
+  if (n < 0 || (n > 0 && (!x || !v || !F || !b || !mass || !vol || !scalar || !group || !id))) return fail(h, MPMB_ERR_INVALID, "every field is required");
+  if (n == 0) return MPMB_OK;
+  MpmbEngine::APool &p = h->apool[which];
+  if (p.n + n >= (1ll << 30)) return fail(h, MPMB_ERR_CAPACITY, "an AsyncMPM pool holds fewer than 2^30 records");
+  if ((rc = apool_reserve(h, p, p.n + n)) != MPMB_OK) return rc;
+  const ARec &r = p.r[p.cur];
+  const size_t o = (size_t)p.n;
+  const struct { void *d; const void *s; size_t w; } cp[] = {{r.x + 3 * o, x, 3}, {r.v + 3 * o, v, 3}, {r.F + 9 * o, F, 9}, {r.b + 9 * o, b, 9},
+                                                            {r.mass + o, mass, 1}, {r.vol + o, vol, 1}, {r.scalar + o, scalar, 1}, {r.group + o, group, 1},
+                                                            {r.id + o, id, 1}};
+  for (const auto &c : cp) CUDA_TRY(h, cudaMemcpyAsync(c.d, c.s, 4 * c.w * (size_t)n, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->a_bad, 0, sizeof(int), h->stream));
+  k_async_blocks<<<nblocks(n), 256, 0, h->stream>>>(r.x + 3 * o, (int)n, h->a_inv_dx, h->anb[0], h->anb[1], h->anb[2], r.block + o, h->a_bad);
+  h->launches++;
+  int bad = 0;
+  CUDA_TRY(h, cudaMemcpyAsync(&bad, h->a_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  if (bad) return fail(h, MPMB_ERR_INVALID, "%d records lie outside the %d x %d x %d scheduler blocks", bad, h->anb[0], h->anb[1], h->anb[2]);
+  p.n += n;
+  return MPMB_OK;
+}
+
+int mpmb_async_block_limits(MpmbHandle h, int32_t with_limits, int64_t cap, int64_t *n_blocks, int32_t *block, float *min_dt, float *max_v2) {
+  CHECK_HANDLE(h);
+  int rc = async_check(h, true);
+  if (rc != MPMB_OK) return rc;
+  if (!n_blocks || (cap > 0 && !block) || (with_limits && cap > 0 && (!min_dt || !max_v2))) return fail(h, MPMB_ERR_INVALID, "null argument");
+  *n_blocks = 0;
+  const int nblk = h->nblk;
+  const MpmbEngine::APool &p = h->apool[0];
+  CUDA_TRY(h, cudaMemsetAsync(h->a_bflag, 0, sizeof(uint32_t) * nblk, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->a_bad, 0, sizeof(int), h->stream));
+  if (with_limits) {
+    k_fill_u32<<<nblocks(nblk), 256, 0, h->stream>>>((uint32_t *)h->a_bmin, nblk, 0x3dcccccdu);   // 0.1f
+    k_fill_u32<<<nblocks(nblk), 256, 0, h->stream>>>((uint32_t *)h->a_bmax, nblk, 0x2539705fu);   // 1e-16f
+    h->launches += 2;
+  }
+  if (p.n > 0) {
+    k_async_limits<<<nblocks(p.n), 256, 0, h->stream>>>(p.r[p.cur], (int)p.n, h->P, with_limits ? 1 : 0, h->a_bflag, h->a_bmin, h->a_bmax, h->a_bad);
+    h->launches++;
+  }
+  int bad = 0, total = 0;
+  CUDA_TRY(h, cudaMemcpyAsync(&bad, h->a_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if ((rc = scan_reserve(h, (size_t)nblk)) != MPMB_OK) return rc;
+  k_async_occupied<<<nblocks(nblk), 256, 0, h->stream>>>(h->a_bflag, nblk, h->scan_a);
+  h->launches++;
+  if ((rc = scan_flags(h, (size_t)nblk, &total)) != MPMB_OK) return rc;
+  if (bad) return fail(h, MPMB_ERR_INVALID, "%d pool particles are of a type without a time-step limit (linear / jelly)", bad);
+  *n_blocks = total;
+  if (total > cap) return fail(h, MPMB_ERR_CAPACITY, "%d occupied blocks do not fit in the %lld entries provided", total, (long long)cap);
+  if (total == 0) return MPMB_OK;
+  float *dmin = h->a_lim, *dmax = h->a_lim + nblk;
+  k_async_block_out<<<nblocks(nblk), 256, 0, h->stream>>>(h->a_bflag, h->a_bmin, h->a_bmax, nblk, h->scan_b, h->a_blk, dmin, dmax);
+  h->launches++;
+  CUDA_TRY(h, cudaMemcpyAsync(block, h->a_blk, sizeof(int) * total, cudaMemcpyDeviceToHost, h->stream));
+  if (with_limits) {
+    CUDA_TRY(h, cudaMemcpyAsync(min_dt, dmin, sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(max_v2, dmax, sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
+  }
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  return MPMB_OK;
+}
+
+int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_gathered) {
+  CHECK_HANDLE(h);
+  int rc = async_check(h, true);
+  if (rc != MPMB_OK) return rc;
+  if (!flags || !n_gathered) return fail(h, MPMB_ERR_INVALID, "null argument");
+  if (!(dt > 0.f) || !std::isfinite(dt)) return fail(h, MPMB_ERR_INVALID, "dt must be positive and finite");
+  *n_gathered = 0;
+  MpmbEngine::APool &P0 = h->apool[0], &B0 = h->apool[1];
+  const int nblk = h->nblk;
+  bool any_swap = false, any_clear = false;
+  for (int i = 0; i < nblk; i++) {
+    any_swap |= (flags[i] & MPMB_ASYNC_SWAP) != 0;
+    any_clear |= (flags[i] & MPMB_ASYNC_CLEAR) != 0;
+  }
+  CUDA_TRY(h, cudaMemcpyAsync(h->a_bfl, flags, (size_t)nblk, cudaMemcpyHostToDevice, h->stream));
+
+  // 1. gather: flagged candidates -> sort by (part, page index) -> first copy of every id -> the set, in that order
+  const int np = (int)P0.n, nbk = (int)B0.n;
+  const int64_t nc_all = 2 * (int64_t)np + nbk;
+  int nc = 0, ng = 0;
+  if (nc_all > 0) {
+    if ((rc = scan_reserve(h, (size_t)nc_all)) != MPMB_OK) return rc;
+    k_async_cand_flags<<<nblocks(nc_all), 256, 0, h->stream>>>(P0.r[P0.cur].block, np, B0.r[B0.cur].block, nbk, h->a_bfl, h->scan_a);
+    h->launches++;
+    if ((rc = scan_flags(h, (size_t)nc_all, &nc)) != MPMB_OK) return rc;
+  }
+  if (nc > 0) {
+    if (nc > h->a_ccap) {
+      const int64_t want = std::max<int64_t>(nc, h->a_ccap + h->a_ccap / 2);
+      for (int k = 0; k < 2; k++) { cudaFree(h->a_key[k]); h->a_key[k] = nullptr; }
+      for (auto &u : h->a_u) { cudaFree(u); u = nullptr; }
+      cudaFree(h->a_rowk); cudaFree(h->a_cub);
+      h->a_rowk = nullptr; h->a_cub = nullptr; h->a_ccap = 0; h->a_cub_bytes = 0;
+      for (int k = 0; k < 2; k++) CUDA_TRY(h, cudaMalloc(&h->a_key[k], sizeof(unsigned long long) * want));
+      for (auto &u : h->a_u) CUDA_TRY(h, cudaMalloc(&u, sizeof(uint32_t) * want));
+      CUDA_TRY(h, cudaMalloc(&h->a_rowk, sizeof(int) * want));
+      size_t b1 = 0, b2 = 0;
+      cub::DeviceRadixSort::SortPairs(nullptr, b1, h->a_key[0], h->a_key[1], h->a_u[0], h->a_u[1], (int)want, 0, 38, h->stream);
+      cub::DeviceRadixSort::SortPairs(nullptr, b2, h->a_u[2], h->a_u[3], h->a_u[0], h->a_u[0], (int)want, 0, 32, h->stream);
+      h->a_cub_bytes = std::max(b1, b2);
+      CUDA_TRY(h, cudaMalloc(&h->a_cub, h->a_cub_bytes));
+      h->a_ccap = want;
+    }
+    // keys and candidate indices; once sorted, the unsorted candidate list holds the positions sorted by id, and a_rowk
+    // (rewritten by the routing) the unsorted positions
+    unsigned long long *key = h->a_key[0], *key_s = h->a_key[1];
+    uint32_t *cand = h->a_u[0], *cand_s = h->a_u[1], *ids = h->a_u[2], *ids_s = h->a_u[3];
+    uint32_t *pos = (uint32_t *)h->a_rowk, *pos_s = h->a_u[0];
+    k_async_cand_keys<<<nblocks(nc_all), 256, 0, h->stream>>>(P0.r[P0.cur].block, np, B0.r[B0.cur].block, nbk, h->scan_a, h->scan_b, h->anb[1], h->anb[2], key, cand);
+    size_t bytes = h->a_cub_bytes;
+    cub::DeviceRadixSort::SortPairs(h->a_cub, bytes, key, key_s, cand, cand_s, nc, 0, 38, h->stream);
+    k_async_cand_ids<<<nblocks(nc), 256, 0, h->stream>>>(cand_s, nc, P0.r[P0.cur].id, np, B0.r[B0.cur].id, ids, pos);
+    bytes = h->a_cub_bytes;
+    cub::DeviceRadixSort::SortPairs(h->a_cub, bytes, ids, ids_s, pos, pos_s, nc, 0, 32, h->stream);
+    k_async_first<<<nblocks(nc), 256, 0, h->stream>>>(ids_s, pos_s, nc, h->scan_a);
+    h->launches += 5;
+    if ((rc = scan_flags(h, (size_t)nc, &ng)) != MPMB_OK) return rc;
+    if (ng > h->a_gcap) {
+      cudaFree(h->a_gbuf);
+      h->a_gbuf = nullptr;
+      h->a_gcap = 0;
+      const int64_t want = std::max<int64_t>(ng, 3 * (int64_t)ng / 2);
+      CUDA_TRY(h, cudaMalloc(&h->a_gbuf, sizeof(float) * AREC_WORDS * (size_t)want));
+      h->a_gcap = want;
+    }
+    h->a_G = arec_layout(h->a_gbuf, h->a_gcap);
+    k_async_gather<<<nblocks(nc), 256, 0, h->stream>>>(cand_s, nc, h->scan_a, h->scan_b, P0.r[P0.cur], np, B0.r[B0.cur], h->a_G);
+    h->launches++;
+    CUDA_TRY(h, cudaGetLastError());
+  }
+  // the engine must hold the set: a configured capacity that is too small changes nothing
+  if (ng > 0 && (rc = ensure_capacity(h, ng)) != MPMB_OK) return rc;
+
+  // 2. the level's pools become their blocks' backups
+  if (any_swap) {
+    if ((rc = apool_split(h, B0, MPMB_ASYNC_SWAP, nullptr)) != MPMB_OK) return rc;
+    if ((rc = apool_split(h, P0, MPMB_ASYNC_SWAP, &B0)) != MPMB_OK) return rc;
+  }
+
+  // 3. one ordinary substep on the set; survivors (storage order) with their new blocks
+  int64_t alive = 0;
+  if (ng > 0) {
+    apply_delta_t(h, dt);
+    h->aos_host_pool = nullptr;
+    const ARec &G = h->a_G;
+    if ((rc = pack_rows(h, ng, G.x, G.v, G.F, G.b, G.mass, G.vol, G.scalar, G.group, 0, 0)) != MPMB_OK) return rc;
+    if ((rc = finish_upload(h, ng)) != MPMB_OK) return rc;
+    if ((rc = mpmb_substep(h, 1)) != MPMB_OK) return rc;
+    if ((rc = mpmb_synchronize(h)) != MPMB_OK) return rc;
+    int ns = 0;
+    if ((rc = read_n_store(h, &ns)) != MPMB_OK) return rc;
+    if (ns > 0 && (rc = live_prefix(h, ns, &alive)) != MPMB_OK) return rc;
+    if (alive > h->a_scap) {
+      cudaFree(h->a_sbuf);
+      h->a_sbuf = nullptr;
+      h->a_scap = 0;
+      const int64_t want = std::max<int64_t>(alive, h->a_gcap);
+      CUDA_TRY(h, cudaMalloc(&h->a_sbuf, sizeof(float) * AREC_WORDS * (size_t)want));
+      h->a_scap = want;
+    }
+    h->a_S = arec_layout(h->a_sbuf, h->a_scap);
+    const ARec &S = h->a_S;
+    if (alive > 0) {
+      unpack_live(h, ns, S.id, S.x, S.v, S.F, S.b, S.mass, S.vol, S.scalar, S.group);
+      k_async_blocks<<<nblocks(alive), 256, 0, h->stream>>>(S.x, (int)alive, h->a_inv_dx, h->anb[0], h->anb[1], h->anb[2], S.block, h->a_bad);
+      h->launches++;
+    }
+  }
+
+  // 4. blocks whose backups were consumed drop them
+  if (any_clear && (rc = apool_split(h, B0, MPMB_ASYNC_CLEAR, nullptr)) != MPMB_OK) return rc;
+
+  // 5. survivors, in gather order, to the pool of their new block (EQUAL) or to the backup (CLEAR, not EQUAL)
+  if (alive > 0) {
+    k_fill_u32<<<nblocks(ng), 256, 0, h->stream>>>((uint32_t *)h->a_rowk, ng, 0xffffffffu);
+    k_async_rank<<<nblocks(alive), 256, 0, h->stream>>>(h->a_S.id, (int)alive, h->a_rowk);
+    h->launches += 2;
+    if ((rc = scan_reserve(h, (size_t)ng)) != MPMB_OK) return rc;
+    for (int to_backup = 0; to_backup < 2; to_backup++) {
+      MpmbEngine::APool &D = to_backup ? B0 : P0;
+      int cnt = 0;
+      k_async_route_flags<<<nblocks(ng), 256, 0, h->stream>>>(h->a_rowk, ng, h->a_S.block, h->a_bfl, to_backup, h->scan_a);
+      h->launches++;
+      if ((rc = scan_flags(h, (size_t)ng, &cnt)) != MPMB_OK) return rc;
+      if (cnt == 0) continue;
+      if ((rc = apool_reserve(h, D, D.n + cnt)) != MPMB_OK) return rc;
+      k_async_route<<<nblocks(ng), 256, 0, h->stream>>>(h->a_rowk, ng, h->scan_a, h->scan_b, h->a_S, h->a_G.id, D.r[D.cur], (int)D.n);
+      h->launches++;
+      D.n += cnt;
+    }
+  }
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  *n_gathered = ng;
+  return MPMB_OK;
+}
+
+int mpmb_async_size(MpmbHandle h, int64_t *n_pool, int64_t *n_backup) {
+  CHECK_HANDLE(h);
+  int rc = async_check(h, true);
+  if (rc != MPMB_OK) return rc;
+  if (n_pool) *n_pool = h->apool[0].n;
+  if (n_backup) *n_backup = h->apool[1].n;
+  return MPMB_OK;
+}
+
+int mpmb_async_download(MpmbHandle h, int32_t which, int64_t cap, int64_t *n_out, uint32_t *id, int32_t *block, float *x, float *v, float *F,
+                        float *b, float *mass, float *vol, float *scalar, int32_t *group) {
+  CHECK_HANDLE(h);
+  int rc = async_check(h, true);
+  if (rc != MPMB_OK) return rc;
+  if (which < 0 || which > 1) return fail(h, MPMB_ERR_INVALID, "which = %d: 0 (particle pool) or 1 (backup pool)", which);
+  if (!n_out) return fail(h, MPMB_ERR_INVALID, "n_out is required");
+  const MpmbEngine::APool &p = h->apool[which];
+  *n_out = p.n;
+  if (p.n > cap) return fail(h, MPMB_ERR_CAPACITY, "%lld records do not fit in the %lld rows provided", (long long)p.n, (long long)cap);
+  const ARec &r = p.r[p.cur];
+  const size_t n = (size_t)p.n;
+  const struct { void *d; const void *s; size_t w; } cp[] = {{id, r.id, 1}, {block, r.block, 1}, {x, r.x, 3}, {v, r.v, 3}, {F, r.F, 9}, {b, r.b, 9},
+                                                            {mass, r.mass, 1}, {vol, r.vol, 1}, {scalar, r.scalar, 1}, {group, r.group, 1}};
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  for (const auto &c : cp)
+    if (c.d && n > 0) CUDA_TRY(h, cudaMemcpyAsync(c.d, c.s, 4 * c.w * n, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  return MPMB_OK;
 }
 
 }  // extern "C"
