@@ -201,6 +201,30 @@ int mpmb_append_particles(MpmbHandle h, int64_t n, const float *x, const float *
  * Survivors keep their ids and state; *n_deleted receives the number removed.  No level set: deletes none.  Between
  * substeps; world == 1 (else MPMB_ERR_STATE).                                                                           */
 int mpmb_delete_inside_levelset(MpmbHandle h, int64_t *n_deleted);
+/* The same two edits for z-slab ranks (world > 1), valid on world == 1 too, with one particle-id sequence across ranks.
+ * Every rank receives the SAME batch and the same first_id; particle k gets id first_id + k on the rank that owns it, the
+ * rank whose tile layers [tile_z0, tile_z1) hold its base node's tile layer (decided on the device with the key that packs
+ * it, as mpmb_seed_lattice decides it).  An in-domain, finite particle is therefore kept by exactly one rank; *n_kept
+ * receives this rank's count.  Dropped particles consume their ids as well: every rank, also one that keeps none, raises
+ * its id end to max(id_end, first_id + n).  first_id must not lie below mpmb_id_end (MPMB_ERR_INVALID, nothing changed);
+ * the next free id of a run is the maximum of mpmb_id_end over its ranks.  On world == 1 the append keeps every particle
+ * mpmb_append_particles keeps and, with first_id = the id that call would hand out, gives the same state bit for bit.
+ * Growth and capacity as mpmb_append_particles; growth on a z-slab rank keeps its migration headroom, and the exchange
+ * buffers the neighbours have mapped (mpmb_xchg_connect) stay where they are.  Ids past 2^28 return MPMB_ERR_CAPACITY.
+ * Contract on z-slab runs: every rank makes the same edit at the same substep boundary (between two mpmb_substep calls, or
+ * after the migration of the last substep when the host drives the stages).  Peer-connected ranks then go on with
+ * mpmb_substep(h, n): the first substep after an edit runs outside the graph, the exchange sequence numbers are untouched.
+ * Appends can unbalance the slabs (cuts stay where they are).  Between substeps (else MPMB_ERR_STATE); x, v, mass, vol
+ * and n_kept are required (MPMB_ERR_INVALID).                                                                           */
+int mpmb_append_owned_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
+                                const float *mass, const float *vol, const float *scalar, const int32_t *group,
+                                int64_t first_id, int64_t *n_kept);
+/* mpmb_delete_inside_levelset on this rank's particles; the level set covers the whole node grid on every rank, so a
+ * particle is deleted exactly when one engine holding it would delete it.  Sum *n_deleted over the ranks for the total. */
+int mpmb_delete_owned_inside_levelset(MpmbHandle h, int64_t *n_deleted);
+/* End of the ids handed out so far (absolute, never below id_base): id_base + n after an upload, id_base + 8 * cells of the
+ * whole lattice after mpmb_seed_lattice (on every rank), raised by every append.                                          */
+int mpmb_id_end(MpmbHandle h, int64_t *id_end);
 /* Number of live particles, counted on the device (4 bytes cross the bus; synchronises).
  * Reference: particles.size().                                                                    */
 int mpmb_num_particles(MpmbHandle h, int64_t *n);

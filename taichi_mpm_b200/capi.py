@@ -22,7 +22,8 @@ MATERIAL_BY_NAME = {"linear": MAT_LINEAR, "jelly": MAT_JELLY, "snow": MAT_SNOW, 
 EXPORTS = [
     "mpmb_create", "mpmb_destroy", "mpmb_last_error", "mpmb_version", "mpmb_set_stream", "mpmb_synchronize",
     "mpmb_set_material", "mpmb_set_delta_t", "mpmb_set_sdf", "mpmb_set_planes", "mpmb_set_levelset_shapes", "mpmb_set_id_base",
-    "mpmb_upload_particles", "mpmb_upload_aos", "mpmb_seed_lattice", "mpmb_append_particles", "mpmb_delete_inside_levelset", "mpmb_num_particles", "mpmb_get_update_count", "mpmb_download_bgeo_points", "mpmb_download_particles", "mpmb_download_aos",
+    "mpmb_upload_particles", "mpmb_upload_aos", "mpmb_seed_lattice", "mpmb_append_particles", "mpmb_delete_inside_levelset",
+    "mpmb_append_owned_particles", "mpmb_delete_owned_inside_levelset", "mpmb_id_end", "mpmb_num_particles", "mpmb_get_update_count", "mpmb_download_bgeo_points", "mpmb_download_particles", "mpmb_download_aos",
     "mpmb_substep", "mpmb_sort_particles_and_populate_grid", "mpmb_rasterize", "mpmb_resample", "mpmb_rasterize_part",
     "mpmb_resample_part", "mpmb_download_grid",
     "mpmb_set_profiling", "mpmb_get_profile", "mpmb_get_counters", "mpmb_get_ordering_stats",
@@ -241,6 +242,32 @@ class Engine:
         """Removes the particles where the level set is negative (delete_particles_inside_level_set); returns how many."""
         n = C.c_int64(0)
         self._check(self.L.mpmb_delete_inside_levelset(self.h, C.byref(n)))
+        return n.value
+
+    def append_owned(self, x, v, mass, vol, F=None, b=None, scalar=None, group=None, *, first_id):
+        """Appends the particles of a batch that this engine owns (z-slab ranks: base node in its tile layers; world == 1:
+        every in-domain one), particle k with id first_id + k.  Every rank of a run gets the same batch and first_id, at
+        least the maximum of id_end() over the ranks (slab.global_id_end).  Returns how many this engine kept."""
+        x = _f32(x).reshape(-1, 3)
+        n = len(x)
+        v, F, b = _f32(v, (n, 3)), _f32(F, (n, 9)), _f32(b, (n, 9))
+        mass, vol, scalar = _f32(mass, (n,)), _f32(vol, (n,)), _f32(scalar, (n,))
+        group = None if group is None else np.ascontiguousarray(group, np.int32).reshape(n)
+        kept = C.c_int64(0)
+        self._check(self.L.mpmb_append_owned_particles(self.h, C.c_int64(n), _ptr(x), _ptr(v), _ptr(F), _ptr(b), _ptr(mass), _ptr(vol),
+                                                       _ptr(scalar), _ptr(group), C.c_int64(int(first_id)), C.byref(kept)))
+        return kept.value
+
+    def delete_owned_inside_levelset(self):
+        """Removes this engine's particles where the level set is negative (any world); returns how many."""
+        n = C.c_int64(0)
+        self._check(self.L.mpmb_delete_owned_inside_levelset(self.h, C.byref(n)))
+        return n.value
+
+    def id_end(self):
+        """End of the ids handed out so far (absolute); the next free id of a z-slab run is the maximum over its ranks."""
+        n = C.c_int64(0)
+        self._check(self.L.mpmb_id_end(self.h, C.byref(n)))
         return n.value
 
     def upload_ptrs(self, n, x, v, F, b, mass, vol, scalar, group):

@@ -301,11 +301,19 @@ __device__ __forceinline__ void pack_one(View &V, const Params &P, int row, uint
   keys[row] = make_key(P, x.x, x.y, x.z);
 }
 
-// Field-wise host arrays (staged on the device) -> q streams: particle i into row row0 + i with id id0 + i.
+// Field-wise host arrays (staged on the device) -> q streams: particle i into row row0 + i with id id0 + i.  With
+// `prefix` (the exclusive scan of k_owned_flags over n + 1 entries) only the flagged particles are packed, compacted:
+// particle i into row row0 + prefix[i], still with id id0 + i.
 __global__ void k_pack_particles(View V, Params P, int n, const float *x, const float *v, const float *F, const float *b,
-                                 const float *mass, const float *vol, const float *scalar, const int *group, uint32_t *keys, int row0, uint32_t id0) {
+                                 const float *mass, const float *vol, const float *scalar, const int *group, uint32_t *keys, int row0, uint32_t id0,
+                                 const int *prefix) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  int row = row0 + i;
+  if (prefix) {
+    if (prefix[i + 1] == prefix[i]) return;
+    row = row0 + prefix[i];
+  }
   Mat3 f, bb;
 #pragma unroll
   for (int k = 0; k < 9; k++) {
@@ -321,7 +329,16 @@ __global__ void k_pack_particles(View V, Params P, int n, const float *x, const 
   }
   float3 xx = make_float3(x[3 * (size_t)i], x[3 * (size_t)i + 1], x[3 * (size_t)i + 2]);
   float3 vv = make_float3(v[3 * (size_t)i], v[3 * (size_t)i + 1], v[3 * (size_t)i + 2]);
-  pack_one(V, P, row0 + i, id0 + (uint32_t)i, xx, vv, f, bb, mass[i], vol[i], ps, g, keys);
+  pack_one(V, P, row, id0 + (uint32_t)i, xx, vv, f, bb, mass[i], vol[i], ps, g, keys);
+}
+
+// Ownership of a particle of a batch that every z-slab rank receives: the rank whose own tiles hold the particle's key
+// (make_key: the tile layer of its base node lies in [tile_z0, tile_z1)).  An in-domain, finite particle is owned by
+// exactly one rank; on world == 1 every in-domain particle is owned.  The rest are not packed at all (an upload packs
+// them with the dead key and the ordering drops them: the same live rows in the same order).
+__global__ void k_owned_flags(Params P, int n, const float *x, int *flags) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) flags[i] = make_key(P, x[3 * (size_t)i], x[3 * (size_t)i + 1], x[3 * (size_t)i + 2]) < (uint32_t)P.ntiles_total ? 1 : 0;
 }
 
 // Reference AoS slots (staged on the device) -> q streams.
@@ -2678,6 +2695,8 @@ struct MpmbEngine {
   int64_t id_span_pending = 0;
   int64_t id_span = 0;   // ids of the resident particles lie in [id_base, id_base + id_span): uploads number 0..n-1, the seeded
                          // lattice numbers by lattice index (gaps where the boundary band is skipped)
+  int64_t id_end = 0;    // every id this engine has handed out or seen handed out lies below id_end (absolute, not relative to
+                         // id_base): on a z-slab rank it covers the whole seeded lattice and every batch appended on any rank
 
   // AsyncMPM pools (mpmb_async_*): [0] particle_pool, [1] backup_pool, each double-buffered for the stable edits
   struct APool {
@@ -3176,12 +3195,16 @@ static int ensure_capacity(MpmbEngine *h, int64_t n) {
 
 // Room for `need` rows that keeps rows [0, n_keep) of the current storage (an append onto a resident set).  With a
 // configured capacity that is too small nothing changes; otherwise the buffers grow by at least half, so that a source
-// that appends every frame reallocates rarely.
+// that appends every frame reallocates rarely.  On z-slab ranks growth keeps the migration headroom of ensure_capacity
+// (immigrants are appended after the last row).  The exchange buffers (rx / tx) are not particle rows: they survive.
 static int grow_keeping_rows(MpmbEngine *h, int64_t need, int n_keep) {
-  if (need <= h->cap) return MPMB_OK;
-  if (h->cfg.capacity > 0)
+  if (h->cfg.capacity > 0) {
+    if (need <= h->cap) return MPMB_OK;
     return fail(h, MPMB_ERR_CAPACITY, "%lld particle rows exceed the configured capacity %lld", (long long)need, (long long)h->cap);
-  const int64_t want = std::max<int64_t>(need, std::min<int64_t>(h->cap + h->cap / 2, (1ll << 30) - 1));
+  }
+  const int64_t room = h->cfg.world > 1 ? need + need / 4 + 16 * h->mig_cap : need;
+  if (room <= h->cap) return MPMB_OK;
+  const int64_t want = std::max<int64_t>(room, std::min<int64_t>(h->cap + h->cap / 2, (1ll << 30) - 1));
   float4 *old_q[N_Q];
   uint32_t *old_keys = h->keys[h->cur];
   for (int k = 0; k < N_Q; k++) { old_q[k] = h->q[h->cur][k]; h->q[h->cur][k] = nullptr; }
@@ -3229,6 +3252,7 @@ static int rigid_reserve_ids(MpmbEngine *h, int64_t n_ids);
 static int finish_upload(MpmbEngine *h, int64_t n) {
   h->id_span = std::max<int64_t>(h->id_span_pending, n);
   h->id_span_pending = 0;
+  h->id_end = (int64_t)h->id_base + h->id_span;
   if (h->rigid_on) {  // new particles start with MPMParticle::states = 0 (mpmb_set_particle_states overrides)
     int rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap));
     if (rc != MPMB_OK) return rc;
@@ -3238,11 +3262,13 @@ static int finish_upload(MpmbEngine *h, int64_t n) {
 }
 
 // Packs n field-wise particles held in DEVICE arrays into rows row0.. with ids id0.. of the current storage (F, b, scalar,
-// group may be NULL).  The one packing path of uploads, appends and AsyncMPM advances.
+// group may be NULL).  The one packing path of uploads, appends and AsyncMPM advances.  With `prefix` only the particles
+// k_owned_flags marked, compacted (k_pack_particles).
 static int pack_rows(MpmbEngine *h, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
-                     const float *vol, const float *scalar, const int *group, int row0, uint32_t id0) {
+                     const float *vol, const float *scalar, const int *group, int row0, uint32_t id0, const int *prefix = nullptr) {
   View V = make_view(h);
-  k_pack_particles<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, x, v, F, b, mass, vol, scalar, group, h->keys[h->cur], row0, id0);
+  k_pack_particles<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, x, v, F, b, mass, vol, scalar, group, h->keys[h->cur], row0, id0,
+                                                                         prefix);
   h->launches++;
   cudaError_t e = cudaStreamSynchronize(h->stream);
   CUDA_TRY(h, e);
@@ -3250,10 +3276,15 @@ static int pack_rows(MpmbEngine *h, int64_t n, const float *x, const float *v, c
   return MPMB_OK;
 }
 
-// Stages n field-wise particles on the device and packs them into rows row0.. with ids id0.. of the current storage.
-static int pack_fields(MpmbEngine *h, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
-                       const float *vol, const float *scalar, const int32_t *group, int row0, uint32_t id0) {
-  // stage the field arrays on the device (one allocation)
+// n field-wise particles staged on the device (F, b, scalar, group NULL where the caller gave none)
+struct StagedFields {
+  float *x, *v, *F, *b, *mass, *vol, *scalar;
+  int *group;
+};
+
+// Copies n field-wise host particles into the staging buffer (one allocation, grow-only); asynchronous.
+static int stage_fields(MpmbEngine *h, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
+                        const float *vol, const float *scalar, const int32_t *group, StagedFields *s) {
   size_t fl = (size_t)n * (3 + 3 + (F ? 9 : 0) + (b ? 9 : 0) + 1 + 1 + (scalar ? 1 : 0)) + (group ? (size_t)n : 0);
   float *stage = nullptr;
   if (h->stage_bytes < fl * sizeof(float)) {
@@ -3272,10 +3303,19 @@ static int pack_fields(MpmbEngine *h, int64_t n, const float *x, const float *v,
     p += count;
     return dst;
   };
-  float *dx_ = put(x, 3 * n), *dv = put(v, 3 * n), *dF = put(F, 9 * n), *db = put(b, 9 * n), *dm = put(mass, n), *dvol = put(vol, n),
-        *ds = put(scalar, n);
-  int *dg = (int *)put(group, n);
-  return pack_rows(h, n, dx_, dv, dF, db, dm, dvol, ds, dg, row0, id0);
+  s->x = put(x, 3 * n); s->v = put(v, 3 * n); s->F = put(F, 9 * n); s->b = put(b, 9 * n); s->mass = put(mass, n); s->vol = put(vol, n);
+  s->scalar = put(scalar, n);
+  s->group = (int *)put(group, n);
+  return MPMB_OK;
+}
+
+// Stages n field-wise particles on the device and packs them into rows row0.. with ids id0.. of the current storage.
+static int pack_fields(MpmbEngine *h, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
+                       const float *vol, const float *scalar, const int32_t *group, int row0, uint32_t id0) {
+  StagedFields s;
+  int rc = stage_fields(h, n, x, v, F, b, mass, vol, scalar, group, &s);
+  if (rc != MPMB_OK) return rc;
+  return pack_rows(h, n, s.x, s.v, s.F, s.b, s.mass, s.vol, s.scalar, s.group, row0, id0);
 }
 
 int mpmb_upload_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
@@ -3315,16 +3355,60 @@ int mpmb_append_particles(MpmbHandle h, int64_t n, const float *x, const float *
   h->aos_host_pool = nullptr;   // the AoS index vector does not cover the new ids: mpmb_download_aos needs a new upload
   if ((rc = pack_fields(h, n, x, v, F, b, mass, vol, scalar, group, ns, h->id_base + (uint32_t)id0)) != MPMB_OK) return rc;
   h->id_span = id0 + n;
+  h->id_end = std::max<int64_t>(h->id_end, (int64_t)h->id_base + h->id_span);
   if (h->rigid_on && (rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap))) != MPMB_OK) return rc;   // keeps the colours
   return reorder_from_scratch(h, (int64_t)ns + n);
 }
 
-int mpmb_delete_inside_levelset(MpmbHandle h, int64_t *n_deleted) {
+static int scan_reserve(MpmbEngine *h, size_t n);
+static int scan_flags(MpmbEngine *h, size_t n, int *total);
+
+int mpmb_append_owned_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
+                                const float *mass, const float *vol, const float *scalar, const int32_t *group, int64_t first_id,
+                                int64_t *n_kept) {
   CHECK_HANDLE(h);
-  if (!n_deleted) return fail(h, MPMB_ERR_INVALID, "null argument");
-  *n_deleted = 0;
-  int rc = edit_allowed(h, "delete_inside_levelset");
-  if (rc != MPMB_OK) return rc;
+  if (!n_kept) return fail(h, MPMB_ERR_INVALID, "null argument");
+  *n_kept = 0;
+  if (n < 0 || (n > 0 && (!x || !v || !mass || !vol))) return fail(h, MPMB_ERR_INVALID, "x, v, mass, vol are required");
+  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "append_owned runs between substeps, not inside one");
+  const int64_t end = std::max<int64_t>(h->id_end, h->id_base);
+  if (first_id < end) return fail(h, MPMB_ERR_INVALID, "first_id %lld lies below the id end %lld", (long long)first_id, (long long)end);
+  if (first_id + n > (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_CAPACITY, "particle ids exceed 2^%d", TAG_ID_BITS);
+  int kept = 0, ns = 0, rc;
+  if (n > 0) {
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    if ((rc = read_n_store(h, &ns)) != MPMB_OK) return rc;
+    StagedFields s;
+    if ((rc = stage_fields(h, n, x, v, F, b, mass, vol, scalar, group, &s)) != MPMB_OK) return rc;
+    if ((rc = scan_reserve(h, (size_t)n)) != MPMB_OK) return rc;
+    k_owned_flags<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(h->P, (int)n, s.x, h->scan_a);
+    h->launches++;
+    if ((rc = scan_flags(h, (size_t)n, &kept)) != MPMB_OK) return rc;
+    if (kept > 0) {
+      if ((rc = grow_keeping_rows(h, (int64_t)ns + kept, ns)) != MPMB_OK) return rc;
+      h->aos_host_pool = nullptr;   // as mpmb_append_particles: the AoS index vector does not cover the new ids
+      if ((rc = pack_rows(h, n, s.x, s.v, s.F, s.b, s.mass, s.vol, s.scalar, s.group, ns, (uint32_t)first_id, h->scan_b)) != MPMB_OK) return rc;
+    }
+  }
+  // the whole batch consumes its ids on every rank, kept or not
+  h->id_end = std::max<int64_t>(h->id_end, first_id + n);
+  h->id_span = std::max<int64_t>(h->id_span, h->id_end - (int64_t)h->id_base);
+  *n_kept = kept;
+  if (h->rigid_on && (rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap))) != MPMB_OK) return rc;   // keeps the colours
+  return kept > 0 ? reorder_from_scratch(h, (int64_t)ns + kept) : MPMB_OK;
+}
+
+int mpmb_id_end(MpmbHandle h, int64_t *id_end) {
+  CHECK_HANDLE(h);
+  if (!id_end) return fail(h, MPMB_ERR_INVALID, "null argument");
+  *id_end = std::max<int64_t>(h->id_end, h->id_base);
+  return MPMB_OK;
+}
+
+// the device part of both level-set deletions: every live row of this engine is sampled against the whole node grid
+// (the level set is not sliced on z-slab ranks), the rows inside get the dead key, the set is ordered again
+static int delete_inside(MpmbEngine *h, int64_t *n_deleted) {
+  int rc;
   h->aos_host_pool = nullptr;
   if (!h->P.has_sdf || h->cap == 0) return MPMB_OK;
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
@@ -3341,6 +3425,23 @@ int mpmb_delete_inside_levelset(MpmbHandle h, int64_t *n_deleted) {
   CUDA_TRY(h, cudaGetLastError());
   *n_deleted = killed;
   return killed > 0 ? reorder_from_scratch(h, ns) : MPMB_OK;
+}
+
+int mpmb_delete_inside_levelset(MpmbHandle h, int64_t *n_deleted) {
+  CHECK_HANDLE(h);
+  if (!n_deleted) return fail(h, MPMB_ERR_INVALID, "null argument");
+  *n_deleted = 0;
+  int rc = edit_allowed(h, "delete_inside_levelset");
+  if (rc != MPMB_OK) return rc;
+  return delete_inside(h, n_deleted);
+}
+
+int mpmb_delete_owned_inside_levelset(MpmbHandle h, int64_t *n_deleted) {
+  CHECK_HANDLE(h);
+  if (!n_deleted) return fail(h, MPMB_ERR_INVALID, "null argument");
+  *n_deleted = 0;
+  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "delete_owned_inside_levelset runs between substeps, not inside one");
+  return delete_inside(h, n_deleted);
 }
 
 // flags / exclusive prefix scratch for n items (grow-only) and the CUB scan over them
@@ -3493,7 +3594,9 @@ int mpmb_seed_lattice(MpmbHandle h, const int32_t lo_cell[3], const int32_t hi_c
   }
   if (n_seeded) *n_seeded = total;
   h->id_span_pending = (int64_t)n_cand;   // ids = lattice index
-  return finish_upload(h, total);
+  rc = finish_upload(h, total);
+  h->id_end = (int64_t)h->id_base + (int64_t)cells * 8;   // the whole lattice's ids, whichever of them this rank created
+  return rc;
 }
 
 static int read_n_store(MpmbEngine *h, int *n_store) {

@@ -182,6 +182,58 @@ class SlabRunner:
                     a.migrate_unpack(1, self.mig_recv[1])
 
 
+class SlabEditError(RuntimeError):
+    """An edit failed on another rank of the run (the failing rank raises the engine's own error)."""
+
+
+def _on_all_ranks(call, dist, op):
+    """Runs `call` on this rank and reduces its integer result over the ranks with dist.ReduceOp.<op> (dist None: one engine).
+    A failure on any rank raises on every rank, after the reduction, so that no rank is left waiting in a later collective."""
+    err, value = None, 0
+    try:
+        value = int(call())
+    except Exception as e:  # noqa: BLE001 - re-raised below, after the other ranks have heard of it
+        err = e
+    if dist is None:
+        if err is not None:
+            raise err
+        return value
+    import torch
+    dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend() == "nccl" else torch.device("cpu")
+    failed = torch.tensor([1 if err is not None else 0], dtype=torch.int64, device=dev)
+    total = torch.tensor([value], dtype=torch.int64, device=dev)
+    dist.all_reduce(failed, op=dist.ReduceOp.MAX)
+    dist.all_reduce(total, op=getattr(dist.ReduceOp, op))
+    if err is not None:
+        raise err
+    if int(failed.item()):
+        raise SlabEditError("the edit failed on another rank")
+    return int(total.item())
+
+
+def global_id_end(engine, dist=None):
+    """The next free particle id of the run: the maximum of engine.id_end() over the ranks."""
+    return _on_all_ranks(engine.id_end, dist, "MAX")
+
+
+def append_particles(engine, batch, first_id, dist=None):
+    """Adds a batch of particles to a z-slab run (or to one engine with dist=None) between substeps, keeping every resident
+    particle's id and state.  Every rank passes the SAME batch (dict x, v, mass, vol and optionally F, b, ps, group) and the
+    same first_id (at least global_id_end); particle k gets id first_id + k on the rank that owns it.  Returns the number
+    kept over all ranks (particles outside the domain are dropped, their ids consumed).
+    If a rank fails, every rank raises.  A rank whose configured capacity is too small raises MPMB_ERR_CAPACITY and is left
+    unchanged, but the other ranks have made their part of the edit: the run is then inconsistent.  Engines created with
+    capacity 0 (the default) grow instead and never fail this way."""
+    return _on_all_ranks(lambda: engine.append_owned(batch["x"], batch["v"], batch["mass"], batch["vol"], batch.get("F"), batch.get("b"),
+                                                     batch.get("ps"), batch.get("group"), first_id=first_id),
+                         dist, "SUM")
+
+
+def delete_inside_levelset(engine, dist=None):
+    """Removes the particles inside the level set (phi < 0) on every rank; returns the number removed over all ranks."""
+    return _on_all_ranks(engine.delete_owned_inside_levelset, dist, "SUM")
+
+
 def connect_peers(engine, rank, world, dist):
     """Maps the ring neighbours' receive buffers into `engine` with CUDA IPC (one process per GPU):
     afterwards engine.substep(n) runs whole z-slab substeps, halo and migration included, with no
