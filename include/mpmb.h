@@ -214,8 +214,8 @@ int mpmb_delete_inside_levelset(MpmbHandle h, int64_t *n_deleted);
  * Contract on z-slab runs: every rank makes the same edit at the same substep boundary (between two mpmb_substep calls, or
  * after the migration of the last substep when the host drives the stages).  Peer-connected ranks then go on with
  * mpmb_substep(h, n): the first substep after an edit runs outside the graph, the exchange sequence numbers are untouched.
- * Appends can unbalance the slabs (cuts stay where they are).  Between substeps (else MPMB_ERR_STATE); x, v, mass, vol
- * and n_kept are required (MPMB_ERR_INVALID).                                                                           */
+ * Appends can unbalance the slabs; mpmb_recut_apply moves the cuts.  Between substeps (else MPMB_ERR_STATE); x, v, mass,
+ * vol and n_kept are required (MPMB_ERR_INVALID).                                                                       */
 int mpmb_append_owned_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
                                 const float *mass, const float *vol, const float *scalar, const int32_t *group,
                                 int64_t first_id, int64_t *n_kept);
@@ -451,6 +451,41 @@ int mpmb_halo_send(MpmbHandle h, int32_t face);     /* after mpmb_rasterize     
 int mpmb_halo_recv(MpmbHandle h, int32_t face);     /* before mpmb_resample                      */
 int mpmb_migrate_send(MpmbHandle h, int32_t face);  /* after mpmb_resample                       */
 int mpmb_migrate_recv(MpmbHandle h, int32_t face);  /* before the next ordering                  */
+
+/* Re-cut of a z-slab run (world > 1): the cuts move between substeps, the particles move to their new owner ranks on the
+ * device and keep their ids and state bit for bit.  Contract as for the slab edits: every rank makes the three calls at
+ * the same substep boundary (between two mpmb_substep calls, or after the migration of the last substep when the host
+ * drives the stages); the host moves the packed records between the ranks (any rank may send to any other, so not through
+ * the ring-only peer buffers; taichi_mpm_b200/slab.py uses NCCL all-to-all).  On world == 1 and inside a substep every
+ * call returns MPMB_ERR_STATE.  The live rows are the rows of the current storage, immigrants of the last migration
+ * included; a row's layer is the global tile layer of its base node, int(z / dx - 0.5) >> 2 in the arithmetic that decides
+ * ownership.
+ *
+ * This rank's live rows per global tile layer: counts[n_layers], n_layers = the domain's tile layers ((res[2] + 4) / 4 + 1;
+ * otherwise MPMB_ERR_INVALID).  One histogram pass on the device; n_layers counters cross the bus.  Sum over the ranks
+ * for the histogram of the run.                                                                                       */
+int mpmb_layer_counts(MpmbHandle h, int32_t n_layers, int64_t *counts);
+/* Departing rows of the new cuts cuts[world + 1] (rank r is to own [cuts[r], cuts[r + 1]); cuts[0] = 0, cuts[world] =
+ * n_layers, strictly increasing, else MPMB_ERR_INVALID): counts[world] receives, per destination rank, the live rows whose
+ * layer lies in that rank's new range (0 for this rank).  With dev_buf (a DEVICE buffer of cap_rows records) they are
+ * packed there, grouped by destination in ascending rank order, in storage order within a destination: deterministic.
+ * A record is the migration record, the particle's N_Q = 10 raw float4 rows (160 B) as stored (the sign of a mover's mass
+ * included), so ids, groups, the plastic scalar, apic_b and the cached affine matrix travel bit for bit.  More rows than
+ * cap_rows: MPMB_ERR_CAPACITY, nothing written.  Read-only: the engine is unchanged until mpmb_recut_apply.            */
+int mpmb_recut_pack(MpmbHandle h, const int32_t *cuts, void *dev_buf, int64_t cap_rows, int64_t *counts);
+/* Re-slices this rank to own tile layers [tile_z0, tile_z1) and appends the n_in records (DEVICE memory, the layout of
+ * mpmb_recut_pack) that the other ranks packed for it.  Checked first, nothing changed on failure: the range (else
+ * MPMB_ERR_INVALID), every record owned under the new range (else MPMB_ERR_INVALID), a configured capacity holding the
+ * kept rows plus n_in (else MPMB_ERR_CAPACITY; with capacity 0 the rows grow, keeping the migration headroom).  Then:
+ * the tile grid is sized for the new slab as mpmb_create sizes it (its tile arrays grow when the slab gets thicker and
+ * keep their size otherwise); the rows whose layer stays in range are kept in storage order, the others are dropped (the
+ * departing rows: another rank received them); the records follow in the order given; id end = max(id end, 1 + the
+ * largest id held), so the next free id of the run is unchanged; the whole set is ordered again from scratch.  Exchange
+ * sequence numbers, the exchange buffers and the peers mapped into them (mpmb_xchg_connect) are untouched (their size
+ * does not depend on the slab thickness): peer-connected ranks go on with mpmb_substep(h, n), whose first substep after
+ * the re-cut runs outside the graph.  A rank may end with no particles.  Rigid bodies and AsyncMPM pools do not exist on
+ * z-slab ranks.                                                                                                         */
+int mpmb_recut_apply(MpmbHandle h, int32_t tile_z0, int32_t tile_z1, int64_t n_in, const void *dev_records);
 
 #ifdef __cplusplus
 }

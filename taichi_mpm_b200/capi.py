@@ -33,8 +33,10 @@ EXPORTS = [
     "mpmb_get_particle_cdf", "mpmb_download_cdf",
     "mpmb_xchg_buffer", "mpmb_xchg_ipc_handle", "mpmb_xchg_connect", "mpmb_halo_send", "mpmb_halo_recv", "mpmb_migrate_send", "mpmb_migrate_recv",
     "mpmb_async_init", "mpmb_async_add", "mpmb_async_block_limits", "mpmb_async_advance", "mpmb_async_size", "mpmb_async_download",
+    "mpmb_layer_counts", "mpmb_recut_pack", "mpmb_recut_apply",
 ]
 ASYNC_SMALLER, ASYNC_EQUAL, ASYNC_LARGER, ASYNC_SWAP, ASYNC_CLEAR = 1, 2, 4, 8, 16   # per-block flags of mpmb_async_advance
+RECORD_BYTES = 160   # one particle record of mpmb_recut_pack / mpmb_recut_apply (and of the migration messages)
 
 
 class MpmbConfig(C.Structure):
@@ -539,6 +541,32 @@ class Engine:
 
     def migrate_recv(self, face):
         self._check(self.L.mpmb_migrate_recv(self.h, C.c_int32(face)))
+
+    # --- re-cut of a z-slab run (device buffers: anything with data_ptr(), numel() and element_size(), e.g. torch tensors)
+    def tile_range(self):
+        """The tile layers [tile_z0, tile_z1) this engine owns now."""
+        return int(self.cfg.tile_z0), int(self.cfg.tile_z1)
+
+    def layer_counts(self):
+        """This engine's live particles per tile layer of the whole domain (int64 array)."""
+        out = np.zeros((self.res[2] + 4) // 4 + 1, np.int64)
+        self._check(self.L.mpmb_layer_counts(self.h, C.c_int32(len(out)), _ptr(out)))
+        return out
+
+    def recut_pack(self, cuts, buf=None):
+        """Departing particles of the new cuts (world + 1 tile layers, rank r owns [cuts[r], cuts[r + 1])): their number per
+        destination rank; with `buf` also packed there (RECORD_BYTES each, by destination in rank order).  Changes nothing."""
+        cuts = np.ascontiguousarray(cuts, np.int32)
+        counts = np.zeros(len(cuts) - 1, np.int64)
+        ptr, cap = (None, 0) if buf is None else (C.c_void_p(buf.data_ptr()), buf.numel() * buf.element_size() // RECORD_BYTES)
+        self._check(self.L.mpmb_recut_pack(self.h, _ptr(cuts), ptr, C.c_int64(cap), _ptr(counts)))
+        return counts
+
+    def recut_apply(self, z0, z1, buf, n_in):
+        """Owns tile layers [z0, z1) from now on: keeps the particles that stay, appends the n_in records of `buf`."""
+        ptr = C.c_void_p(buf.data_ptr()) if buf is not None and n_in > 0 else None
+        self._check(self.L.mpmb_recut_apply(self.h, C.c_int32(int(z0)), C.c_int32(int(z1)), C.c_int64(int(n_in)), ptr))
+        self.cfg.tile_z0, self.cfg.tile_z1 = int(z0), int(z1)
 
     # --- profiling
     def set_profiling(self, enabled):

@@ -2386,6 +2386,97 @@ __global__ void k_migrate_commit(Counters *c, const int *hdr, int cap, int cap_p
   c->n_movers += n;
 }
 
+// ---- re-cut of the z slabs (mpmb_layer_counts, mpmb_recut_pack, mpmb_recut_apply), between substeps.  The GLOBAL tile layer
+// of a row's base node, with make_key's arithmetic; a live row's layer lies in its rank's [tile_z0, tile_z1).
+__device__ __forceinline__ int base_layer(float z, float inv_dx) {
+  int bz;
+  float r;
+  base_rel(z, inv_dx, bz, r);
+  return bz >> 2;
+}
+constexpr int RECUT_MAX_LAYERS = 1026;  // tile layers of a 4096-cell axis
+
+// live rows of the current storage per global tile layer: a shared-memory histogram per CTA, one 64-bit integer atomic
+// per non-empty bin into hist (zeroed by the caller)
+__global__ void __launch_bounds__(256) k_layer_hist(const uint32_t *keys, const float4 *q0, uint32_t special_min, float inv_dx, int n_layers,
+                                                    const Counters *cnt, unsigned long long *hist) {
+  __shared__ int s_h[RECUT_MAX_LAYERS];
+  for (int l = threadIdx.x; l < n_layers; l += blockDim.x) s_h[l] = 0;
+  __syncthreads();
+  const int n = cnt->n_store;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (keys[i] >= special_min) continue;
+    const int l = base_layer(q0[i].z, inv_dx);
+    if (l >= 0 && l < n_layers) atomicAdd(&s_h[l], 1);
+  }
+  __syncthreads();
+  for (int l = threadIdx.x; l < n_layers; l += blockDim.x)
+    if (s_h[l]) atomicAdd(&hist[l], (unsigned long long)s_h[l]);
+}
+
+// flags[i] = 1 for the live rows whose base layer lies in [lo, hi)
+__global__ void k_layer_flags(const uint32_t *keys, const float4 *q0, int n, uint32_t special_min, float inv_dx, int lo, int hi, int *flags) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int f = 0;
+  if (keys[i] < special_min) {
+    const int l = base_layer(q0[i].z, inv_dx);
+    f = l >= lo && l < hi;
+  }
+  flags[i] = f;
+}
+
+// the rows k_layer_flags marked (prefix = its exclusive scan), in storage order, as migration records: N_Q raw float4 rows
+__global__ void k_recut_pack(View V, int n, const int *prefix, float4 *rec) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || prefix[i + 1] == prefix[i]) return;
+  const size_t o = (size_t)prefix[i];
+#pragma unroll
+  for (int k = 0; k < N_Q; k++) rec[o * N_Q + k] = V.q[k][i];
+}
+
+// the rows k_layer_flags marked, compacted in storage order into the other buffer and keyed under the new slicing P;
+// *max_id = the largest id among them (warp maximum, one atomic per warp)
+__global__ void __launch_bounds__(256) k_recut_keep(View V, Params P, int n, const int *prefix, int *max_id) {
+  int m = -1;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (prefix[i + 1] == prefix[i]) continue;
+    const size_t o = (size_t)prefix[i];
+#pragma unroll
+    for (int k = 0; k < N_Q; k++) V.qn[k][o] = V.q[k][i];
+    const float4 r0 = V.q[0][i];
+    V.keys_next[o] = make_key(P, r0.x, r0.y, r0.z);
+    m = max(m, (int)(__float_as_uint(V.q[6][i].w) & TAG_ID_MASK));
+  }
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31) == 0 && m >= 0) atomicMax(max_id, m);
+}
+
+// the arriving records of a re-cut, before anything changes: *bad counts those the new slicing P does not own, *max_id
+// receives their largest id
+__global__ void __launch_bounds__(256) k_recut_check(Params P, int n, const float4 *rec, int *bad, int *max_id) {
+  int m = -1, b = 0;
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
+    const float4 r0 = rec[(size_t)e * N_Q];
+    b += make_key(P, r0.x, r0.y, r0.z) >= (uint32_t)P.ntiles_total;
+    m = max(m, (int)(__float_as_uint(rec[(size_t)e * N_Q + 6].w) & TAG_ID_MASK));
+  }
+  if (b) atomicAdd(bad, b);
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31) == 0 && m >= 0) atomicMax(max_id, m);
+}
+
+// the arriving records after row row0 of the current storage, keyed under P (as k_migrate_recv2 appends immigrants)
+__global__ void k_recut_unpack(View V, Params P, int n, int row0, const float4 *rec) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const int dst = row0 + e;
+#pragma unroll
+  for (int k = 0; k < N_Q; k++) V.q[k][dst] = rec[(size_t)e * N_Q + k];
+  const float4 r0 = rec[(size_t)e * N_Q];
+  V.keys[dst] = make_key(P, r0.x, r0.y, r0.z);
+}
+
 // ------------------------------------------------------------------------------ AsyncMPM pools (mpmb_async_*)
 // One pool of AsyncMPM particle records, SoA: x[3n] v[3n] F[9n] b[9n] mass vol scalar group id block (the linear index of
 // the record's 4x4x8-node scheduler block).
@@ -2665,6 +2756,7 @@ struct MpmbEngine {
   uint32_t id_base = 0;
   int num_sms = 132;  // H100 SXM; queried from the device in mpmb_create
   int nt2_global = 0;  // tile layers of the whole domain (P.nt[2] is slab-local)
+  unsigned long long *recut_buf = nullptr;  // re-cut scratch: layer histogram [nt2_global], then two ints (bad arrivals, largest id)
   int grid_p2g = 132 * 4, grid_g2p = 132 * 4;  // persistent grids = SMs x resident CTAs (queried)
   int64_t launches = 0;
 
@@ -2897,6 +2989,69 @@ static int alloc_particles(MpmbEngine *h, int64_t cap) {
   return MPMB_OK;
 }
 
+// The dense tile grid of an engine that owns tile layers [z0, z1) of the domain: on a z-slab rank its own layers plus one
+// ghost layer on each side, on world == 1 the whole domain; the keys of that grid and the ordering's block count.
+// mpmb_create sizes an engine with it, mpmb_recut_apply re-slices one.
+struct Slicing {
+  int tz_off, nt2, tile_z0, tile_z1, ntot, key_bits, ord_blocks;
+};
+static bool slab_slicing(const Params &P, int nt2_global, int world, int z0, int z1, Slicing *s) {
+  s->tz_off = 0; s->nt2 = nt2_global; s->tile_z0 = 0; s->tile_z1 = nt2_global;
+  if (world > 1) {
+    s->tz_off = z0 - 1;    // one ghost layer below ...
+    s->nt2 = z1 - z0 + 2;  // ... and one above the owned layers
+    s->tile_z0 = z0; s->tile_z1 = z1;
+  }
+  const unsigned long long ntot = (unsigned long long)P.nt[0] * P.nt[1] * s->nt2;
+  s->key_bits = 1;
+  while ((1ull << s->key_bits) <= ntot + SPECIAL_DEAD) s->key_bits++;
+  if (s->key_bits > 31) return false;  // tile grid too large for 32-bit keys
+  s->ntot = (int)ntot;
+  s->ord_blocks = (int)((ntot + ORD_TILE - 1) / ORD_TILE);
+  return true;
+}
+static void set_slicing(MpmbEngine *h, const Slicing &s) {
+  Params &P = h->P;
+  P.tz_off = s.tz_off; P.nt[2] = s.nt2; P.tile_z0 = s.tile_z0; P.tile_z1 = s.tile_z1; P.ntiles_total = s.ntot;
+  h->ntot = s.ntot;
+  h->special_min = (uint32_t)s.ntot;
+  h->key_dead = (uint32_t)s.ntot + SPECIAL_DEAD;
+  h->key_bits = s.key_bits;
+  h->ord_blocks = s.ord_blocks;
+}
+
+// Dense per-tile arrays, active-tile records, arenas (plus the all-zero arena read for absent neighbours, past the last
+// slot), node velocities and the ordering's block sums for `cap_tiles` tiles.  All or nothing: on failure the engine keeps
+// the arrays it had.
+static int alloc_tile_arrays(MpmbEngine *h, int64_t cap_tiles) {
+  int *dense[11] = {}, *blocksum = nullptr;
+  TileMeta *meta = nullptr;
+  float4 *arena = nullptr, *vel = nullptr;
+  const int64_t blocks = (cap_tiles + ORD_TILE - 1) / ORD_TILE;
+  bool ok = true;
+  for (int *&p : dense) ok = ok && cudaMalloc(&p, sizeof(int) * cap_tiles) == cudaSuccess;
+  ok = ok && cudaMalloc(&blocksum, sizeof(int) * 3 * (blocks + 1)) == cudaSuccess;
+  ok = ok && cudaMalloc(&meta, sizeof(TileMeta) * cap_tiles) == cudaSuccess;
+  ok = ok && cudaMalloc(&arena, sizeof(float4) * ARENA * (cap_tiles + 1)) == cudaSuccess;
+  ok = ok && cudaMalloc(&vel, sizeof(float4) * ARENA * cap_tiles) == cudaSuccess;
+  if (!ok) {
+    const std::string msg = cudaGetErrorString(cudaGetLastError());
+    for (int *p : dense) cudaFree(p);
+    cudaFree(blocksum); cudaFree(meta); cudaFree(arena); cudaFree(vel);
+    return fail(h, MPMB_ERR_CUDA, "cudaMalloc of the tile arrays (%lld tiles): %s", (long long)cap_tiles, msg.c_str());
+  }
+  for (int *p : dense) cudaMemsetAsync(p, 0, sizeof(int) * cap_tiles, h->stream);
+  cudaMemsetAsync(arena + (size_t)ARENA * cap_tiles, 0, sizeof(float4) * ARENA, h->stream);
+  int **mine[] = {&h->run_begin[0], &h->run_begin[1], &h->run_len[0], &h->run_len[1], &h->stay[0], &h->stay[1],
+                  &h->arr_cnt, &h->arr_off, &h->arr_len, &h->arr_cur, &h->slot_map};
+  for (int k = 0; k < 11; k++) { cudaFree(*mine[k]); *mine[k] = dense[k]; }
+  cudaMemsetAsync(h->slot_map, 0xFF, sizeof(int) * cap_tiles, h->stream);
+  cudaFree(h->blocksum); cudaFree(h->meta); cudaFree(h->arena); cudaFree(h->vel);
+  h->blocksum = blocksum; h->meta = meta; h->arena = arena; h->vel = vel;
+  h->cap_tiles = (int)cap_tiles;
+  return MPMB_OK;
+}
+
 extern "C" {
 
 static int read_n_store(MpmbEngine *h, int *n_store);
@@ -2919,7 +3074,6 @@ int mpmb_create(const MpmbConfig *cfg, MpmbHandle *out) {
   h->cfg = *cfg;
   if (h->cfg.world <= 0) h->cfg.world = 1;
   Params &P = h->P;
-  size_t ntot = 1;
   for (int d = 0; d < 3; d++) {
     P.res[d] = cfg->res[d];
     P.nnode[d] = cfg->res[d] + 1;
@@ -2927,18 +3081,14 @@ int mpmb_create(const MpmbConfig *cfg, MpmbHandle *out) {
     P.gdt[d] = cfg->gravity[d] * cfg->dt;
   }
   h->nt2_global = P.nt[2];
-  P.tz_off = 0;
-  if (h->cfg.world > 1) {
-    if (cfg->tile_z0 < 0 || cfg->tile_z1 > P.nt[2] || cfg->tile_z0 >= cfg->tile_z1) {
-      const int n2 = P.nt[2];
-      delete h;
-      return fail(nullptr, MPMB_ERR_INVALID, "bad slab [%d,%d) for %d tile layers", cfg->tile_z0, cfg->tile_z1, n2);
-    }
-    P.tz_off = cfg->tile_z0 - 1;                   // one ghost layer below ...
-    P.nt[2] = cfg->tile_z1 - cfg->tile_z0 + 2;     // ... and one above the owned layers
+  if (h->cfg.world > 1 && (cfg->tile_z0 < 0 || cfg->tile_z1 > P.nt[2] || cfg->tile_z0 >= cfg->tile_z1)) {
+    const int n2 = P.nt[2];
+    delete h;
+    return fail(nullptr, MPMB_ERR_INVALID, "bad slab [%d,%d) for %d tile layers", cfg->tile_z0, cfg->tile_z1, n2);
   }
-  for (int d = 0; d < 3; d++) ntot *= (size_t)P.nt[d];
-  P.ntiles_total = (int)ntot;
+  Slicing sl;
+  if (!slab_slicing(P, h->nt2_global, h->cfg.world, cfg->tile_z0, cfg->tile_z1, &sl)) { delete h; return fail(nullptr, MPMB_ERR_INVALID, "tile grid too large for 32-bit keys"); }
+  set_slicing(h, sl);
   P.dx = cfg->dx;
   P.inv_dx = 1.0f / cfg->dx;
   P.dt = cfg->dt;
@@ -2947,8 +3097,6 @@ int mpmb_create(const MpmbConfig *cfg, MpmbHandle *out) {
   P.friction = 0.f;
   P.has_sdf = 0;
   P.world = h->cfg.world;
-  P.tile_z0 = h->cfg.world > 1 ? cfg->tile_z0 : 0;
-  P.tile_z1 = h->cfg.world > 1 ? cfg->tile_z1 : P.nt[2];
   for (int g = 0; g < MPMB_MAX_GROUPS; g++) {
     P.mats[g].kind = MAT_JELLY;  // JellyParticle defaults E=1e5, nu=0.3 (src/particles.cpp:383-389)
     for (int k = 0; k < 8; k++) P.mats[g].p[k] = 0.f;
@@ -2957,11 +3105,6 @@ int mpmb_create(const MpmbConfig *cfg, MpmbHandle *out) {
   }
   h->use_graph = cfg->no_graph == 0;
   if (const char *g = getenv("MPMB_GRAPH")) h->use_graph = g[0] != '0';   // MPMB_GRAPH=0: launch every kernel from the host (A/B, debugging)
-  h->special_min = (uint32_t)ntot;
-  h->key_dead = (uint32_t)ntot + SPECIAL_DEAD;
-  h->key_bits = 1;
-  while ((1ull << h->key_bits) <= (unsigned long long)ntot + SPECIAL_DEAD) h->key_bits++;
-  if (h->key_bits > 31) { delete h; return fail(nullptr, MPMB_ERR_INVALID, "tile grid too large for 32-bit keys"); }
   if (cudaSetDevice(cfg->device) != cudaSuccess) { delete h; return fail(nullptr, MPMB_ERR_CUDA, "cudaSetDevice failed"); }
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, cfg->device);
@@ -2972,31 +3115,18 @@ int mpmb_create(const MpmbConfig *cfg, MpmbHandle *out) {
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_p2g, P2G_T, P2G_DYN_BYTES) == cudaSuccess && occ > 0) h->grid_p2g = h->num_sms * occ;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_g2p<128, true, true>, 128, 0) == cudaSuccess && occ > 0) h->grid_g2p = h->num_sms * occ;
   }
-  // tiles: every tile of the (slab of the) domain can be active
-  int64_t cap_tiles = (int64_t)ntot;
-  h->cap_tiles = (int)cap_tiles;
   auto bail = [&](const char *what) {
     std::string msg = std::string(what) + ": " + cudaGetErrorString(cudaGetLastError());
     mpmb_destroy(h);
     return fail(nullptr, MPMB_ERR_CUDA, "%s", msg.c_str());
   };
-  h->ntot = (int)ntot;
-  h->ord_blocks = (int)((ntot + ORD_TILE - 1) / ORD_TILE);
-  {
-    int **dense[] = {&h->run_begin[0], &h->run_begin[1], &h->run_len[0], &h->run_len[1], &h->stay[0], &h->stay[1],
-                     &h->arr_cnt, &h->arr_off, &h->arr_len, &h->arr_cur, &h->slot_map};
-    for (int **pp : dense) {
-      if (cudaMalloc(pp, sizeof(int) * ntot) != cudaSuccess) return bail("cudaMalloc dense tile array");
-      cudaMemset(*pp, 0, sizeof(int) * ntot);
-    }
+  // tiles: every tile of the (slab of the) domain can be active
+  if (alloc_tile_arrays(h, sl.ntot) != MPMB_OK) {
+    g_create_error = h->err;
+    mpmb_destroy(h);
+    return MPMB_ERR_CUDA;
   }
-  if (cudaMalloc(&h->blocksum, sizeof(int) * 3 * (h->ord_blocks + 1)) != cudaSuccess) return bail("cudaMalloc blocksum");
-  if (cudaMalloc(&h->meta, sizeof(TileMeta) * cap_tiles) != cudaSuccess) return bail("cudaMalloc meta");
-  if (cudaMalloc(&h->arena, sizeof(float4) * ARENA * (cap_tiles + 1)) != cudaSuccess) return bail("cudaMalloc arena");
-  cudaMemset(h->arena + (size_t)ARENA * cap_tiles, 0, sizeof(float4) * ARENA);  // the all-zero arena read for absent neighbours
-  if (cudaMalloc(&h->vel, sizeof(float4) * ARENA * cap_tiles) != cudaSuccess) return bail("cudaMalloc vel");
   if (cudaMalloc(&h->cnt, sizeof(Counters)) != cudaSuccess) return bail("cudaMalloc counters");
-  cudaMemset(h->slot_map, 0xFF, sizeof(int) * ntot);
   cudaMemset(h->cnt, 0, sizeof(Counters));
   h->mig_cap = h->cfg.world > 1 ? (cfg->migrate_capacity > 0 ? cfg->migrate_capacity : 65536) : 0;
   if (h->cfg.world > 1) {
@@ -3026,7 +3156,7 @@ int mpmb_destroy(MpmbHandle h) {
   cudaFree(h->arr_cnt); cudaFree(h->arr_off); cudaFree(h->arr_len); cudaFree(h->arr_cur); cudaFree(h->slot_map); cudaFree(h->blocksum);
   cudaFree(h->meta);
   cudaFree(h->arena); cudaFree(h->vel); cudaFree(h->sdf4); cudaFree(h->cnt); cudaFree(h->stage_buf); cudaFree(h->xcount);
-  cudaFree(h->aos_pool); cudaFree(h->aos_idx); cudaFree(h->scan_a); cudaFree(h->scan_b); cudaFree(h->scan_tmp);
+  cudaFree(h->aos_pool); cudaFree(h->aos_idx); cudaFree(h->scan_a); cudaFree(h->scan_b); cudaFree(h->scan_tmp); cudaFree(h->recut_buf);
   for (int k = 0; k < 2; k++)
     for (int f = 0; f < 2; f++) {
       if (h->tx_ipc[k][f] && h->tx[k][f]) cudaIpcCloseMemHandle(h->tx[k][f]);
@@ -4646,6 +4776,152 @@ int mpmb_migrate_recv(MpmbHandle h, int32_t face) {
   if (h->cfg.world <= 1 || face < 0 || face > 1 || !h->tx[1][face]) return fail(h, MPMB_ERR_STATE, "no connected peer through face %d", face);
   if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "migrate_recv must follow resample");
   return xchg_migrate_launch(h, 0, 1 << face);
+}
+
+// ------------------------------------------------------------------------------ re-cut of the z slabs
+static int recut_allowed(MpmbEngine *h, const char *what) {
+  if (h->cfg.world <= 1) return fail(h, MPMB_ERR_STATE, "%s re-cuts z-slab runs (world > 1)", what);
+  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "%s runs between substeps, not inside one", what);
+  return MPMB_OK;
+}
+
+// the scratch of the re-cut kernels: the layer histogram, then {bad arrivals, largest id}
+static int recut_reserve(MpmbEngine *h) {
+  if (!h->recut_buf) CUDA_TRY(h, cudaMalloc(&h->recut_buf, sizeof(unsigned long long) * (h->nt2_global + 1)));
+  return MPMB_OK;
+}
+static int *recut_ints(MpmbEngine *h) { return (int *)(h->recut_buf + h->nt2_global); }
+
+// live rows per global tile layer into counts[nt2_global] (synchronises; nt2_global counters cross the bus)
+static int layer_hist(MpmbEngine *h, int64_t *counts) {
+  int rc = recut_reserve(h);
+  if (rc != MPMB_OK) return rc;
+  const int nl = h->nt2_global;
+  CUDA_TRY(h, cudaMemsetAsync(h->recut_buf, 0, sizeof(unsigned long long) * nl, h->stream));
+  if (h->cap > 0) {
+    k_layer_hist<<<h->num_sms * 4, 256, 0, h->stream>>>(h->keys[h->cur], h->q[h->cur][0], h->special_min, h->P.inv_dx, nl, h->cnt, h->recut_buf);
+    h->launches++;
+  }
+  static_assert(sizeof(int64_t) == sizeof(unsigned long long), "64-bit counters");
+  CUDA_TRY(h, cudaMemcpyAsync(counts, h->recut_buf, sizeof(int64_t) * nl, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  return MPMB_OK;
+}
+
+int mpmb_layer_counts(MpmbHandle h, int32_t n_layers, int64_t *counts) {
+  CHECK_HANDLE(h);
+  int rc = recut_allowed(h, "layer_counts");
+  if (rc != MPMB_OK) return rc;
+  if (!counts) return fail(h, MPMB_ERR_INVALID, "null argument");
+  if (n_layers != h->nt2_global) return fail(h, MPMB_ERR_INVALID, "n_layers %d: the domain has %d tile layers", n_layers, h->nt2_global);
+  return layer_hist(h, counts);
+}
+
+int mpmb_recut_pack(MpmbHandle h, const int32_t *cuts, void *dev_buf, int64_t cap_rows, int64_t *counts) {
+  CHECK_HANDLE(h);
+  int rc = recut_allowed(h, "recut_pack");
+  if (rc != MPMB_OK) return rc;
+  const int world = h->cfg.world, nl = h->nt2_global;
+  if (!cuts || !counts || cap_rows < 0) return fail(h, MPMB_ERR_INVALID, "bad argument");
+  if (cuts[0] != 0 || cuts[world] != nl) return fail(h, MPMB_ERR_INVALID, "cuts must run from 0 to %d tile layers", nl);
+  for (int r = 0; r < world; r++)
+    if (cuts[r + 1] <= cuts[r]) return fail(h, MPMB_ERR_INVALID, "cuts must increase strictly (rank %d: [%d, %d))", r, cuts[r], cuts[r + 1]);
+  std::vector<int64_t> hist(nl);
+  if ((rc = layer_hist(h, hist.data())) != MPMB_OK) return rc;
+  int64_t total = 0;
+  for (int d = 0; d < world; d++) {
+    counts[d] = 0;
+    if (d != h->cfg.rank)
+      for (int l = cuts[d]; l < cuts[d + 1]; l++) counts[d] += hist[l];
+    total += counts[d];
+  }
+  if (!dev_buf || total == 0) return MPMB_OK;
+  if (total > cap_rows) return fail(h, MPMB_ERR_CAPACITY, "%lld departing rows do not fit in the %lld records provided", (long long)total, (long long)cap_rows);
+  int ns = 0;
+  if ((rc = read_n_store(h, &ns)) != MPMB_OK) return rc;
+  if ((rc = scan_reserve(h, (size_t)ns)) != MPMB_OK) return rc;
+  View V = make_view(h);
+  int64_t off = 0;
+  for (int d = 0; d < world; d++) {   // grouped by destination in ascending rank order, storage order within a destination
+    if (counts[d] == 0) continue;
+    k_layer_flags<<<(ns + 255) / 256, 256, 0, h->stream>>>(h->keys[h->cur], h->q[h->cur][0], ns, h->special_min, h->P.inv_dx, cuts[d], cuts[d + 1], h->scan_a);
+    int got = 0;
+    if ((rc = scan_flags(h, (size_t)ns, &got)) != MPMB_OK) return rc;
+    if (got != counts[d]) return fail(h, MPMB_ERR_STATE, "rank %d: %d rows flagged, %lld counted", d, got, (long long)counts[d]);
+    k_recut_pack<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, ns, h->scan_b, (float4 *)dev_buf + (size_t)off * N_Q);
+    h->launches += 2;
+    off += counts[d];
+  }
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  return MPMB_OK;
+}
+
+int mpmb_recut_apply(MpmbHandle h, int32_t tile_z0, int32_t tile_z1, int64_t n_in, const void *dev_records) {
+  CHECK_HANDLE(h);
+  int rc = recut_allowed(h, "recut_apply");
+  if (rc != MPMB_OK) return rc;
+  if (tile_z0 < 0 || tile_z1 > h->nt2_global || tile_z0 >= tile_z1)
+    return fail(h, MPMB_ERR_INVALID, "bad slab [%d,%d) for %d tile layers", tile_z0, tile_z1, h->nt2_global);
+  if (n_in < 0 || (n_in > 0 && !dev_records)) return fail(h, MPMB_ERR_INVALID, "n_in >= 0 records are required");
+  if (n_in >= (1ll << 30)) return fail(h, MPMB_ERR_CAPACITY, "%lld arriving records exceed 2^30 particle rows per GPU", (long long)n_in);
+  Slicing sl;
+  if (!slab_slicing(h->P, h->nt2_global, h->cfg.world, tile_z0, tile_z1, &sl)) return fail(h, MPMB_ERR_INVALID, "tile grid too large for 32-bit keys");
+  Params Pn = h->P;
+  Pn.tz_off = sl.tz_off; Pn.nt[2] = sl.nt2; Pn.tile_z0 = sl.tile_z0; Pn.tile_z1 = sl.tile_z1; Pn.ntiles_total = sl.ntot;
+  if ((rc = recut_reserve(h)) != MPMB_OK) return rc;
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  int ns = 0, kept = 0;
+  if (h->cap > 0 && (rc = read_n_store(h, &ns)) != MPMB_OK) return rc;
+  // checks first: what stays, whether every arrival belongs here, whether a configured capacity holds both
+  if (ns > 0) {
+    if ((rc = scan_reserve(h, (size_t)ns)) != MPMB_OK) return rc;
+    k_layer_flags<<<(ns + 255) / 256, 256, 0, h->stream>>>(h->keys[h->cur], h->q[h->cur][0], ns, h->special_min, h->P.inv_dx, tile_z0, tile_z1, h->scan_a);
+    h->launches++;
+    if ((rc = scan_flags(h, (size_t)ns, &kept)) != MPMB_OK) return rc;
+  }
+  int *ints = recut_ints(h);   // {bad arrivals, largest id held}
+  CUDA_TRY(h, cudaMemsetAsync(ints, 0, sizeof(int), h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(ints + 1, 0xFF, sizeof(int), h->stream));
+  if (n_in > 0) {
+    k_recut_check<<<std::min<int64_t>((n_in + 255) / 256, h->num_sms * 8), 256, 0, h->stream>>>(Pn, (int)n_in, (const float4 *)dev_records, ints, ints + 1);
+    h->launches++;
+    int bad = 0;
+    CUDA_TRY(h, cudaMemcpyAsync(&bad, ints, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    CUDA_TRY(h, cudaGetLastError());
+    if (bad) return fail(h, MPMB_ERR_INVALID, "%d of %lld arriving records lie outside tile layers [%d, %d)", bad, (long long)n_in, tile_z0, tile_z1);
+  }
+  const int64_t need = (int64_t)kept + n_in;
+  if (need >= (1ll << 30)) return fail(h, MPMB_ERR_CAPACITY, "%lld particle rows exceed 2^30 per GPU", (long long)need);
+  if (h->cfg.capacity > 0 && need > h->cap)
+    return fail(h, MPMB_ERR_CAPACITY, "%lld particle rows exceed the configured capacity %lld", (long long)need, (long long)h->cap);
+  // the engine changes from here on: a thicker slab grows the tile arrays, the rows grow if they must
+  if (sl.ntot > h->cap_tiles && (rc = alloc_tile_arrays(h, sl.ntot)) != MPMB_OK) return rc;
+  if (need > 0 && (rc = grow_keeping_rows(h, need, ns)) != MPMB_OK) return rc;
+  set_slicing(h, sl);
+  h->cfg.tile_z0 = tile_z0;
+  h->cfg.tile_z1 = tile_z1;
+  if (h->cap > 0) {
+    if (kept > 0) {   // the staying rows, compacted in storage order into the other buffer, re-keyed; departing rows are left behind
+      k_recut_keep<<<std::min((ns + 255) / 256, h->num_sms * 8), 256, 0, h->stream>>>(make_view(h), h->P, ns, h->scan_b, ints + 1);
+      h->launches++;
+    }
+    h->cur ^= 1;
+    if (n_in > 0) {
+      k_recut_unpack<<<(unsigned)((n_in + 127) / 128), 128, 0, h->stream>>>(make_view(h), h->P, (int)n_in, kept, (const float4 *)dev_records);
+      h->launches++;
+    }
+  }
+  int max_id = -1;
+  CUDA_TRY(h, cudaMemcpyAsync(&max_id, ints + 1, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  h->id_end = std::max<int64_t>(h->id_end, (int64_t)max_id + 1);
+  h->aos_host_pool = nullptr;
+  graph_reset(h);
+  return reorder_from_scratch(h, need);
 }
 
 }  // extern "C"

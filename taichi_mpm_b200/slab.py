@@ -25,13 +25,17 @@ def base_tile_z(z, dx):
     return (X - np.float32(0.5)).astype(np.int32) >> 2
 
 
-def slab_partition(tile_z, n_layers, world):
-    """Cuts [0, n_layers) into `world` contiguous slabs with balanced particle counts.
+def layer_histogram(tile_z, n_layers):
+    """Particles per tile layer of [0, n_layers), from the tile layer of every particle."""
+    return np.bincount(np.asarray(tile_z, np.int64), minlength=n_layers)[:n_layers]
 
-    tile_z: tile layer of every particle.  Returns [(z0, z1)] * world; every slab has >= 1 layer and
-    the cuts are placed by the prefix sum of the per-layer particle histogram over the occupied
-    extent (column-collapse scenes occupy a small part of the domain, SURVEY §8e)."""
-    hist = np.bincount(np.asarray(tile_z, np.int64), minlength=n_layers)[:n_layers].astype(np.float64)
+
+def partition_counts(hist, world):
+    """Cuts the tile layers of a particle histogram (hist[l] = particles in layer l) into `world` contiguous slabs with
+    balanced particle counts.  Returns [(z0, z1)] * world; every slab has >= 1 layer and the cuts are placed by the prefix
+    sum of the histogram over the occupied extent (column-collapse scenes occupy a small part of the domain, SURVEY §8e)."""
+    hist = np.asarray(hist, np.float64)
+    n_layers = len(hist)
     cum = np.cumsum(hist)
     total = cum[-1] if len(cum) else 0.0
     cuts = [0]
@@ -45,6 +49,11 @@ def slab_partition(tile_z, n_layers, world):
         cuts.append(z)
     cuts.append(n_layers)
     return [(cuts[r], cuts[r + 1]) for r in range(world)]
+
+
+def slab_partition(tile_z, n_layers, world):
+    """partition_counts of the histogram of tile_z (the tile layer of every particle)."""
+    return partition_counts(layer_histogram(tile_z, n_layers), world)
 
 
 class EngineAdapter:
@@ -247,3 +256,47 @@ def connect_peers(engine, rank, world, dist):
         if rank < world - 1:
             engine.xchg_connect(k, 1, handle=everyone[rank + 1][(k, 0)])   # my face 1 -> upper neighbour's face-0 buffer
     dist.barrier()
+
+
+def rebalance(engine, rank, world, dist, cuts=None):
+    """Re-cuts a z-slab run between substeps (every rank calls it at the same substep boundary): the cuts balance the run's
+    particle histogram again (partition_counts of the layer counts summed over the ranks), or are `cuts` ([(z0, z1)] per
+    rank) when given, and the particles move to their new owner ranks with their ids and state.  Returns (old_cuts,
+    new_cuts, rows_moved over all ranks); unchanged cuts move nothing.
+
+    The bytes go through dist.all_to_all_single on device buffers (NCCL) rather than the ring neighbours' peer mappings: a
+    re-cut is rare and may send particles to any rank.  Configured capacities are checked on every rank before any rank
+    changes; if one is too small, every rank raises SlabEditError and nothing changes."""
+    import torch
+    from .capi import RECORD_BYTES
+    dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend() == "nccl" else torch.device("cpu")
+    mine = np.asarray(engine.layer_counts(), np.int64)
+    hist = torch.as_tensor(mine, device=dev)
+    dist.all_reduce(hist)
+    ranges = [None] * world
+    dist.all_gather_object(ranges, tuple(engine.tile_range()))
+    old = [tuple(int(z) for z in r) for r in ranges]
+    new = partition_counts(hist.cpu().numpy(), world) if cuts is None else [(int(a), int(b)) for a, b in cuts]
+    if new == old:
+        return old, new, 0
+    flat = [new[0][0]] + [z1 for _, z1 in new]
+    z0, z1 = new[rank]
+    send_n = np.asarray(engine.recut_pack(flat), np.int64)   # per destination rank
+    recv_t = torch.empty(world, dtype=torch.int64, device=dev)
+    dist.all_to_all_single(recv_t, torch.as_tensor(send_n, device=dev))
+    recv_n = recv_t.cpu().numpy()
+    n_in = int(recv_n.sum())
+
+    def capacity_check():
+        need, cap = int(mine[z0:z1].sum()) + n_in, int(engine.cfg.capacity)
+        if cap > 0 and need > cap:
+            raise SlabEditError("rank %d: %d particles after the re-cut exceed its configured capacity %d" % (rank, need, cap))
+        return int(send_n.sum())
+
+    moved = _on_all_ranks(capacity_check, dist, "SUM")
+    send = torch.empty(int(send_n.sum()) * RECORD_BYTES, dtype=torch.uint8, device=dev)
+    engine.recut_pack(flat, send)
+    recv = torch.empty(n_in * RECORD_BYTES, dtype=torch.uint8, device=dev)
+    dist.all_to_all_single(recv, send, [int(c) * RECORD_BYTES for c in recv_n], [int(c) * RECORD_BYTES for c in send_n])
+    _on_all_ranks(lambda: engine.recut_apply(z0, z1, recv, n_in) or 0, dist, "SUM")
+    return old, new, moved
