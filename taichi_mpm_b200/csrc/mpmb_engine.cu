@@ -2698,6 +2698,59 @@ __global__ void k_async_route(const int *rowk, int ng, const int *flags, const i
 // =====================================================================================
 using namespace mpmb;
 
+// One device allocation of n elements of T, owned: freed by the destructor or by the next allocation.  Move-only, so every
+// address has exactly one owner; kernels and their argument structs get the raw pointer (get()), never the buffer.
+template <class T>
+class DevBuf {
+ public:
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  DevBuf(DevBuf &&o) noexcept : p_(o.p_), n_(o.n_) { o.p_ = nullptr; o.n_ = 0; }
+  DevBuf &operator=(DevBuf &&o) noexcept {   // frees what this buffer held
+    if (this != &o) {
+      reset();
+      p_ = o.p_; n_ = o.n_;
+      o.p_ = nullptr; o.n_ = 0;
+    }
+    return *this;
+  }
+  ~DevBuf() { reset(); }
+  // exactly n elements, content undefined; the old allocation is freed first, so after a failure the buffer is empty
+  cudaError_t alloc(size_t n) {
+    reset();
+    cudaError_t e = cudaMalloc(&p_, sizeof(T) * n);
+    if (e != cudaSuccess) p_ = nullptr;
+    else n_ = n;
+    return e;
+  }
+  // at least n elements: a smaller buffer is replaced by one of exactly n, its content discarded
+  cudaError_t reserve(size_t n) { return n <= n_ ? cudaSuccess : alloc(n); }
+  void reset() {
+    if (p_) cudaFree(p_);
+    p_ = nullptr;
+    n_ = 0;
+  }
+  T *get() const { return p_; }
+  size_t size() const { return n_; }
+
+ private:
+  T *p_ = nullptr;
+  size_t n_ = 0;
+};
+
+// fields of `cap` records laid out one after another in one allocation of AREC_WORDS * cap words
+static ARec arec_layout(float *w, int64_t cap) {
+  const size_t c = (size_t)cap;
+  ARec r;
+  r.x = w; r.v = w + 3 * c; r.F = w + 6 * c; r.b = w + 15 * c; r.mass = w + 24 * c; r.vol = w + 25 * c; r.scalar = w + 26 * c;
+  r.group = (int *)(w + 27 * c); r.id = (uint32_t *)(w + 28 * c); r.block = (int *)(w + 29 * c);
+  return r;
+}
+// a buffer of whole records and the layout of its records
+static int64_t arec_cap(const DevBuf<float> &buf) { return (int64_t)(buf.size() / AREC_WORDS); }
+static ARec arec_of(const DevBuf<float> &buf) { return arec_layout(buf.get(), arec_cap(buf)); }
+
 struct MpmbEngine {
   MpmbConfig cfg{};
   Params P{};
@@ -2710,53 +2763,49 @@ struct MpmbEngine {
   int ord = 0;           // which (run,stay) set is current
   int mov = 0;           // which mover list the next ordering consumes
   bool fresh = false;    // storage was just uploaded: arrival lists come from the radix sort
-  float4 *q[2][N_Q] = {};
-  uint32_t *keys[2] = {};       // tile of every row (cur / next)
-  uint32_t *outpos = nullptr;
-  uint32_t *mover_dst[2] = {}, *mover_idx[2] = {};
-  uint32_t *arrivals = nullptr, *arrivals_sorted = nullptr;
-  uint32_t *keys_sorted = nullptr, *iota = nullptr;  // upload-time radix sort scratch
+  DevBuf<float4> q[2][N_Q];
+  DevBuf<uint32_t> keys[2];       // tile of every row (cur / next)
+  DevBuf<uint32_t> outpos;
+  DevBuf<uint32_t> mover_dst[2], mover_idx[2];
+  DevBuf<uint32_t> arrivals, arrivals_sorted;
+  DevBuf<uint32_t> keys_sorted, iota;  // upload-time radix sort scratch
   uint32_t special_min = 0, key_dead = 0;
-  void *cub_temp = nullptr;
-  size_t cub_bytes = 0;
+  DevBuf<unsigned char> cub_temp;
   int key_bits = 32;
 
   int cap_tiles = 0;
   int ntot = 0;           // tiles of the dense tile grid
   int ord_blocks = 0;
-  int *run_begin[2] = {}, *run_len[2] = {}, *stay[2] = {};  // [ord]: current / next
-  int *arr_cnt = nullptr, *arr_off = nullptr, *arr_len = nullptr, *arr_cur = nullptr, *slot_map = nullptr, *blocksum = nullptr;
-  TileMeta *meta = nullptr;
-  float4 *arena = nullptr;
-  float4 *vel = nullptr;  // node velocities per active tile (k_grid -> k_g2p)
-  float4 *sdf4 = nullptr;
-  Counters *cnt = nullptr;
+  DevBuf<int> run_begin[2], run_len[2], stay[2];  // [ord]: current / next
+  DevBuf<int> arr_cnt, arr_off, arr_len, arr_cur, slot_map, blocksum;
+  DevBuf<TileMeta> meta;
+  DevBuf<float4> arena;
+  DevBuf<float4> vel;  // node velocities per active tile (k_grid -> k_g2p)
+  DevBuf<float4> sdf4;
+  DevBuf<Counters> cnt;
 
   int stage = 0;  // 0 idle/after resample, 1 after sort, 2 after rasterize
   int64_t mig_cap = 0;
   // peer-memory exchange: rx = my receive buffers [kind 0 halo / 1 migration][face], tx = the
-  // neighbour's receive buffer I write into through face f (mapped by IPC or same-process pointer)
-  char *rx[2][2] = {}, *tx[2][2] = {};
+  // neighbour's receive buffer I write into through face f
+  DevBuf<char> rx[2][2];
+  char *tx[2][2] = {};    // not owned: the neighbour's rx, mapped by IPC (closed by mpmb_destroy) or given by the same process
   bool tx_ipc[2][2] = {};
-  int *xcount = nullptr;  // local pack counters (int4 per [kind][face])
+  DevBuf<int> xcount;     // local pack counters (int4 per [kind][face])
   int xstep = 0;          // substeps completed since the peers were connected
   bool skip_b = false;        // intermediate substeps of mpmb_substep do not store apic_b
-  void *stage_buf = nullptr;  // cached staging buffer of the host<->device marshalling
-  size_t stage_bytes = 0;
+  DevBuf<unsigned char> stage_buf;  // cached staging buffer of the host<->device marshalling
   // device image of the reference's AoS pool + index vector, kept from mpmb_upload_aos to mpmb_download_aos
-  unsigned char *aos_pool = nullptr;
-  uint32_t *aos_idx = nullptr;
-  size_t aos_pool_bytes = 0, aos_idx_cap = 0;
-  const void *aos_host_pool = nullptr;  // identity of the image: host pool pointer, slots and particle count
+  DevBuf<unsigned char> aos_pool;
+  DevBuf<uint32_t> aos_idx;
+  const void *aos_host_pool = nullptr;  // not owned: the host pool, kept only to identify the image (with slots and particle count)
   int64_t aos_slots = 0, aos_n = 0;
-  int *scan_a = nullptr, *scan_b = nullptr;  // flags / prefix scratch (downloads, seeding)
-  size_t scan_cap = 0;
-  void *scan_tmp = nullptr;
-  size_t scan_tmp_bytes = 0;
+  DevBuf<int> scan_a, scan_b;  // flags / prefix scratch (downloads, seeding)
+  DevBuf<unsigned char> scan_tmp;
   uint32_t id_base = 0;
   int num_sms = 132;  // H100 SXM; queried from the device in mpmb_create
   int nt2_global = 0;  // tile layers of the whole domain (P.nt[2] is slab-local)
-  unsigned long long *recut_buf = nullptr;  // re-cut scratch: layer histogram [nt2_global], then two ints (bad arrivals, largest id)
+  DevBuf<unsigned long long> recut_buf;  // re-cut scratch: layer histogram [nt2_global], then two ints (bad arrivals, largest id)
   int grid_p2g = 132 * 4, grid_g2p = 132 * 4;  // persistent grids = SMs x resident CTAs (queried)
   int64_t launches = 0;
 
@@ -2767,23 +2816,33 @@ struct MpmbEngine {
   cudaStream_t cap_stream = nullptr;
   bool use_graph = true;
 
-  // CPIC rigid coupling (enabled by mpmb_set_rigid_samples with at least one sample)
-  RigidView R{};
+  // CPIC rigid coupling (enabled by mpmb_set_rigid_samples with at least one sample); rigid_view() hands it to the kernels
   bool rigid_on = false;
-  float *rs_offset = nullptr, *rs_tri = nullptr;
-  int *rs_rigid = nullptr;
-  size_t rigid_nodes = 0;
-  // bodies advanced on the device (mpmb_set_rigid_motion): master states, script table, contacts
+  int rigid_bodies = 0, rigid_samples = 0;
+  int rigid_nb[3] = {};                // rigid_page_map blocks (4x4x8 nodes) per axis
+  float penalty = 0.f, pushing_force = 0.f;
+  DevBuf<RigidDev> bodies;             // [RIGID_MAX]
+  DevBuf<float> rs_offset, rs_tri;     // boundary samples
+  DevBuf<int> rs_rigid, s_base;
+  DevBuf<unsigned long long> node_key; // colour field of the whole node grid
+  DevBuf<uint32_t> node_tags;
+  DevBuf<unsigned char> page, tile_flag;
+  DevBuf<uint32_t> p_states;           // by particle id - id_base: its size is the number of ids tracked
+  DevBuf<float4> p_cdf;
+  DevBuf<uint32_t> p_mark;
+  DevBuf<uint32_t> epoch;
+  // bodies advanced on the device (mpmb_set_rigid_motion): master states, script table, contacts; motion_view() for the kernels
   bool motion_on = false;
   bool motion_scripted = false;        // some body follows the script table
   bool motion_collide = false;         // the level-set collision was asked for (it runs while a level set is set)
-  MotionView M{};
   RigidMaster h_master[RIGID_MAX] = {};  // host image: motion parameters (+ the state last written by the host)
-  double *script = nullptr;
-  size_t script_cap = 0;               // doubles
+  DevBuf<RigidMaster> master;          // [RIGID_MAX]
+  DevBuf<int> cursor;                  // next script entry
+  DevBuf<double> script;               // grow-only: its size is the capacity in doubles
   int64_t script_left = 0;             // entries not yet consumed (host-side count of the device cursor)
-  int *s_order = nullptr;
-  double *contact = nullptr;
+  DevBuf<int> s_order;                 // sample indices grouped by body; body b owns s_order[s_begin[b] .. s_begin[b + 1])
+  int s_begin[RIGID_MAX + 1] = {};
+  DevBuf<double> contact;
   int64_t id_span_pending = 0;
   int64_t id_span = 0;   // ids of the resident particles lie in [id_base, id_base + id_span): uploads number 0..n-1, the seeded
                          // lattice numbers by lattice index (gaps where the boundary band is skipped)
@@ -2792,31 +2851,27 @@ struct MpmbEngine {
 
   // AsyncMPM pools (mpmb_async_*): [0] particle_pool, [1] backup_pool, each double-buffered for the stable edits
   struct APool {
-    void *buf[2] = {};
-    ARec r[2] = {};
+    DevBuf<float> buf[2];   // record layout (arec_of), both of the same capacity
     int cur = 0;
-    int64_t n = 0, cap = 0;
+    int64_t n = 0;
+    ARec rec(int b) const { return arec_of(buf[b]); }
   };
   bool async_on = false;
   int anb[3] = {};
   int nblk = 0;
   float a_inv_dx = 0.f;
   APool apool[2];
-  uint8_t *a_bfl = nullptr;                                         // [nblk] MPMB_ASYNC_* flags of the current advance
-  uint32_t *a_bflag = nullptr;                                      // [nblk] block reductions of mpmb_async_block_limits
-  int *a_bmin = nullptr, *a_bmax = nullptr;
-  int *a_blk = nullptr;                                             // [nblk] compacted block list
-  float *a_lim = nullptr;                                           // [2 nblk] compacted min_dt, max_v2
-  int *a_bad = nullptr;
-  void *a_gbuf = nullptr, *a_sbuf = nullptr;                        // gathered set / survivors (record layout)
-  ARec a_G{}, a_S{};
-  int64_t a_gcap = 0, a_scap = 0;
-  unsigned long long *a_key[2] = {};                                // gather: candidate keys, candidate / id / position lists
-  uint32_t *a_u[4] = {};
-  int *a_rowk = nullptr;
-  int64_t a_ccap = 0;
-  void *a_cub = nullptr;
-  size_t a_cub_bytes = 0;
+  DevBuf<uint8_t> a_bfl;                                            // [nblk] MPMB_ASYNC_* flags of the current advance
+  DevBuf<uint32_t> a_bflag;                                         // [nblk] block reductions of mpmb_async_block_limits
+  DevBuf<int> a_bmin, a_bmax;
+  DevBuf<int> a_blk;                                                // [nblk] compacted block list
+  DevBuf<float> a_lim;                                              // [2 nblk] compacted min_dt, max_v2
+  DevBuf<int> a_bad;
+  DevBuf<float> a_gbuf, a_sbuf;                                     // gathered set / survivors (record layout)
+  DevBuf<unsigned long long> a_key[2];                              // gather: candidate keys, candidate / id / position lists
+  DevBuf<uint32_t> a_u[4];
+  DevBuf<int> a_rowk;                                               // its size is the candidate capacity
+  DevBuf<unsigned char> a_cub;
 
   bool profiling = false;
   struct Ev { cudaEvent_t a, b; int stage; };
@@ -2827,32 +2882,6 @@ struct MpmbEngine {
 };
 
 static thread_local std::string g_create_error;
-
-// fields of `cap` records laid out one after another in one allocation of AREC_WORDS * cap words
-static ARec arec_layout(void *buf, int64_t cap) {
-  float *w = (float *)buf;
-  const size_t c = (size_t)cap;
-  ARec r;
-  r.x = w; r.v = w + 3 * c; r.F = w + 6 * c; r.b = w + 15 * c; r.mass = w + 24 * c; r.vol = w + 25 * c; r.scalar = w + 26 * c;
-  r.group = (int *)(w + 27 * c); r.id = (uint32_t *)(w + 28 * c); r.block = (int *)(w + 29 * c);
-  return r;
-}
-
-static void async_free(MpmbEngine *h) {
-  for (auto &p : h->apool) {
-    for (int b = 0; b < 2; b++) { cudaFree(p.buf[b]); p.buf[b] = nullptr; }
-    p.n = p.cap = 0;
-    p.cur = 0;
-  }
-  cudaFree(h->a_bfl); cudaFree(h->a_bflag); cudaFree(h->a_bmin); cudaFree(h->a_bmax); cudaFree(h->a_blk); cudaFree(h->a_lim); cudaFree(h->a_bad);
-  cudaFree(h->a_gbuf); cudaFree(h->a_sbuf); cudaFree(h->a_key[0]); cudaFree(h->a_key[1]); cudaFree(h->a_rowk); cudaFree(h->a_cub);
-  for (auto &u : h->a_u) { cudaFree(u); u = nullptr; }
-  h->a_bfl = nullptr; h->a_bflag = nullptr; h->a_bmin = h->a_bmax = nullptr; h->a_blk = nullptr; h->a_lim = nullptr; h->a_bad = nullptr;
-  h->a_gbuf = h->a_sbuf = nullptr; h->a_key[0] = h->a_key[1] = nullptr; h->a_rowk = nullptr; h->a_cub = nullptr;
-  h->a_gcap = h->a_scap = h->a_ccap = 0;
-  h->a_cub_bytes = 0;
-  h->async_on = false;
-}
 
 static int fail(MpmbEngine *h, int code, const char *fmt, ...) {
   char buf[512];
@@ -2890,38 +2919,71 @@ static void graph_reset(MpmbEngine *h) {
 static View make_view(MpmbEngine *h) {
   View V{};
   for (int k = 0; k < N_Q; k++) {
-    V.q[k] = h->q[h->cur][k];
-    V.qn[k] = h->q[h->cur ^ 1][k];
+    V.q[k] = h->q[h->cur][k].get();
+    V.qn[k] = h->q[h->cur ^ 1][k].get();
   }
-  V.keys = h->keys[h->cur];
-  V.keys_next = h->keys[h->cur ^ 1];
-  V.outpos = h->outpos;
-  V.run_begin = h->run_begin[h->ord];
-  V.run_len = h->run_len[h->ord];
-  V.out_begin = h->run_begin[h->ord ^ 1];
-  V.total = h->run_len[h->ord ^ 1];
-  V.stay_cnt = h->stay[h->ord];
-  V.stay_next = h->stay[h->ord ^ 1];
-  V.arr_cnt = h->arr_cnt;
-  V.arr_off = h->arr_off;
-  V.arr_len = h->arr_len;
-  V.arr_cur = h->arr_cur;
-  V.slot_map = h->slot_map;
-  V.meta = h->meta;
-  V.mover_dst = h->mover_dst[h->mov];
-  V.mover_idx = h->mover_idx[h->mov];
-  V.mover_dst_n = h->mover_dst[h->mov ^ 1];
-  V.mover_idx_n = h->mover_idx[h->mov ^ 1];
-  V.arrivals = h->arrivals;
-  V.arrivals_sorted = h->arrivals_sorted;
-  V.blocksum = h->blocksum;
-  V.arena = h->arena;
-  V.sdf4 = h->sdf4;
-  V.cnt = h->cnt;
+  V.keys = h->keys[h->cur].get();
+  V.keys_next = h->keys[h->cur ^ 1].get();
+  V.outpos = h->outpos.get();
+  V.run_begin = h->run_begin[h->ord].get();
+  V.run_len = h->run_len[h->ord].get();
+  V.out_begin = h->run_begin[h->ord ^ 1].get();
+  V.total = h->run_len[h->ord ^ 1].get();
+  V.stay_cnt = h->stay[h->ord].get();
+  V.stay_next = h->stay[h->ord ^ 1].get();
+  V.arr_cnt = h->arr_cnt.get();
+  V.arr_off = h->arr_off.get();
+  V.arr_len = h->arr_len.get();
+  V.arr_cur = h->arr_cur.get();
+  V.slot_map = h->slot_map.get();
+  V.meta = h->meta.get();
+  V.mover_dst = h->mover_dst[h->mov].get();
+  V.mover_idx = h->mover_idx[h->mov].get();
+  V.mover_dst_n = h->mover_dst[h->mov ^ 1].get();
+  V.mover_idx_n = h->mover_idx[h->mov ^ 1].get();
+  V.arrivals = h->arrivals.get();
+  V.arrivals_sorted = h->arrivals_sorted.get();
+  V.blocksum = h->blocksum.get();
+  V.arena = h->arena.get();
+  V.sdf4 = h->sdf4.get();
+  V.cnt = h->cnt.get();
   V.cap_tiles = h->cap_tiles;
   V.cap_particles = (int)h->cap;
-  V.rigid_flag = h->rigid_on ? h->R.tile_flag : nullptr;
+  V.rigid_flag = h->rigid_on ? h->tile_flag.get() : nullptr;
   return V;
+}
+
+// the rigid coupling and the device-advanced bodies as the kernels take them, built at every launch as make_view is
+static RigidView rigid_view(MpmbEngine *h) {
+  RigidView R{};
+  R.bodies = h->bodies.get();
+  R.n_bodies = h->rigid_bodies;
+  R.n_samples = h->rigid_samples;
+  R.s_offset = h->rs_offset.get(); R.s_tri = h->rs_tri.get(); R.s_rigid = h->rs_rigid.get();
+  R.s_base = h->s_base.get();
+  R.node_key = h->node_key.get();
+  R.node_tags = h->node_tags.get();
+  R.page = h->page.get();
+  for (int d = 0; d < 3; d++) R.nb[d] = h->rigid_nb[d];
+  R.tile_flag = h->tile_flag.get();
+  R.p_states = h->p_states.get(); R.p_cdf = h->p_cdf.get(); R.p_mark = h->p_mark.get();
+  R.epoch = h->epoch.get();
+  R.id_base = h->id_base;
+  R.id_cap = (int)h->p_states.size();
+  R.penalty = h->penalty;
+  R.pushing_force = h->pushing_force;
+  return R;
+}
+static MotionView motion_view(MpmbEngine *h) {
+  MotionView M{};
+  M.m = h->master.get();
+  M.script = h->script.get();
+  M.cursor = h->cursor.get();
+  M.s_order = h->s_order.get();
+  for (int b = 0; b <= RIGID_MAX; b++) M.s_begin[b] = h->s_begin[b];
+  M.contact = h->contact.get();
+  M.collide = h->motion_collide && h->P.has_sdf;   // without a level set there are no contacts: the advance must not read the buffer
+  return M;                                        // (changing the level set resets the captured graphs)
 }
 
 static void prof_begin(MpmbEngine *h, int stage) {
@@ -2951,40 +3013,32 @@ static void prof_collect(MpmbEngine *h) {
   h->events_used = 0;
 }
 
-static int free_particles(MpmbEngine *h) {
+// Frees every particle-row buffer, then allocates them for `cap` rows: a reallocation never holds the old and the new set.
+static int alloc_particles(MpmbEngine *h, int64_t cap) {
   graph_reset(h);
   for (int b = 0; b < 2; b++) {
-    for (int k = 0; k < N_Q; k++) { cudaFree(h->q[b][k]); h->q[b][k] = nullptr; }
-    cudaFree(h->keys[b]); h->keys[b] = nullptr;
-    cudaFree(h->mover_dst[b]); cudaFree(h->mover_idx[b]);
-    h->mover_dst[b] = h->mover_idx[b] = nullptr;
+    for (auto &q : h->q[b]) q.reset();
+    h->keys[b].reset(); h->mover_dst[b].reset(); h->mover_idx[b].reset();
   }
-  cudaFree(h->outpos); cudaFree(h->arrivals); cudaFree(h->arrivals_sorted); cudaFree(h->keys_sorted); cudaFree(h->iota); cudaFree(h->cub_temp);
-  h->outpos = h->arrivals = h->arrivals_sorted = h->keys_sorted = h->iota = nullptr;
-  h->cub_temp = nullptr;
+  h->outpos.reset(); h->arrivals.reset(); h->arrivals_sorted.reset(); h->keys_sorted.reset(); h->iota.reset(); h->cub_temp.reset();
   h->cap = 0;
-  return 0;
-}
-
-static int alloc_particles(MpmbEngine *h, int64_t cap) {
-  free_particles(h);
   if (cap >= (1ll << 30)) return fail(h, MPMB_ERR_CAPACITY, "capacity %lld exceeds 2^30 particle rows per GPU", (long long)cap);
   if (cap < 1) cap = 1;
   for (int b = 0; b < 2; b++) {
-    for (int k = 0; k < N_Q; k++) CUDA_TRY(h, cudaMalloc(&h->q[b][k], sizeof(float4) * cap));
-    CUDA_TRY(h, cudaMalloc(&h->keys[b], sizeof(uint32_t) * cap));
-    CUDA_TRY(h, cudaMalloc(&h->mover_dst[b], sizeof(uint32_t) * cap));
-    CUDA_TRY(h, cudaMalloc(&h->mover_idx[b], sizeof(uint32_t) * cap));
+    for (auto &q : h->q[b]) CUDA_TRY(h, q.alloc(cap));
+    CUDA_TRY(h, h->keys[b].alloc(cap));
+    CUDA_TRY(h, h->mover_dst[b].alloc(cap));
+    CUDA_TRY(h, h->mover_idx[b].alloc(cap));
   }
-  CUDA_TRY(h, cudaMalloc(&h->outpos, sizeof(uint32_t) * (cap + 8)));  // the bulk copy of a run's words is widened to 16-byte bounds
-  CUDA_TRY(h, cudaMalloc(&h->arrivals, sizeof(uint32_t) * cap));
-  CUDA_TRY(h, cudaMalloc(&h->arrivals_sorted, sizeof(uint32_t) * cap));
-  CUDA_TRY(h, cudaMalloc(&h->keys_sorted, sizeof(uint32_t) * cap));
-  CUDA_TRY(h, cudaMalloc(&h->iota, sizeof(uint32_t) * cap));
-  k_iota<<<(unsigned)((cap + 255) / 256), 256, 0, h->stream>>>(h->iota, (int)cap);
-  h->cub_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, h->cub_bytes, h->keys[0], h->keys_sorted, h->iota, h->arrivals_sorted, (int)cap, 0, 32, h->stream);
-  CUDA_TRY(h, cudaMalloc(&h->cub_temp, h->cub_bytes));
+  CUDA_TRY(h, h->outpos.alloc(cap + 8));  // the bulk copy of a run's words is widened to 16-byte bounds
+  CUDA_TRY(h, h->arrivals.alloc(cap));
+  CUDA_TRY(h, h->arrivals_sorted.alloc(cap));
+  CUDA_TRY(h, h->keys_sorted.alloc(cap));
+  CUDA_TRY(h, h->iota.alloc(cap));
+  k_iota<<<(unsigned)((cap + 255) / 256), 256, 0, h->stream>>>(h->iota.get(), (int)cap);
+  size_t cub_bytes = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, h->keys[0].get(), h->keys_sorted.get(), h->iota.get(), h->arrivals_sorted.get(), (int)cap, 0, 32, h->stream);
+  CUDA_TRY(h, h->cub_temp.alloc(cub_bytes));
   h->cap = cap;
   return MPMB_OK;
 }
@@ -3024,30 +3078,24 @@ static void set_slicing(MpmbEngine *h, const Slicing &s) {
 // slot), node velocities and the ordering's block sums for `cap_tiles` tiles.  All or nothing: on failure the engine keeps
 // the arrays it had.
 static int alloc_tile_arrays(MpmbEngine *h, int64_t cap_tiles) {
-  int *dense[11] = {}, *blocksum = nullptr;
-  TileMeta *meta = nullptr;
-  float4 *arena = nullptr, *vel = nullptr;
+  DevBuf<int> dense[11], blocksum;
+  DevBuf<TileMeta> meta;
+  DevBuf<float4> arena, vel;
   const int64_t blocks = (cap_tiles + ORD_TILE - 1) / ORD_TILE;
   bool ok = true;
-  for (int *&p : dense) ok = ok && cudaMalloc(&p, sizeof(int) * cap_tiles) == cudaSuccess;
-  ok = ok && cudaMalloc(&blocksum, sizeof(int) * 3 * (blocks + 1)) == cudaSuccess;
-  ok = ok && cudaMalloc(&meta, sizeof(TileMeta) * cap_tiles) == cudaSuccess;
-  ok = ok && cudaMalloc(&arena, sizeof(float4) * ARENA * (cap_tiles + 1)) == cudaSuccess;
-  ok = ok && cudaMalloc(&vel, sizeof(float4) * ARENA * cap_tiles) == cudaSuccess;
-  if (!ok) {
-    const std::string msg = cudaGetErrorString(cudaGetLastError());
-    for (int *p : dense) cudaFree(p);
-    cudaFree(blocksum); cudaFree(meta); cudaFree(arena); cudaFree(vel);
-    return fail(h, MPMB_ERR_CUDA, "cudaMalloc of the tile arrays (%lld tiles): %s", (long long)cap_tiles, msg.c_str());
-  }
-  for (int *p : dense) cudaMemsetAsync(p, 0, sizeof(int) * cap_tiles, h->stream);
-  cudaMemsetAsync(arena + (size_t)ARENA * cap_tiles, 0, sizeof(float4) * ARENA, h->stream);
-  int **mine[] = {&h->run_begin[0], &h->run_begin[1], &h->run_len[0], &h->run_len[1], &h->stay[0], &h->stay[1],
-                  &h->arr_cnt, &h->arr_off, &h->arr_len, &h->arr_cur, &h->slot_map};
-  for (int k = 0; k < 11; k++) { cudaFree(*mine[k]); *mine[k] = dense[k]; }
-  cudaMemsetAsync(h->slot_map, 0xFF, sizeof(int) * cap_tiles, h->stream);
-  cudaFree(h->blocksum); cudaFree(h->meta); cudaFree(h->arena); cudaFree(h->vel);
-  h->blocksum = blocksum; h->meta = meta; h->arena = arena; h->vel = vel;
+  for (auto &d : dense) ok = ok && d.alloc(cap_tiles) == cudaSuccess;
+  ok = ok && blocksum.alloc(3 * (blocks + 1)) == cudaSuccess;
+  ok = ok && meta.alloc(cap_tiles) == cudaSuccess;
+  ok = ok && arena.alloc((size_t)ARENA * (cap_tiles + 1)) == cudaSuccess;
+  ok = ok && vel.alloc((size_t)ARENA * cap_tiles) == cudaSuccess;
+  if (!ok) return fail(h, MPMB_ERR_CUDA, "cudaMalloc of the tile arrays (%lld tiles): %s", (long long)cap_tiles, cudaGetErrorString(cudaGetLastError()));
+  for (auto &d : dense) cudaMemsetAsync(d.get(), 0, sizeof(int) * cap_tiles, h->stream);
+  cudaMemsetAsync(arena.get() + (size_t)ARENA * cap_tiles, 0, sizeof(float4) * ARENA, h->stream);
+  DevBuf<int> *mine[] = {&h->run_begin[0], &h->run_begin[1], &h->run_len[0], &h->run_len[1], &h->stay[0], &h->stay[1],
+                         &h->arr_cnt, &h->arr_off, &h->arr_len, &h->arr_cur, &h->slot_map};
+  for (int k = 0; k < 11; k++) *mine[k] = std::move(dense[k]);
+  cudaMemsetAsync(h->slot_map.get(), 0xFF, sizeof(int) * cap_tiles, h->stream);
+  h->blocksum = std::move(blocksum); h->meta = std::move(meta); h->arena = std::move(arena); h->vel = std::move(vel);
   h->cap_tiles = (int)cap_tiles;
   return MPMB_OK;
 }
@@ -3126,18 +3174,18 @@ int mpmb_create(const MpmbConfig *cfg, MpmbHandle *out) {
     mpmb_destroy(h);
     return MPMB_ERR_CUDA;
   }
-  if (cudaMalloc(&h->cnt, sizeof(Counters)) != cudaSuccess) return bail("cudaMalloc counters");
-  cudaMemset(h->cnt, 0, sizeof(Counters));
+  if (h->cnt.alloc(1) != cudaSuccess) return bail("cudaMalloc counters");
+  cudaMemset(h->cnt.get(), 0, sizeof(Counters));
   h->mig_cap = h->cfg.world > 1 ? (cfg->migrate_capacity > 0 ? cfg->migrate_capacity : 65536) : 0;
   if (h->cfg.world > 1) {
     const int64_t bytes[2] = {mpmb_halo_bytes(h), mpmb_migrate_bytes(h)};
     for (int k = 0; k < 2; k++)
       for (int f = 0; f < 2; f++) {
-        if (cudaMalloc(&h->rx[k][f], bytes[k]) != cudaSuccess) return bail("cudaMalloc exchange buffer");
-        cudaMemset(h->rx[k][f], 0, 16);
+        if (h->rx[k][f].alloc(bytes[k]) != cudaSuccess) return bail("cudaMalloc exchange buffer");
+        cudaMemset(h->rx[k][f].get(), 0, 16);
       }
-    if (cudaMalloc(&h->xcount, sizeof(int) * 32) != cudaSuccess) return bail("cudaMalloc exchange counters");
-    cudaMemset(h->xcount, 0, sizeof(int) * 32);  // [0],[4] halo counts, [8],[12] migration counts, [16],[20] finished-CTA counters
+    if (h->xcount.alloc(32) != cudaSuccess) return bail("cudaMalloc exchange counters");
+    cudaMemset(h->xcount.get(), 0, sizeof(int) * 32);  // [0],[4] halo counts, [8],[12] migration counts, [16],[20] finished-CTA counters
   }
   if (cfg->capacity > 0) {
     int rc = alloc_particles(h, cfg->capacity);
@@ -3151,25 +3199,13 @@ int mpmb_destroy(MpmbHandle h) {
   if (!h) return MPMB_OK;
   cudaSetDevice(h->cfg.device);
   cudaDeviceSynchronize();
-  free_particles(h);
-  for (int b = 0; b < 2; b++) { cudaFree(h->run_begin[b]); cudaFree(h->run_len[b]); cudaFree(h->stay[b]); }
-  cudaFree(h->arr_cnt); cudaFree(h->arr_off); cudaFree(h->arr_len); cudaFree(h->arr_cur); cudaFree(h->slot_map); cudaFree(h->blocksum);
-  cudaFree(h->meta);
-  cudaFree(h->arena); cudaFree(h->vel); cudaFree(h->sdf4); cudaFree(h->cnt); cudaFree(h->stage_buf); cudaFree(h->xcount);
-  cudaFree(h->aos_pool); cudaFree(h->aos_idx); cudaFree(h->scan_a); cudaFree(h->scan_b); cudaFree(h->scan_tmp); cudaFree(h->recut_buf);
+  // memory is freed by the buffers' destructors (with this device current); here go the handles that are not memory
   for (int k = 0; k < 2; k++)
-    for (int f = 0; f < 2; f++) {
+    for (int f = 0; f < 2; f++)
       if (h->tx_ipc[k][f] && h->tx[k][f]) cudaIpcCloseMemHandle(h->tx[k][f]);
-      cudaFree(h->rx[k][f]);
-    }
   for (auto &e : h->events) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
   graph_reset(h);
   if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
-  cudaFree(h->R.bodies); cudaFree(h->rs_offset); cudaFree(h->rs_tri); cudaFree(h->rs_rigid); cudaFree(h->R.s_base); cudaFree(h->R.node_key);
-  cudaFree(h->R.node_tags); cudaFree(h->R.page); cudaFree(h->R.tile_flag); cudaFree(h->R.p_states); cudaFree(h->R.p_cdf); cudaFree(h->R.p_mark);
-  cudaFree(h->R.epoch); cudaFree(h->M.m); cudaFree(h->M.cursor); cudaFree(h->s_order); cudaFree(h->contact); cudaFree(h->script);
-  async_free(h);
-
   delete h;
   return MPMB_OK;
 }
@@ -3184,7 +3220,7 @@ int mpmb_synchronize(MpmbHandle h) {
   CHECK_HANDLE(h);
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   Counters c;
-  CUDA_TRY(h, cudaMemcpy(&c, h->cnt, sizeof(c), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(&c, h->cnt.get(), sizeof(c), cudaMemcpyDeviceToHost));
   if (c.error & DEVERR_TILE_CAPACITY) return fail(h, MPMB_ERR_CAPACITY, "active tile capacity exceeded");
   if (c.error & DEVERR_MIGRATE_CAPACITY) return fail(h, MPMB_ERR_CAPACITY, "migration buffer capacity exceeded");
   if (c.error & DEVERR_PARTICLE_CAPACITY) return fail(h, MPMB_ERR_CAPACITY, "particle capacity exceeded");
@@ -3208,7 +3244,7 @@ int mpmb_set_material(MpmbHandle h, int32_t group, int32_t kind, const float *pa
     if (rc != MPMB_OK) return rc;
     if (ns > 0) {
       View V = make_view(h);
-      k_refresh_affine<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, h->P, h->keys[h->cur], ns, h->special_min, group);
+      k_refresh_affine<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, h->P, h->keys[h->cur].get(), ns, h->special_min, group);
       h->launches++;
       CUDA_TRY(h, cudaGetLastError());
     }
@@ -3239,7 +3275,7 @@ int mpmb_set_delta_t(MpmbHandle h, float dt) {
     if (ns > 0) {
       View V = make_view(h);
       for (int g = 0; g < MPMB_MAX_GROUPS; g++) {
-        k_refresh_affine<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, h->P, h->keys[h->cur], ns, h->special_min, g);
+        k_refresh_affine<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, h->P, h->keys[h->cur].get(), ns, h->special_min, g);
         h->launches++;
       }
       CUDA_TRY(h, cudaGetLastError());
@@ -3264,8 +3300,8 @@ int mpmb_set_sdf(MpmbHandle h, const float *sdf4, float friction) {
     graph_reset(h);
     return MPMB_OK;
   }
-  if (!h->sdf4) CUDA_TRY(h, cudaMalloc(&h->sdf4, sizeof(float4) * n));
-  CUDA_TRY(h, cudaMemcpyAsync(h->sdf4, sdf4, sizeof(float4) * n, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, h->sdf4.reserve(n));
+  CUDA_TRY(h, cudaMemcpyAsync(h->sdf4.get(), sdf4, sizeof(float4) * n, cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   h->P.has_sdf = 1;
   h->P.friction = friction;
@@ -3277,14 +3313,13 @@ int mpmb_set_planes(MpmbHandle h, int32_t n_planes, const float *planes4, float 
   CHECK_HANDLE(h);
   if (n_planes <= 0 || n_planes > 64 || !planes4) return fail(h, MPMB_ERR_INVALID, "need 1..64 planes");
   size_t n = (size_t)h->P.nnode[0] * h->P.nnode[1] * h->P.nnode[2];
-  if (!h->sdf4) CUDA_TRY(h, cudaMalloc(&h->sdf4, sizeof(float4) * n));
-  float4 *d_planes = nullptr;
-  CUDA_TRY(h, cudaMalloc(&d_planes, sizeof(float4) * n_planes));
-  CUDA_TRY(h, cudaMemcpyAsync(d_planes, planes4, sizeof(float4) * n_planes, cudaMemcpyHostToDevice, h->stream));
-  k_planes_to_sdf<<<h->num_sms * 8, 256, 0, h->stream>>>(h->P, n_planes, d_planes, h->sdf4);
+  CUDA_TRY(h, h->sdf4.reserve(n));
+  DevBuf<float4> d_planes;
+  CUDA_TRY(h, d_planes.alloc(n_planes));
+  CUDA_TRY(h, cudaMemcpyAsync(d_planes.get(), planes4, sizeof(float4) * n_planes, cudaMemcpyHostToDevice, h->stream));
+  k_planes_to_sdf<<<h->num_sms * 8, 256, 0, h->stream>>>(h->P, n_planes, d_planes.get(), h->sdf4.get());
   h->launches++;
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  cudaFree(d_planes);
   h->P.has_sdf = 1;
   h->P.friction = friction;
   graph_reset(h);
@@ -3297,15 +3332,13 @@ int mpmb_set_levelset_shapes(MpmbHandle h, int32_t n_shapes, const MpmbShape *sh
   for (int k = 0; k < n_shapes; k++)
     if (shapes[k].kind < MPMB_SHAPE_PLANE || shapes[k].kind > MPMB_SHAPE_CUBOID) return fail(h, MPMB_ERR_INVALID, "unknown shape kind %d", shapes[k].kind);
   size_t n = (size_t)h->P.nnode[0] * h->P.nnode[1] * h->P.nnode[2];
-  if (!h->sdf4) CUDA_TRY(h, cudaMalloc(&h->sdf4, sizeof(float4) * n));
-  MpmbShape *d_shapes = nullptr;
-  CUDA_TRY(h, cudaMalloc(&d_shapes, sizeof(MpmbShape) * n_shapes));
-  CUDA_TRY(h, cudaMemcpyAsync(d_shapes, shapes, sizeof(MpmbShape) * n_shapes, cudaMemcpyHostToDevice, h->stream));
-  k_shapes_to_sdf<<<h->num_sms * 8, 256, 0, h->stream>>>(h->P, n_shapes, d_shapes, h->sdf4);
+  CUDA_TRY(h, h->sdf4.reserve(n));
+  DevBuf<MpmbShape> d_shapes;
+  CUDA_TRY(h, d_shapes.alloc(n_shapes));
+  CUDA_TRY(h, cudaMemcpyAsync(d_shapes.get(), shapes, sizeof(MpmbShape) * n_shapes, cudaMemcpyHostToDevice, h->stream));
+  k_shapes_to_sdf<<<h->num_sms * 8, 256, 0, h->stream>>>(h->P, n_shapes, d_shapes.get(), h->sdf4.get());
   h->launches++;
-  cudaError_t e = cudaStreamSynchronize(h->stream);
-  cudaFree(d_shapes);
-  CUDA_TRY(h, e);
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   h->P.has_sdf = 1;
   h->P.friction = friction;
   graph_reset(h);
@@ -3335,19 +3368,16 @@ static int grow_keeping_rows(MpmbEngine *h, int64_t need, int n_keep) {
   const int64_t room = h->cfg.world > 1 ? need + need / 4 + 16 * h->mig_cap : need;
   if (room <= h->cap) return MPMB_OK;
   const int64_t want = std::max<int64_t>(room, std::min<int64_t>(h->cap + h->cap / 2, (1ll << 30) - 1));
-  float4 *old_q[N_Q];
-  uint32_t *old_keys = h->keys[h->cur];
-  for (int k = 0; k < N_Q; k++) { old_q[k] = h->q[h->cur][k]; h->q[h->cur][k] = nullptr; }
-  h->keys[h->cur] = nullptr;
+  DevBuf<float4> old_q[N_Q];   // the current rows survive the reallocation here
+  for (int k = 0; k < N_Q; k++) old_q[k] = std::move(h->q[h->cur][k]);
+  DevBuf<uint32_t> old_keys = std::move(h->keys[h->cur]);
   int rc = alloc_particles(h, want);   // frees everything else (scratch, the other buffer) and resets the graphs
   if (rc == MPMB_OK && n_keep > 0) {
     for (int k = 0; k < N_Q; k++)
-      CUDA_TRY(h, cudaMemcpyAsync(h->q[h->cur][k], old_q[k], sizeof(float4) * n_keep, cudaMemcpyDeviceToDevice, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(h->keys[h->cur], old_keys, sizeof(uint32_t) * n_keep, cudaMemcpyDeviceToDevice, h->stream));
+      CUDA_TRY(h, cudaMemcpyAsync(h->q[h->cur][k].get(), old_q[k].get(), sizeof(float4) * n_keep, cudaMemcpyDeviceToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->keys[h->cur].get(), old_keys.get(), sizeof(uint32_t) * n_keep, cudaMemcpyDeviceToDevice, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   }
-  for (int k = 0; k < N_Q; k++) cudaFree(old_q[k]);
-  cudaFree(old_keys);
   return rc;
 }
 
@@ -3357,17 +3387,18 @@ static int grow_keeping_rows(MpmbEngine *h, int64_t need, int n_keep) {
 static int reorder_from_scratch(MpmbEngine *h, int64_t n_rows) {
   View V = make_view(h);
   const size_t dense = sizeof(int) * (size_t)h->ntot;
-  CUDA_TRY(h, cudaMemsetAsync(h->run_begin[h->ord], 0, dense, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->run_len[h->ord], 0, dense, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->stay[h->ord], 0, dense, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->arr_cnt, 0, dense, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->run_begin[h->ord].get(), 0, dense, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->run_len[h->ord].get(), 0, dense, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->stay[h->ord].get(), 0, dense, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->arr_cnt.get(), 0, dense, h->stream));
   Counters c{};
   c.n_store = (int)n_rows;
-  CUDA_TRY(h, cudaMemcpyAsync(h->cnt, &c, sizeof(int) * 3, cudaMemcpyHostToDevice, h->stream));          // n_store, n_tiles, n_ghost
-  CUDA_TRY(h, cudaMemsetAsync(&h->cnt->n_movers, 0, sizeof(int) * 3, h->stream));                          // n_movers, n_movers_next, n_alive
+  CUDA_TRY(h, cudaMemcpyAsync(h->cnt.get(), &c, sizeof(int) * 3, cudaMemcpyHostToDevice, h->stream));          // n_store, n_tiles, n_ghost
+  CUDA_TRY(h, cudaMemsetAsync(&h->cnt.get()->n_movers, 0, sizeof(int) * 3, h->stream));                          // n_movers, n_movers_next, n_alive
   if (n_rows > 0) {
-    cub::DeviceRadixSort::SortPairs(h->cub_temp, h->cub_bytes, h->keys[h->cur], h->keys_sorted, h->iota, h->arrivals_sorted, (int)n_rows, 0, h->key_bits, h->stream);
-    k_count_sorted<<<(unsigned)((n_rows + 255) / 256), 256, 0, h->stream>>>(V, h->keys_sorted, (int)n_rows, h->ntot);
+    size_t cub_bytes = h->cub_temp.size();
+    cub::DeviceRadixSort::SortPairs(h->cub_temp.get(), cub_bytes, h->keys[h->cur].get(), h->keys_sorted.get(), h->iota.get(), h->arrivals_sorted.get(), (int)n_rows, 0, h->key_bits, h->stream);
+    k_count_sorted<<<(unsigned)((n_rows + 255) / 256), 256, 0, h->stream>>>(V, h->keys_sorted.get(), (int)n_rows, h->ntot);
     h->launches++;
   }
   h->fresh = true;
@@ -3386,7 +3417,7 @@ static int finish_upload(MpmbEngine *h, int64_t n) {
   if (h->rigid_on) {  // new particles start with MPMParticle::states = 0 (mpmb_set_particle_states overrides)
     int rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap));
     if (rc != MPMB_OK) return rc;
-    CUDA_TRY(h, cudaMemsetAsync(h->R.p_states, 0, sizeof(uint32_t) * h->R.id_cap, h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->p_states.get(), 0, sizeof(uint32_t) * h->p_states.size(), h->stream));
   }
   return reorder_from_scratch(h, n);
 }
@@ -3397,7 +3428,7 @@ static int finish_upload(MpmbEngine *h, int64_t n) {
 static int pack_rows(MpmbEngine *h, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
                      const float *vol, const float *scalar, const int *group, int row0, uint32_t id0, const int *prefix = nullptr) {
   View V = make_view(h);
-  k_pack_particles<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, x, v, F, b, mass, vol, scalar, group, h->keys[h->cur], row0, id0,
+  k_pack_particles<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, x, v, F, b, mass, vol, scalar, group, h->keys[h->cur].get(), row0, id0,
                                                                          prefix);
   h->launches++;
   cudaError_t e = cudaStreamSynchronize(h->stream);
@@ -3416,16 +3447,8 @@ struct StagedFields {
 static int stage_fields(MpmbEngine *h, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
                         const float *vol, const float *scalar, const int32_t *group, StagedFields *s) {
   size_t fl = (size_t)n * (3 + 3 + (F ? 9 : 0) + (b ? 9 : 0) + 1 + 1 + (scalar ? 1 : 0)) + (group ? (size_t)n : 0);
-  float *stage = nullptr;
-  if (h->stage_bytes < fl * sizeof(float)) {
-    cudaFree(h->stage_buf);
-    h->stage_buf = nullptr;
-    h->stage_bytes = 0;
-    CUDA_TRY(h, cudaMalloc(&h->stage_buf, fl * sizeof(float)));
-    h->stage_bytes = fl * sizeof(float);
-  }
-  stage = (float *)h->stage_buf;
-  float *p = stage;
+  CUDA_TRY(h, h->stage_buf.reserve(fl * sizeof(float)));
+  float *p = (float *)h->stage_buf.get();
   auto put = [&](const void *src, size_t count) -> float * {
     if (!src) return nullptr;
     float *dst = p;
@@ -3511,13 +3534,13 @@ int mpmb_append_owned_particles(MpmbHandle h, int64_t n, const float *x, const f
     StagedFields s;
     if ((rc = stage_fields(h, n, x, v, F, b, mass, vol, scalar, group, &s)) != MPMB_OK) return rc;
     if ((rc = scan_reserve(h, (size_t)n)) != MPMB_OK) return rc;
-    k_owned_flags<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(h->P, (int)n, s.x, h->scan_a);
+    k_owned_flags<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(h->P, (int)n, s.x, h->scan_a.get());
     h->launches++;
     if ((rc = scan_flags(h, (size_t)n, &kept)) != MPMB_OK) return rc;
     if (kept > 0) {
       if ((rc = grow_keeping_rows(h, (int64_t)ns + kept, ns)) != MPMB_OK) return rc;
       h->aos_host_pool = nullptr;   // as mpmb_append_particles: the AoS index vector does not cover the new ids
-      if ((rc = pack_rows(h, n, s.x, s.v, s.F, s.b, s.mass, s.vol, s.scalar, s.group, ns, (uint32_t)first_id, h->scan_b)) != MPMB_OK) return rc;
+      if ((rc = pack_rows(h, n, s.x, s.v, s.F, s.b, s.mass, s.vol, s.scalar, s.group, ns, (uint32_t)first_id, h->scan_b.get())) != MPMB_OK) return rc;
     }
   }
   // the whole batch consumes its ids on every rank, kept or not
@@ -3545,12 +3568,12 @@ static int delete_inside(MpmbEngine *h, int64_t *n_deleted) {
   int ns = 0;
   if ((rc = read_n_store(h, &ns)) != MPMB_OK) return rc;
   if (ns == 0) return MPMB_OK;
-  CUDA_TRY(h, cudaMemsetAsync(&h->cnt->n_live, 0, sizeof(int), h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(&h->cnt.get()->n_live, 0, sizeof(int), h->stream));
   View V = make_view(h);
   k_delete_inside<<<(unsigned)((ns + 255) / 256), 256, 0, h->stream>>>(V, h->P, ns, h->special_min, h->key_dead);
   h->launches++;
   int killed = 0;
-  CUDA_TRY(h, cudaMemcpyAsync(&killed, &h->cnt->n_live, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(&killed, &h->cnt.get()->n_live, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
   *n_deleted = killed;
@@ -3576,31 +3599,19 @@ int mpmb_delete_owned_inside_levelset(MpmbHandle h, int64_t *n_deleted) {
 
 // flags / exclusive prefix scratch for n items (grow-only) and the CUB scan over them
 static int scan_reserve(MpmbEngine *h, size_t n) {
-  if (n + 1 > h->scan_cap) {
-    cudaFree(h->scan_a); cudaFree(h->scan_b);
-    h->scan_a = h->scan_b = nullptr;
-    h->scan_cap = 0;
-    CUDA_TRY(h, cudaMalloc(&h->scan_a, sizeof(int) * (n + 1)));
-    CUDA_TRY(h, cudaMalloc(&h->scan_b, sizeof(int) * (n + 1)));
-    h->scan_cap = n + 1;
-  }
+  CUDA_TRY(h, h->scan_a.reserve(n + 1));
+  CUDA_TRY(h, h->scan_b.reserve(n + 1));
   size_t need = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, need, h->scan_a, h->scan_b, (int)(n + 1), h->stream);
-  if (need > h->scan_tmp_bytes) {
-    cudaFree(h->scan_tmp);
-    h->scan_tmp = nullptr;
-    h->scan_tmp_bytes = 0;
-    CUDA_TRY(h, cudaMalloc(&h->scan_tmp, need));
-    h->scan_tmp_bytes = need;
-  }
+  cub::DeviceScan::ExclusiveSum(nullptr, need, h->scan_a.get(), h->scan_b.get(), (int)(n + 1), h->stream);
+  CUDA_TRY(h, h->scan_tmp.reserve(need));
   return MPMB_OK;
 }
 // prefix = exclusive scan of flags over n (+1 so that prefix[n] is the total); returns the total
 static int scan_flags(MpmbEngine *h, size_t n, int *total) {
-  CUDA_TRY(h, cudaMemsetAsync(h->scan_a + n, 0, sizeof(int), h->stream));
-  size_t bytes = h->scan_tmp_bytes;
-  cub::DeviceScan::ExclusiveSum(h->scan_tmp, bytes, h->scan_a, h->scan_b, (int)(n + 1), h->stream);
-  CUDA_TRY(h, cudaMemcpyAsync(total, h->scan_b + n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->scan_a.get() + n, 0, sizeof(int), h->stream));
+  size_t bytes = h->scan_tmp.size();
+  cub::DeviceScan::ExclusiveSum(h->scan_tmp.get(), bytes, h->scan_a.get(), h->scan_b.get(), (int)(n + 1), h->stream);
+  CUDA_TRY(h, cudaMemcpyAsync(total, h->scan_b.get() + n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   return MPMB_OK;
 }
@@ -3619,20 +3630,8 @@ static void aos_window(const MpmbAosLayout *L, int *lo, int *hi) {
 }
 
 static int aos_reserve(MpmbEngine *h, size_t pool_bytes, size_t n_idx) {
-  if (pool_bytes > h->aos_pool_bytes) {
-    cudaFree(h->aos_pool);
-    h->aos_pool = nullptr;
-    h->aos_pool_bytes = 0;
-    CUDA_TRY(h, cudaMalloc(&h->aos_pool, pool_bytes));
-    h->aos_pool_bytes = pool_bytes;
-  }
-  if (n_idx > h->aos_idx_cap) {
-    cudaFree(h->aos_idx);
-    h->aos_idx = nullptr;
-    h->aos_idx_cap = 0;
-    CUDA_TRY(h, cudaMalloc(&h->aos_idx, sizeof(uint32_t) * n_idx));
-    h->aos_idx_cap = n_idx;
-  }
+  CUDA_TRY(h, h->aos_pool.reserve(pool_bytes));
+  CUDA_TRY(h, h->aos_idx.reserve(n_idx));
   return MPMB_OK;
 }
 
@@ -3651,25 +3650,19 @@ int mpmb_upload_aos(MpmbHandle h, int64_t n, const void *pool, int64_t pool_slot
   if ((rc = aos_reserve(h, pool_bytes, (size_t)n)) != MPMB_OK) return rc;
   int *d_grp = nullptr;
   if (group) {
-    if (h->stage_bytes < sizeof(int) * (size_t)n) {
-      cudaFree(h->stage_buf);
-      h->stage_buf = nullptr;
-      h->stage_bytes = 0;
-      CUDA_TRY(h, cudaMalloc(&h->stage_buf, sizeof(int) * (size_t)n));
-      h->stage_bytes = sizeof(int) * (size_t)n;
-    }
-    d_grp = (int *)h->stage_buf;
+    CUDA_TRY(h, h->stage_buf.reserve(sizeof(int) * (size_t)n));
+    d_grp = (int *)h->stage_buf.get();
     CUDA_TRY(h, cudaMemcpyAsync(d_grp, group, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
   }
-  CUDA_TRY(h, cudaMemcpyAsync(h->aos_idx, indices, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(h->aos_idx.get(), indices, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, h->stream));
   {
     int lo, hi;
     aos_window(L, &lo, &hi);
-    CUDA_TRY(h, cudaMemcpy2DAsync(h->aos_pool + lo, (size_t)L->stride, (const char *)pool + lo, (size_t)L->stride, (size_t)(hi - lo), (size_t)pool_slots,
+    CUDA_TRY(h, cudaMemcpy2DAsync(h->aos_pool.get() + lo, (size_t)L->stride, (const char *)pool + lo, (size_t)L->stride, (size_t)(hi - lo), (size_t)pool_slots,
                                   cudaMemcpyHostToDevice, h->stream));
   }
   View V = make_view(h);
-  k_pack_aos<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, h->aos_pool, h->aos_idx, *L, d_grp, h->keys[h->cur], h->id_base);
+  k_pack_aos<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, h->aos_pool.get(), h->aos_idx.get(), *L, d_grp, h->keys[h->cur].get(), h->id_base);
   h->launches++;
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
@@ -3711,13 +3704,13 @@ int mpmb_seed_lattice(MpmbHandle h, const int32_t lo_cell[3], const int32_t hi_c
   int total = 0, rc;
   if (n_cand > 0) {
     if ((rc = scan_reserve(h, n_cand)) != MPMB_OK) return rc;
-    k_seed_flags<<<h->num_sms * 8, 256, 0, h->stream>>>(h->P, B, n_cand, h->scan_a);
+    k_seed_flags<<<h->num_sms * 8, 256, 0, h->stream>>>(h->P, B, n_cand, h->scan_a.get());
     if ((rc = scan_flags(h, n_cand, &total)) != MPMB_OK) return rc;
   }
   if ((rc = ensure_capacity(h, total)) != MPMB_OK) return rc;
   if (total > 0) {
     View V = make_view(h);
-    k_seed_write<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, B, n_cand, h->scan_a, h->scan_b, h->keys[h->cur]);
+    k_seed_write<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, B, n_cand, h->scan_a.get(), h->scan_b.get(), h->keys[h->cur].get());
     h->launches += 2;
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     CUDA_TRY(h, cudaGetLastError());
@@ -3731,7 +3724,7 @@ int mpmb_seed_lattice(MpmbHandle h, const int32_t lo_cell[3], const int32_t hi_c
 
 static int read_n_store(MpmbEngine *h, int *n_store) {
   Counters c;
-  CUDA_TRY(h, cudaMemcpy(&c, h->cnt, sizeof(c), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(&c, h->cnt.get(), sizeof(c), cudaMemcpyDeviceToHost));
   *n_store = c.n_store;
   return MPMB_OK;
 }
@@ -3741,13 +3734,13 @@ int mpmb_num_particles(MpmbHandle h, int64_t *n) {
   if (!n) return fail(h, MPMB_ERR_INVALID, "null argument");
   *n = 0;
   if (h->cap == 0) return MPMB_OK;
-  CUDA_TRY(h, cudaMemsetAsync(&h->cnt->n_live, 0, sizeof(int), h->stream));
-  k_count_live<<<h->num_sms * 4, 256, 0, h->stream>>>(h->keys[h->cur], h->special_min, h->cnt);
+  CUDA_TRY(h, cudaMemsetAsync(&h->cnt.get()->n_live, 0, sizeof(int), h->stream));
+  k_count_live<<<h->num_sms * 4, 256, 0, h->stream>>>(h->keys[h->cur].get(), h->special_min, h->cnt.get());
   h->launches++;
   int rc = mpmb_synchronize(h);
   if (rc != MPMB_OK) return rc;
   int live = 0;
-  CUDA_TRY(h, cudaMemcpy(&live, &h->cnt->n_live, sizeof(int), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(&live, &h->cnt.get()->n_live, sizeof(int), cudaMemcpyDeviceToHost));
   *n = live;
   return MPMB_OK;
 }
@@ -3758,7 +3751,7 @@ int mpmb_get_update_count(MpmbHandle h, int64_t *updates) {
   int rc = mpmb_synchronize(h);
   if (rc != MPMB_OK) return rc;
   unsigned long long u = 0;
-  CUDA_TRY(h, cudaMemcpy(&u, &h->cnt->updates, sizeof(u), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(&u, &h->cnt.get()->updates, sizeof(u), cudaMemcpyDeviceToHost));
   *updates = (int64_t)u;
   return MPMB_OK;
 }
@@ -3768,7 +3761,7 @@ int mpmb_get_update_count(MpmbHandle h, int64_t *updates) {
 static int live_prefix(MpmbEngine *h, int n, int64_t *alive) {
   int rc, total = 0;
   if ((rc = scan_reserve(h, (size_t)n)) != MPMB_OK) return rc;
-  k_alive_flags<<<(n + 255) / 256, 256, 0, h->stream>>>(h->keys[h->cur], n, h->special_min, h->scan_a);
+  k_alive_flags<<<(n + 255) / 256, 256, 0, h->stream>>>(h->keys[h->cur].get(), n, h->special_min, h->scan_a.get());
   if ((rc = scan_flags(h, (size_t)n, &total)) != MPMB_OK) return rc;
   *alive = total;
   return MPMB_OK;
@@ -3777,7 +3770,7 @@ static int live_prefix(MpmbEngine *h, int n, int64_t *alive) {
 // The live rows, compacted in storage order, into DEVICE arrays (any may be NULL); id = the engine's particle id.
 static void unpack_live(MpmbEngine *h, int n, uint32_t *id, float *x, float *v, float *F, float *b, float *mass, float *vol, float *scalar, int *group) {
   View V = make_view(h);
-  k_unpack_particles<<<(n + 127) / 128, 128, 0, h->stream>>>(V, h->keys[h->cur], n, h->special_min, id, x, v, F, b, mass, vol, scalar, group, h->scan_b);
+  k_unpack_particles<<<(n + 127) / 128, 128, 0, h->stream>>>(V, h->keys[h->cur].get(), n, h->special_min, id, x, v, F, b, mass, vol, scalar, group, h->scan_b.get());
   h->launches += 2;
 }
 
@@ -3796,16 +3789,8 @@ int mpmb_download_particles(MpmbHandle h, int64_t cap, int64_t *n_out, uint32_t 
   if (alive > cap) return fail(h, MPMB_ERR_CAPACITY, "%lld live particles do not fit in the %lld rows provided", (long long)alive, (long long)cap);
   size_t fl = (size_t)alive * ((x ? 3 : 0) + (v ? 3 : 0) + (F ? 9 : 0) + (b ? 9 : 0) + (mass ? 1 : 0) + (vol ? 1 : 0) + (scalar ? 1 : 0) +
                                (id ? 1 : 0) + (group ? 1 : 0));
-  float *stage = nullptr;
-  if (h->stage_bytes < fl * sizeof(float)) {
-    cudaFree(h->stage_buf);
-    h->stage_buf = nullptr;
-    h->stage_bytes = 0;
-    CUDA_TRY(h, cudaMalloc(&h->stage_buf, fl * sizeof(float)));
-    h->stage_bytes = fl * sizeof(float);
-  }
-  stage = (float *)h->stage_buf;
-  float *p = stage;
+  CUDA_TRY(h, h->stage_buf.reserve(fl * sizeof(float)));
+  float *p = (float *)h->stage_buf.get();
   auto take = [&](bool want, size_t per) -> float * {
     if (!want) return nullptr;
     float *r = p;
@@ -3839,32 +3824,32 @@ int mpmb_download_aos(MpmbHandle h, void *pool, int64_t pool_slots, uint32_t *in
   if (n_indices == 0) return MPMB_OK;
   const size_t pool_bytes = (size_t)pool_slots * L->stride;
   // the device image of the pool: still resident from mpmb_upload_aos of the same pool, else brought in now
-  const bool resident = h->aos_host_pool == pool && h->aos_slots == pool_slots && h->aos_n == n_indices && h->aos_pool;
+  const bool resident = h->aos_host_pool == pool && h->aos_slots == pool_slots && h->aos_n == n_indices && h->aos_pool.get();
   if (!resident) {
     if ((rc = aos_reserve(h, pool_bytes, (size_t)n_indices)) != MPMB_OK) return rc;
-    CUDA_TRY(h, cudaMemcpyAsync(h->aos_idx, indices, sizeof(uint32_t) * n_indices, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(h->aos_pool, pool, pool_bytes, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->aos_idx.get(), indices, sizeof(uint32_t) * n_indices, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->aos_pool.get(), pool, pool_bytes, cudaMemcpyHostToDevice, h->stream));
   }
   (void)pool_bytes;
   if ((rc = scan_reserve(h, (size_t)n_indices)) != MPMB_OK) return rc;
-  CUDA_TRY(h, cudaMemsetAsync(h->scan_a, 0, sizeof(int) * (size_t)n_indices, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->scan_a.get(), 0, sizeof(int) * (size_t)n_indices, h->stream));
   if (ns > 0 && h->cap > 0) {
     View V = make_view(h);
-    k_aos_scatter<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, h->keys[h->cur], ns, h->special_min, h->aos_pool, h->aos_idx, n_indices, pool_slots, *L,
-                                                           h->id_base, h->scan_a, h->cnt);
+    k_aos_scatter<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, h->keys[h->cur].get(), ns, h->special_min, h->aos_pool.get(), h->aos_idx.get(), n_indices, pool_slots, *L,
+                                                           h->id_base, h->scan_a.get(), h->cnt.get());
     h->launches++;
   }
   int alive = 0;
   if ((rc = scan_flags(h, (size_t)n_indices, &alive)) != MPMB_OK) return rc;
   // survivors' slots in id order == what clear_boundary_particles leaves in MPM::particles (src/mpm.cpp:618-622)
-  uint32_t *d_surv = (uint32_t *)h->keys_sorted;  // upload-time scratch, free between uploads; cap >= n rows
+  uint32_t *d_surv = (uint32_t *)h->keys_sorted.get();  // upload-time scratch, free between uploads; cap >= n rows
   if ((int64_t)h->cap < n_indices) return fail(h, MPMB_ERR_CAPACITY, "index vector longer than the particle capacity");
-  k_compact_survivors<<<(unsigned)((n_indices + 255) / 256), 256, 0, h->stream>>>(h->aos_idx, h->scan_a, h->scan_b, n_indices, d_surv);
+  k_compact_survivors<<<(unsigned)((n_indices + 255) / 256), 256, 0, h->stream>>>(h->aos_idx.get(), h->scan_a.get(), h->scan_b.get(), n_indices, d_surv);
   h->launches++;
   {  // only the window of every slot that holds the layout's fields comes back; the rest of the host pool is untouched
     int lo, hi;
     aos_window(L, &lo, &hi);
-    CUDA_TRY(h, cudaMemcpy2DAsync((char *)pool + lo, (size_t)L->stride, h->aos_pool + lo, (size_t)L->stride, (size_t)(hi - lo), (size_t)pool_slots,
+    CUDA_TRY(h, cudaMemcpy2DAsync((char *)pool + lo, (size_t)L->stride, h->aos_pool.get() + lo, (size_t)L->stride, (size_t)(hi - lo), (size_t)pool_slots,
                                   cudaMemcpyDeviceToHost, h->stream));
   }
   if (alive > 0) CUDA_TRY(h, cudaMemcpyAsync(indices, d_surv, sizeof(uint32_t) * (size_t)alive, cudaMemcpyDeviceToHost, h->stream));
@@ -3884,23 +3869,17 @@ int mpmb_download_bgeo_points(MpmbHandle h, int64_t id_range, void *records, int
   *n_out = 0;
   if (ns == 0 || h->cap == 0) return MPMB_OK;
   if ((rc = scan_reserve(h, (size_t)id_range)) != MPMB_OK) return rc;
-  CUDA_TRY(h, cudaMemsetAsync(h->scan_a, 0, sizeof(int) * (size_t)id_range, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->scan_a.get(), 0, sizeof(int) * (size_t)id_range, h->stream));
   View V = make_view(h);
-  k_id_flags<<<(ns + 255) / 256, 256, 0, h->stream>>>(V, h->keys[h->cur], ns, h->special_min, h->id_base, id_range, h->scan_a, h->cnt);
+  k_id_flags<<<(ns + 255) / 256, 256, 0, h->stream>>>(V, h->keys[h->cur].get(), ns, h->special_min, h->id_base, id_range, h->scan_a.get(), h->cnt.get());
   int alive = 0;
   if ((rc = scan_flags(h, (size_t)id_range, &alive)) != MPMB_OK) return rc;
   if (alive > cap_records) return fail(h, MPMB_ERR_CAPACITY, "%d live particles do not fit in the %lld records provided", alive, (long long)cap_records);
   const size_t bytes = (size_t)alive * 48;
-  if (h->stage_bytes < bytes) {
-    cudaFree(h->stage_buf);
-    h->stage_buf = nullptr;
-    h->stage_bytes = 0;
-    CUDA_TRY(h, cudaMalloc(&h->stage_buf, bytes));
-    h->stage_bytes = bytes;
-  }
-  k_bgeo_points<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, h->keys[h->cur], ns, h->special_min, h->id_base, id_range, h->scan_b, (uint32_t *)h->stage_buf);
+  CUDA_TRY(h, h->stage_buf.reserve(bytes));
+  k_bgeo_points<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, h->keys[h->cur].get(), ns, h->special_min, h->id_base, id_range, h->scan_b.get(), (uint32_t *)h->stage_buf.get());
   h->launches += 2;
-  CUDA_TRY(h, cudaMemcpyAsync(records, h->stage_buf, bytes, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(records, h->stage_buf.get(), bytes, cudaMemcpyDeviceToHost, h->stream));
   if ((rc = mpmb_synchronize(h)) != MPMB_OK) return rc;
   CUDA_TRY(h, cudaGetLastError());
   *n_out = alive;
@@ -3909,34 +3888,31 @@ int mpmb_download_bgeo_points(MpmbHandle h, int64_t id_range, void *records, int
 
 // ------------------------------------------------------------------------------ CPIC host side
 static int rigid_reserve_ids(MpmbEngine *h, int64_t n_ids) {
-  if (n_ids <= h->R.id_cap && h->R.p_states) return MPMB_OK;
+  if (h->p_states.get() && n_ids <= (int64_t)h->p_states.size()) return MPMB_OK;
   const int64_t cap = std::max<int64_t>(n_ids, 1024);
-  uint32_t *st = nullptr;
-  float4 *cdf = nullptr;
-  uint32_t *nr = nullptr;
-  CUDA_TRY(h, cudaMalloc(&st, sizeof(uint32_t) * cap));
-  CUDA_TRY(h, cudaMalloc(&cdf, sizeof(float4) * cap));
-  CUDA_TRY(h, cudaMalloc(&nr, sizeof(uint32_t) * cap));
-  CUDA_TRY(h, cudaMemsetAsync(st, 0, sizeof(uint32_t) * cap, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(cdf, 0, sizeof(float4) * cap, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(nr, 0, sizeof(uint32_t) * cap, h->stream));   // epoch 0 is never current
-  if (h->R.p_states && h->R.id_cap > 0) CUDA_TRY(h, cudaMemcpyAsync(st, h->R.p_states, sizeof(uint32_t) * h->R.id_cap, cudaMemcpyDeviceToDevice, h->stream));
+  DevBuf<uint32_t> st, nr;
+  DevBuf<float4> cdf;
+  CUDA_TRY(h, st.alloc(cap));
+  CUDA_TRY(h, cdf.alloc(cap));
+  CUDA_TRY(h, nr.alloc(cap));
+  CUDA_TRY(h, cudaMemsetAsync(st.get(), 0, sizeof(uint32_t) * cap, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(cdf.get(), 0, sizeof(float4) * cap, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(nr.get(), 0, sizeof(uint32_t) * cap, h->stream));   // epoch 0 is never current
+  if (h->p_states.size() > 0)
+    CUDA_TRY(h, cudaMemcpyAsync(st.get(), h->p_states.get(), sizeof(uint32_t) * h->p_states.size(), cudaMemcpyDeviceToDevice, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  cudaFree(h->R.p_states); cudaFree(h->R.p_cdf); cudaFree(h->R.p_mark);
-  h->R.p_states = st; h->R.p_cdf = cdf; h->R.p_mark = nr;
-  h->R.id_cap = (int)cap;
+  h->p_states = std::move(st); h->p_cdf = std::move(cdf); h->p_mark = std::move(nr);
   graph_reset(h);   // the captured rigid kernels hold the freed arrays and the old id_cap
   return MPMB_OK;
 }
 
 // per substep, after the ordering: pages + colour field of this pose, tile flags, particle colours
 static int rigid_prepare(MpmbEngine *h, const View &V, int *nl) {
-  RigidView &R = h->R;
-  R.id_base = h->id_base;
-  if (!R.p_states || R.id_cap < h->id_span) { int rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap)); if (rc != MPMB_OK) return rc; }
+  if (!h->p_states.get() || (int64_t)h->p_states.size() < h->id_span) { int rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap)); if (rc != MPMB_OK) return rc; }
+  const RigidView R = rigid_view(h);
   const int ns = R.n_samples, sb = (ns + 127) / 128;
   k_cdf_clear<<<sb, 128, 0, h->stream>>>(R, h->P);
-  CUDA_TRY(h, cudaMemsetAsync(R.page, 0, (size_t)R.nb[0] * R.nb[1] * R.nb[2], h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(R.page, 0, h->page.size(), h->stream));
   k_cdf_raster<<<sb, 128, 0, h->stream>>>(R, h->P);
   k_rigid_tile_flags<<<(h->cap_tiles + 127) / 128, 128, 0, h->stream>>>(V, h->P, R);
   k_gather_cdf<<<(int)((h->cap + 127) / 128), 128, 0, h->stream>>>(V, h->P, R);
@@ -3953,57 +3929,51 @@ int mpmb_set_rigid_samples(MpmbHandle h, int32_t n_bodies, int64_t n_samples, co
   if (h->P.nnode[0] > 1023 || h->P.nnode[1] > 1023 || h->P.nnode[2] > 1023) return fail(h, MPMB_ERR_INVALID, "rigid coupling supports grids up to 1022 cells per axis");
   for (int64_t s = 0; s < n_samples; s++)
     if (rigid_id[s] < 1 || rigid_id[s] >= n_bodies) return fail(h, MPMB_ERR_INVALID, "sample %lld names body %d (valid: 1..%d)", (long long)s, rigid_id[s], n_bodies - 1);
-  RigidView &R = h->R;
-  cudaFree(h->rs_offset); cudaFree(h->rs_tri); cudaFree(h->rs_rigid); cudaFree(R.s_base);
-  h->rs_offset = h->rs_tri = nullptr; h->rs_rigid = nullptr; R.s_base = nullptr;
-  CUDA_TRY(h, cudaMalloc(&h->rs_offset, sizeof(float) * 3 * n_samples));
-  CUDA_TRY(h, cudaMalloc(&h->rs_tri, sizeof(float) * 9 * n_samples));
-  CUDA_TRY(h, cudaMalloc(&h->rs_rigid, sizeof(int) * n_samples));
-  CUDA_TRY(h, cudaMalloc(&R.s_base, sizeof(int) * n_samples));
-  CUDA_TRY(h, cudaMemcpyAsync(h->rs_offset, offset3, sizeof(float) * 3 * n_samples, cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(h->rs_tri, tri9, sizeof(float) * 9 * n_samples, cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(h->rs_rigid, rigid_id, sizeof(int) * n_samples, cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(R.s_base, 0xff, sizeof(int) * n_samples, h->stream));
-  R.s_offset = h->rs_offset; R.s_tri = h->rs_tri; R.s_rigid = h->rs_rigid;
-  R.n_samples = (int)n_samples;
-  R.n_bodies = n_bodies;
-  if (!R.bodies) {
-    CUDA_TRY(h, cudaMalloc(&R.bodies, sizeof(RigidDev) * RIGID_MAX));
-    CUDA_TRY(h, cudaMemsetAsync(R.bodies, 0, sizeof(RigidDev) * RIGID_MAX, h->stream));
-    CUDA_TRY(h, cudaMalloc(&R.epoch, sizeof(uint32_t)));
-    CUDA_TRY(h, cudaMemsetAsync(R.epoch, 0, sizeof(uint32_t), h->stream));
-    CUDA_TRY(h, cudaMalloc(&h->M.m, sizeof(RigidMaster) * RIGID_MAX));
-    CUDA_TRY(h, cudaMalloc(&h->M.cursor, sizeof(int)));
-    CUDA_TRY(h, cudaMemsetAsync(h->M.cursor, 0, sizeof(int), h->stream));
+  h->rs_offset.reset(); h->rs_tri.reset(); h->rs_rigid.reset(); h->s_base.reset();   // the old samples go before the new ones come
+  CUDA_TRY(h, h->rs_offset.alloc(3 * n_samples));
+  CUDA_TRY(h, h->rs_tri.alloc(9 * n_samples));
+  CUDA_TRY(h, h->rs_rigid.alloc(n_samples));
+  CUDA_TRY(h, h->s_base.alloc(n_samples));
+  CUDA_TRY(h, cudaMemcpyAsync(h->rs_offset.get(), offset3, sizeof(float) * 3 * n_samples, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(h->rs_tri.get(), tri9, sizeof(float) * 9 * n_samples, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(h->rs_rigid.get(), rigid_id, sizeof(int) * n_samples, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->s_base.get(), 0xff, sizeof(int) * n_samples, h->stream));
+  h->rigid_samples = (int)n_samples;
+  h->rigid_bodies = n_bodies;
+  if (!h->bodies.get()) {
+    CUDA_TRY(h, h->bodies.alloc(RIGID_MAX));
+    CUDA_TRY(h, cudaMemsetAsync(h->bodies.get(), 0, sizeof(RigidDev) * RIGID_MAX, h->stream));
+    CUDA_TRY(h, h->epoch.alloc(1));
+    CUDA_TRY(h, cudaMemsetAsync(h->epoch.get(), 0, sizeof(uint32_t), h->stream));
+    CUDA_TRY(h, h->master.alloc(RIGID_MAX));
+    CUDA_TRY(h, h->cursor.alloc(1));
+    CUDA_TRY(h, cudaMemsetAsync(h->cursor.get(), 0, sizeof(int), h->stream));
   }
   {  // per-body sample lists for the level-set collision (samples need not be grouped by body)
     std::vector<int> order((size_t)n_samples);
     int cnt[RIGID_MAX + 1] = {};
     for (int64_t s = 0; s < n_samples; s++) cnt[rigid_id[s] + 1]++;
     for (int b = 0; b < RIGID_MAX; b++) cnt[b + 1] += cnt[b];
-    for (int b = 0; b <= RIGID_MAX; b++) h->M.s_begin[b] = cnt[b];
+    for (int b = 0; b <= RIGID_MAX; b++) h->s_begin[b] = cnt[b];
     for (int64_t s = 0; s < n_samples; s++) order[(size_t)cnt[rigid_id[s]]++] = (int)s;
-    cudaFree(h->s_order); cudaFree(h->contact);   // contacts: allocated by mpmb_set_rigid_motion when the collision is asked for
-    h->s_order = nullptr; h->contact = nullptr;
-    CUDA_TRY(h, cudaMalloc(&h->s_order, sizeof(int) * n_samples));
-    CUDA_TRY(h, cudaMemcpyAsync(h->s_order, order.data(), sizeof(int) * n_samples, cudaMemcpyHostToDevice, h->stream));
+    h->contact.reset();   // contacts: allocated by mpmb_set_rigid_motion when the collision is asked for
+    CUDA_TRY(h, h->s_order.alloc(n_samples));
+    CUDA_TRY(h, cudaMemcpyAsync(h->s_order.get(), order.data(), sizeof(int) * n_samples, cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));   // `order` lives on this stack frame
-    h->M.s_order = h->s_order;
-    h->M.contact = h->contact;
   }
   const size_t nn = (size_t)h->P.nnode[0] * h->P.nnode[1] * h->P.nnode[2];
-  if (!R.node_key) {
-    CUDA_TRY(h, cudaMalloc(&R.node_key, sizeof(unsigned long long) * nn));
-    CUDA_TRY(h, cudaMalloc(&R.node_tags, sizeof(uint32_t) * nn));
-    R.nb[0] = (h->P.nnode[0] + 3) / 4 + 1; R.nb[1] = (h->P.nnode[1] + 3) / 4 + 1; R.nb[2] = (h->P.nnode[2] + 7) / 8 + 1;
-    CUDA_TRY(h, cudaMalloc(&R.page, (size_t)R.nb[0] * R.nb[1] * R.nb[2]));
-    CUDA_TRY(h, cudaMalloc(&R.tile_flag, (size_t)std::max(h->cap_tiles, 1)));
-    CUDA_TRY(h, cudaMemsetAsync(R.tile_flag, 0, (size_t)std::max(h->cap_tiles, 1), h->stream));
-    h->rigid_nodes = nn;
+  if (!h->node_key.get()) {
+    CUDA_TRY(h, h->node_key.alloc(nn));
+    CUDA_TRY(h, h->node_tags.alloc(nn));
+    int *nb = h->rigid_nb;
+    nb[0] = (h->P.nnode[0] + 3) / 4 + 1; nb[1] = (h->P.nnode[1] + 3) / 4 + 1; nb[2] = (h->P.nnode[2] + 7) / 8 + 1;
+    CUDA_TRY(h, h->page.alloc((size_t)nb[0] * nb[1] * nb[2]));
+    CUDA_TRY(h, h->tile_flag.alloc(std::max(h->cap_tiles, 1)));
+    CUDA_TRY(h, cudaMemsetAsync(h->tile_flag.get(), 0, h->tile_flag.size(), h->stream));
   }
-  CUDA_TRY(h, cudaMemsetAsync(R.node_key, 0xff, sizeof(unsigned long long) * nn, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(R.node_tags, 0, sizeof(uint32_t) * nn, h->stream));
-  if (R.pushing_force == 0.f && R.penalty == 0.f) R.pushing_force = 20000.0f;   // src/mpm.cpp:35,40 defaults
+  CUDA_TRY(h, cudaMemsetAsync(h->node_key.get(), 0xff, sizeof(unsigned long long) * nn, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->node_tags.get(), 0, sizeof(uint32_t) * nn, h->stream));
+  if (h->pushing_force == 0.f && h->penalty == 0.f) h->pushing_force = 20000.0f;   // src/mpm.cpp:35,40 defaults
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   h->rigid_on = true;
   h->motion_on = false;   // motion records describe a set of bodies: mpmb_set_rigid_motion follows the samples
@@ -4015,8 +3985,8 @@ int mpmb_set_rigid_samples(MpmbHandle h, int32_t n_bodies, int64_t n_samples, co
 
 int mpmb_set_rigid_coupling(MpmbHandle h, float penalty, float pushing_force) {
   CHECK_HANDLE(h);
-  h->R.penalty = penalty;
-  h->R.pushing_force = pushing_force;
+  h->penalty = penalty;
+  h->pushing_force = pushing_force;
   graph_reset(h);   // both are kernel arguments
   return MPMB_OK;
 }
@@ -4024,7 +3994,7 @@ int mpmb_set_rigid_coupling(MpmbHandle h, float penalty, float pushing_force) {
 int mpmb_set_rigid_state(MpmbHandle h, int32_t n_bodies, const MpmbRigidBody *bodies) {
   CHECK_HANDLE(h);
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies: call mpmb_set_rigid_samples first");
-  if (n_bodies != h->R.n_bodies || !bodies) return fail(h, MPMB_ERR_INVALID, "expected %d bodies", h->R.n_bodies);
+  if (n_bodies != h->rigid_bodies || !bodies) return fail(h, MPMB_ERR_INVALID, "expected %d bodies", h->rigid_bodies);
   RigidDev dev[RIGID_MAX];
   memset(dev, 0, sizeof(dev));
   for (int b = 0; b < n_bodies; b++) {
@@ -4035,14 +4005,14 @@ int mpmb_set_rigid_state(MpmbHandle h, int32_t n_bodies, const MpmbRigidBody *bo
     d.inv_mass = s.inv_mass;
     d.fric[0] = s.frictions[0]; d.fric[1] = s.frictions[1];
   }
-  CUDA_TRY(h, cudaMemcpyAsync(h->R.bodies, dev, sizeof(RigidDev) * RIGID_MAX, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(h->bodies.get(), dev, sizeof(RigidDev) * RIGID_MAX, cudaMemcpyHostToDevice, h->stream));
   if (h->motion_on) {   // the master states restart from the given records
     for (int b = 0; b < n_bodies; b++) {
       RigidMaster &m = h->h_master[b];
       for (int k = 0; k < 3; k++) { m.pos[k] = dev[b].pos[k]; m.vel[k] = dev[b].vel[k]; m.ang[k] = dev[b].ang[k]; }
       for (int k = 0; k < 9; k++) m.rot[k] = dev[b].rot[k];
     }
-    CUDA_TRY(h, cudaMemcpyAsync(h->M.m, h->h_master, sizeof(RigidMaster) * RIGID_MAX, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->master.get(), h->h_master, sizeof(RigidMaster) * RIGID_MAX, cudaMemcpyHostToDevice, h->stream));
   }
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));   // `dev` lives on this stack frame
   return MPMB_OK;
@@ -4051,9 +4021,9 @@ int mpmb_set_rigid_state(MpmbHandle h, int32_t n_bodies, const MpmbRigidBody *bo
 int mpmb_get_rigid_state(MpmbHandle h, int32_t n_bodies, MpmbRigidBody *bodies) {
   CHECK_HANDLE(h);
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies");
-  if (n_bodies != h->R.n_bodies || !bodies) return fail(h, MPMB_ERR_INVALID, "expected %d bodies", h->R.n_bodies);
+  if (n_bodies != h->rigid_bodies || !bodies) return fail(h, MPMB_ERR_INVALID, "expected %d bodies", h->rigid_bodies);
   RigidDev dev[RIGID_MAX];
-  CUDA_TRY(h, cudaMemcpyAsync(dev, h->R.bodies, sizeof(RigidDev) * RIGID_MAX, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(dev, h->bodies.get(), sizeof(RigidDev) * RIGID_MAX, cudaMemcpyDeviceToHost, h->stream));
   int rc = mpmb_synchronize(h);
   if (rc != MPMB_OK) return rc;
   for (int b = 0; b < n_bodies; b++) {
@@ -4072,7 +4042,7 @@ int mpmb_set_rigid_motion(MpmbHandle h, int32_t n_bodies, const MpmbRigidMotion 
   if (n_bodies == 0) { h->motion_on = false; graph_reset(h); return MPMB_OK; }
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies: call mpmb_set_rigid_samples first");
   if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "rigid motion changes between substeps, not inside one");
-  if (n_bodies != h->R.n_bodies || !motion) return fail(h, MPMB_ERR_INVALID, "expected %d motion records", h->R.n_bodies);
+  if (n_bodies != h->rigid_bodies || !motion) return fail(h, MPMB_ERR_INVALID, "expected %d motion records", h->rigid_bodies);
   bool scripted = false;
   for (int b = 1; b < n_bodies; b++) {
     const MpmbRigidMotion &m = motion[b];
@@ -4084,7 +4054,7 @@ int mpmb_set_rigid_motion(MpmbHandle h, int32_t n_bodies, const MpmbRigidMotion 
     scripted = scripted || m.scripted_position || m.scripted_rotation;
   }
   RigidDev dev[RIGID_MAX];   // the master states start from the current records
-  CUDA_TRY(h, cudaMemcpyAsync(dev, h->R.bodies, sizeof(RigidDev) * RIGID_MAX, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(dev, h->bodies.get(), sizeof(RigidDev) * RIGID_MAX, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   memset(h->h_master, 0, sizeof(h->h_master));
   for (int b = 1; b < n_bodies; b++) {
@@ -4098,13 +4068,10 @@ int mpmb_set_rigid_motion(MpmbHandle h, int32_t n_bodies, const MpmbRigidMotion 
     m.scripted_pos = s.scripted_position != 0;
     m.scripted_rot = s.scripted_rotation != 0;
   }
-  CUDA_TRY(h, cudaMemcpyAsync(h->M.m, h->h_master, sizeof(RigidMaster) * RIGID_MAX, cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->M.cursor, 0, sizeof(int), h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(h->master.get(), h->h_master, sizeof(RigidMaster) * RIGID_MAX, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->cursor.get(), 0, sizeof(int), h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  if (levelset_collision && !h->contact) {
-    CUDA_TRY(h, cudaMalloc(&h->contact, sizeof(double) * CONTACT_STRIDE * h->R.n_samples));
-    h->M.contact = h->contact;
-  }
+  if (levelset_collision) CUDA_TRY(h, h->contact.reserve((size_t)CONTACT_STRIDE * h->rigid_samples));
   h->script_left = 0;
   h->motion_scripted = scripted;
   h->motion_collide = levelset_collision != 0;
@@ -4118,7 +4085,7 @@ int mpmb_set_rigid_script(MpmbHandle h, int32_t n_substeps, const double *poses)
   if (!h->rigid_on || !h->motion_on) return fail(h, MPMB_ERR_STATE, "no device-advanced bodies: call mpmb_set_rigid_motion first");
   if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "the script changes between substeps, not inside one");
   if (n_substeps < 0 || (n_substeps > 0 && !poses)) return fail(h, MPMB_ERR_INVALID, "need n_substeps >= 0 and a table");
-  const int nb = h->R.n_bodies;
+  const int nb = h->rigid_bodies;
   const size_t n = (size_t)n_substeps * nb * SCRIPT_STRIDE;
   for (int64_t e = 0; e < n_substeps; e++)   // only the scripted parts are read
     for (int b = 1; b < nb; b++) {
@@ -4129,18 +4096,12 @@ int mpmb_set_rigid_script(MpmbHandle h, int32_t n_substeps, const double *poses)
       if (h->h_master[b].scripted_rot) for (int k = 15; k < 18; k++) ok = ok && std::isfinite(p[k]);
       if (!ok) return fail(h, MPMB_ERR_INVALID, "script entry %lld of body %d is not finite", (long long)e, b);
     }
-  if (n > h->script_cap) {   // geometric growth: a fixed frame length allocates once (and keeps the captured graphs)
-    const size_t cap = std::max(n, 2 * h->script_cap);
-    cudaFree(h->script);
-    h->script = nullptr;
-    h->script_cap = 0;
-    CUDA_TRY(h, cudaMalloc(&h->script, sizeof(double) * cap));
-    h->script_cap = cap;
-    h->M.script = h->script;
+  if (n > h->script.size()) {   // geometric growth: a fixed frame length allocates once (and keeps the captured graphs)
+    CUDA_TRY(h, h->script.alloc(std::max(n, 2 * h->script.size())));
     graph_reset(h);
   }
-  if (n) CUDA_TRY(h, cudaMemcpyAsync(h->script, poses, sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->M.cursor, 0, sizeof(int), h->stream));
+  if (n) CUDA_TRY(h, cudaMemcpyAsync(h->script.get(), poses, sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->cursor.get(), 0, sizeof(int), h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));   // the caller owns `poses`
   h->script_left = n_substeps;
   return MPMB_OK;
@@ -4148,13 +4109,13 @@ int mpmb_set_rigid_script(MpmbHandle h, int32_t n_substeps, const double *poses)
 
 // after the second apic_b-velocity transfer of a substep: level-set impulses, then the advance (one script entry)
 static void launch_rigid_motion(MpmbEngine *h) {
-  MotionView M = h->M;   // without a level set there are no contacts: the advance must not read the buffer
-  M.collide = h->motion_collide && h->P.has_sdf;   // (changing the level set resets the captured graphs)
+  const RigidView R = rigid_view(h);
+  const MotionView M = motion_view(h);
   if (M.collide) {
-    k_rigid_contacts<<<(h->R.n_samples + 127) / 128, 128, 0, h->stream>>>(h->R, M, h->P, h->sdf4);
+    k_rigid_contacts<<<(R.n_samples + 127) / 128, 128, 0, h->stream>>>(R, M, h->P, h->sdf4.get());
     h->launches++;
   }
-  k_rigid_advance<<<1, 32, 0, h->stream>>>(h->R, M, h->P, make_float3(h->cfg.gravity[0], h->cfg.gravity[1], h->cfg.gravity[2]));
+  k_rigid_advance<<<1, 32, 0, h->stream>>>(R, M, h->P, make_float3(h->cfg.gravity[0], h->cfg.gravity[1], h->cfg.gravity[2]));
   h->launches++;
   if (h->motion_scripted) h->script_left--;
 }
@@ -4165,22 +4126,22 @@ int mpmb_set_particle_states(MpmbHandle h, int64_t n, const uint32_t *states) {
   if (n < 0 || (n > 0 && !states)) return fail(h, MPMB_ERR_INVALID, "bad argument");
   int rc = rigid_reserve_ids(h, std::max<int64_t>(n, h->cap));
   if (rc != MPMB_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(h->R.p_states, states, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(h->p_states.get(), states, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   return MPMB_OK;
 }
 
 int mpmb_get_particle_cdf(MpmbHandle h, int64_t n, uint32_t *states, float *normal3, float *distance, uint8_t *near_boundary) {
   CHECK_HANDLE(h);
-  if (!h->rigid_on || !h->R.p_states) return fail(h, MPMB_ERR_STATE, "no rigid bodies / no substep yet");
-  if (n < 0 || n > h->R.id_cap) return fail(h, MPMB_ERR_INVALID, "n exceeds the %d particle ids tracked", h->R.id_cap);
+  if (!h->rigid_on || !h->p_states.get()) return fail(h, MPMB_ERR_STATE, "no rigid bodies / no substep yet");
+  if (n < 0 || n > (int64_t)h->p_states.size()) return fail(h, MPMB_ERR_INVALID, "n exceeds the %d particle ids tracked", (int)h->p_states.size());
   std::vector<float4> cdf((size_t)n);
   std::vector<uint32_t> mark((size_t)n);
   uint32_t epoch = 0;
-  CUDA_TRY(h, cudaMemcpyAsync(&epoch, h->R.epoch, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-  if (states) CUDA_TRY(h, cudaMemcpyAsync(states, h->R.p_states, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(mark.data(), h->R.p_mark, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(cdf.data(), h->R.p_cdf, sizeof(float4) * n, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(&epoch, h->epoch.get(), sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  if (states) CUDA_TRY(h, cudaMemcpyAsync(states, h->p_states.get(), sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(mark.data(), h->p_mark.get(), sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(cdf.data(), h->p_cdf.get(), sizeof(float4) * n, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   for (int64_t i = 0; i < n; i++) {   // particles gather_cdf did not see in the last substep: distance 0, normal 0, not near (138-146)
     const bool fresh = (mark[i] >> 1) == epoch;
@@ -4194,11 +4155,11 @@ int mpmb_get_particle_cdf(MpmbHandle h, int64_t n, uint32_t *states, float *norm
 int mpmb_download_cdf(MpmbHandle h, uint32_t *node_states, float *node_distance) {
   CHECK_HANDLE(h);
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies");
-  const size_t nn = h->rigid_nodes;
+  const size_t nn = h->node_key.size();
   std::vector<unsigned long long> key(nn);
   std::vector<uint32_t> tags(nn);
-  CUDA_TRY(h, cudaMemcpyAsync(key.data(), h->R.node_key, sizeof(unsigned long long) * nn, cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(tags.data(), h->R.node_tags, sizeof(uint32_t) * nn, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(key.data(), h->node_key.get(), sizeof(unsigned long long) * nn, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(tags.data(), h->node_tags.get(), sizeof(uint32_t) * nn, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   for (size_t i = 0; i < nn; i++) {
     const bool has = key[i] != CDF_NO_KEY;
@@ -4253,8 +4214,8 @@ int mpmb_rasterize(MpmbHandle h) {
   if (h->cap > 0) k_p2g<<<h->grid_p2g, P2G_T, P2G_DYN_BYTES, h->stream>>>(V, h->P, 0);
   h->launches += 1;
   if (h->cap > 0 && h->rigid_on) {  // block_op_rigid for the tiles of rigid pages, then apply_tmp_velocity (src/transfer.cpp:578-580)
-    k_p2g_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, h->R);
-    k_rigid_apply<<<1, 32, 0, h->stream>>>(h->R);
+    k_p2g_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h));
+    k_rigid_apply<<<1, 32, 0, h->stream>>>(rigid_view(h));
     h->launches += 2;
   }
   prof_end(h, 1);
@@ -4268,11 +4229,11 @@ static void launch_g2p(MpmbEngine *h, const View &V, int part, int commit, bool 
   bool ext = false;
   for (int g = 0; g < MPMB_MAX_GROUPS; g++) ext |= h->P.mats[g].kind > MAT_SAND;
   if (ext) {
-    if (store_b) k_g2p<128, true, true><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel, part, commit);
-    else k_g2p<128, false, true><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel, part, commit);
+    if (store_b) k_g2p<128, true, true><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel.get(), part, commit);
+    else k_g2p<128, false, true><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel.get(), part, commit);
   } else {
-    if (store_b) k_g2p<128, true, false><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel, part, commit);
-    else k_g2p<128, false, false><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel, part, commit);
+    if (store_b) k_g2p<128, true, false><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel.get(), part, commit);
+    else k_g2p<128, false, false><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel.get(), part, commit);
   }
 }
 
@@ -4283,17 +4244,17 @@ int mpmb_resample(MpmbHandle h) {
   if (motion && h->motion_scripted && h->script_left < 1) return fail(h, MPMB_ERR_STATE, "the rigid script has no entry left for this substep");
   View V = make_view(h);
   prof_begin(h, 4);
-  if (h->cap > 0) k_grid<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, h->vel, 0);
+  if (h->cap > 0) k_grid<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, h->vel.get(), 0);
   prof_end(h, 1);
   prof_begin(h, 2);
   if (h->cap > 0) {
     if (h->rigid_on) {
-      k_g2p_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, h->R, h->vel);
+      k_g2p_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h), h->vel.get());
       h->launches += 1;
     }
     launch_g2p(h, V, 0, 1, !h->skip_b || h->rigid_on);   // rigid tiles read apic_b back (the impulse needs dt * force)
     if (h->rigid_on) {
-      k_rigid_apply<<<1, 32, 0, h->stream>>>(h->R);       // src/transfer.cpp:967-969
+      k_rigid_apply<<<1, 32, 0, h->stream>>>(rigid_view(h));       // src/transfer.cpp:967-969
       h->launches += 1;
     }
   }
@@ -4341,7 +4302,7 @@ int mpmb_resample_part(MpmbHandle h, int32_t part) {
   View V = make_view(h);
   int nl = 2;
   if (h->cap > 0) {
-    k_grid<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, h->vel, part);
+    k_grid<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, h->vel.get(), part);
     launch_g2p(h, V, part, part == 1 ? 1 : 0, true);
   }
   h->launches += nl;
@@ -4415,7 +4376,7 @@ int mpmb_substep(MpmbHandle h, int32_t nsub) {
   if (nsub > 0 && h->rigid_on && h->motion_on && h->motion_scripted && h->script_left < nsub)
     return fail(h, MPMB_ERR_STATE, "the rigid script has %lld entries left, %d substeps asked", (long long)h->script_left, nsub);
   // the by-id colour arrays cover every id before any capture: allocating them inside one would end graph replay for good
-  if (nsub > 0 && h->rigid_on && h->cap > 0 && (!h->R.p_states || h->R.id_cap < h->id_span) &&
+  if (nsub > 0 && h->rigid_on && h->cap > 0 && (!h->p_states.get() || (int64_t)h->p_states.size() < h->id_span) &&
       (rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap))) != MPMB_OK)
     return rc;
   // the first substep after an upload takes the radix-sorted arrival lists (a different ordering launch): never in a graph
@@ -4447,15 +4408,13 @@ int mpmb_download_grid(MpmbHandle h, int32_t which, float *dense4) {
   if (h->stage != 2) return fail(h, MPMB_ERR_STATE, "the grid exists between rasterize and resample");
   if (!dense4 || which < 0 || which > 1) return fail(h, MPMB_ERR_INVALID, "bad argument");
   size_t n = (size_t)h->P.nnode[0] * h->P.nnode[1] * h->P.nnode[2];
-  float4 *d = nullptr;
-  CUDA_TRY(h, cudaMalloc(&d, sizeof(float4) * n));
+  DevBuf<float4> d;
+  CUDA_TRY(h, d.alloc(n));
   View V = make_view(h);
-  k_dense_grid<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, which, d);
+  k_dense_grid<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, which, d.get());
   h->launches++;
-  cudaError_t e = cudaMemcpyAsync(dense4, d, sizeof(float4) * n, cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-  cudaFree(d);
-  CUDA_TRY(h, e);
+  CUDA_TRY(h, cudaMemcpyAsync(dense4, d.get(), sizeof(float4) * n, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   return MPMB_OK;
 }
 
@@ -4467,7 +4426,7 @@ extern "C" int mpmb_debug_check(MpmbHandle h, int *out8) {
   CHECK_HANDLE(h);
   cudaStreamSynchronize(h->stream);
   Counters c;
-  if (cudaMemcpy(&c, h->cnt, sizeof(c), cudaMemcpyDeviceToHost) != cudaSuccess) return MPMB_ERR_CUDA;
+  if (cudaMemcpy(&c, h->cnt.get(), sizeof(c), cudaMemcpyDeviceToHost) != cudaSuccess) return MPMB_ERR_CUDA;
   for (int k = 0; k < 8; k++) out8[k] = c.chk[k];
   out8[4] = c.n_store; out8[5] = c.n_alive; out8[6] = c.n_movers; out8[7] = c.n_tiles;
   return MPMB_OK;
@@ -4487,9 +4446,9 @@ extern "C" int mpmb_debug_dense(MpmbHandle h, int which, int *out) {
 extern "C" int mpmb_debug_rows(MpmbHandle h, int n, uint32_t *keys, float *mass4, int *counters8) {
   CHECK_HANDLE(h);
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  if (keys) CUDA_TRY(h, cudaMemcpy(keys, h->keys[h->cur], sizeof(uint32_t) * n, cudaMemcpyDeviceToHost));
-  if (mass4) CUDA_TRY(h, cudaMemcpy(mass4, h->q[h->cur][0], sizeof(float4) * n, cudaMemcpyDeviceToHost));
-  if (counters8) CUDA_TRY(h, cudaMemcpy(counters8, h->cnt, sizeof(Counters), cudaMemcpyDeviceToHost));
+  if (keys) CUDA_TRY(h, cudaMemcpy(keys, h->keys[h->cur].get(), sizeof(uint32_t) * n, cudaMemcpyDeviceToHost));
+  if (mass4) CUDA_TRY(h, cudaMemcpy(mass4, h->q[h->cur][0].get(), sizeof(float4) * n, cudaMemcpyDeviceToHost));
+  if (counters8) CUDA_TRY(h, cudaMemcpy(counters8, h->cnt.get(), sizeof(Counters), cudaMemcpyDeviceToHost));
   return MPMB_OK;
 }
 #endif  // MPMB_DEBUG_EXPORTS
@@ -4519,7 +4478,7 @@ int mpmb_get_counters(MpmbHandle h, int64_t *active_tiles, int64_t *alive, int64
   int rc = mpmb_synchronize(h);
   if (rc != MPMB_OK) return rc;
   Counters c;
-  CUDA_TRY(h, cudaMemcpy(&c, h->cnt, sizeof(c), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(&c, h->cnt.get(), sizeof(c), cudaMemcpyDeviceToHost));
   if (active_tiles) *active_tiles = c.n_tiles;
   if (alive) *alive = c.n_alive;
   if (kernel_launches) *kernel_launches = h->launches;
@@ -4532,7 +4491,7 @@ int mpmb_get_ordering_stats(MpmbHandle h, int64_t *rows, int64_t *movers, int64_
   int rc = mpmb_synchronize(h);
   if (rc != MPMB_OK) return rc;
   Counters c;
-  CUDA_TRY(h, cudaMemcpy(&c, h->cnt, sizeof(c), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(&c, h->cnt.get(), sizeof(c), cudaMemcpyDeviceToHost));
   if (rows) *rows = c.n_store;
   if (movers) *movers = c.n_movers;
   if (ghost_tiles) *ghost_tiles = c.n_ghost;
@@ -4619,7 +4578,7 @@ int mpmb_migrate_unpack(MpmbHandle h, int32_t face, const void *dev_buf) {
   const char *b = (const char *)dev_buf;
   View V = make_view(h);
   k_migrate_unpack<<<64, 256, 0, h->stream>>>(V, h->P, (int)h->mig_cap, (const int *)b, (const float4 *)(b + 16));
-  k_migrate_commit<<<1, 1, 0, h->stream>>>(h->cnt, (const int *)b, (int)h->mig_cap, (int)h->cap);
+  k_migrate_commit<<<1, 1, 0, h->stream>>>(h->cnt.get(), (const int *)b, (int)h->mig_cap, (int)h->cap);
   h->launches += 2;
   prof_end(h, 2);
   CUDA_TRY(h, cudaGetLastError());
@@ -4631,7 +4590,7 @@ int mpmb_migrate_unpack(MpmbHandle h, int32_t face, const void *dev_buf) {
 int mpmb_xchg_buffer(MpmbHandle h, int32_t kind, int32_t face, void **dev_ptr) {
   CHECK_HANDLE(h);
   if (h->cfg.world <= 1 || kind < 0 || kind > 1 || face < 0 || face > 1 || !dev_ptr) return fail(h, MPMB_ERR_INVALID, "bad argument");
-  *dev_ptr = h->rx[kind][face];
+  *dev_ptr = h->rx[kind][face].get();
   return MPMB_OK;
 }
 
@@ -4640,7 +4599,7 @@ int mpmb_xchg_ipc_handle(MpmbHandle h, int32_t kind, int32_t face, void *out64) 
   if (h->cfg.world <= 1 || kind < 0 || kind > 1 || face < 0 || face > 1 || !out64) return fail(h, MPMB_ERR_INVALID, "bad argument");
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
   cudaIpcMemHandle_t hd;
-  CUDA_TRY(h, cudaIpcGetMemHandle(&hd, h->rx[kind][face]));
+  CUDA_TRY(h, cudaIpcGetMemHandle(&hd, h->rx[kind][face].get()));
   memcpy(out64, &hd, 64);
   return MPMB_OK;
 }
@@ -4664,8 +4623,8 @@ int mpmb_xchg_connect(MpmbHandle h, int32_t kind, int32_t face, const void *hand
   }
   // a (re)connection restarts the sequence: my own receive headers of this kind must not hold an old, larger seq
   for (int f = 0; f < 2; f++)
-    if (h->rx[kind][f]) CUDA_TRY(h, cudaMemset(h->rx[kind][f], 0, 16));
-  CUDA_TRY(h, cudaMemset(&h->cnt->xstep, 0, sizeof(int)));
+    if (h->rx[kind][f].get()) CUDA_TRY(h, cudaMemset(h->rx[kind][f].get(), 0, 16));
+  CUDA_TRY(h, cudaMemset(&h->cnt.get()->xstep, 0, sizeof(int)));
   h->xstep = 0;
   graph_reset(h);
   return MPMB_OK;
@@ -4686,7 +4645,7 @@ static void xfaces(MpmbEngine *h, int kind, XFace f[2], int *mask) {
   *mask = 0;
   for (int k = 0; k < 2; k++) {
     f[k].tx = h->tx[kind][k];
-    f[k].rx = h->rx[kind][k];
+    f[k].rx = h->rx[kind][k].get();
     f[k].layer = 0;
     f[k].key = h->special_min + (k == 0 ? SPECIAL_MIG_DOWN : SPECIAL_MIG_UP);
     if (h->tx[kind][k]) *mask |= 1 << k;
@@ -4704,8 +4663,8 @@ static int xchg_halo_launch(MpmbEngine *h, int mask_send, int mask_recv) {
   View V = make_view(h);
   int nl = 0;
   if (mask_send & mask) {
-    k_halo_send2<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, (int)halo_cap_xy(h), (int)halo_idx_bytes(h), s[0], s[1], mask_send & mask, h->xcount,
-                                                         h->xcount + 16);
+    k_halo_send2<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, (int)halo_cap_xy(h), (int)halo_idx_bytes(h), s[0], s[1], mask_send & mask, h->xcount.get(),
+                                                         h->xcount.get() + 16);
     nl++;
   }
   if (mask_recv & mask) {
@@ -4726,7 +4685,7 @@ static int xchg_migrate_launch(MpmbEngine *h, int mask_send, int mask_recv) {
   View V = make_view(h);
   int nl = 0;
   if (mask_send & mask) {
-    k_migrate_send2<<<h->num_sms * 2, 256, 0, h->stream>>>(V, h->key_dead, (int)h->mig_cap, f[0], f[1], mask_send & mask, h->xcount + 8, h->xcount + 20);
+    k_migrate_send2<<<h->num_sms * 2, 256, 0, h->stream>>>(V, h->key_dead, (int)h->mig_cap, f[0], f[1], mask_send & mask, h->xcount.get() + 8, h->xcount.get() + 20);
     nl++;
   }
   if (mask_recv & mask) {
@@ -4787,23 +4746,23 @@ static int recut_allowed(MpmbEngine *h, const char *what) {
 
 // the scratch of the re-cut kernels: the layer histogram, then {bad arrivals, largest id}
 static int recut_reserve(MpmbEngine *h) {
-  if (!h->recut_buf) CUDA_TRY(h, cudaMalloc(&h->recut_buf, sizeof(unsigned long long) * (h->nt2_global + 1)));
+  CUDA_TRY(h, h->recut_buf.reserve(h->nt2_global + 1));   // allocated once: nt2_global does not change
   return MPMB_OK;
 }
-static int *recut_ints(MpmbEngine *h) { return (int *)(h->recut_buf + h->nt2_global); }
+static int *recut_ints(MpmbEngine *h) { return (int *)(h->recut_buf.get() + h->nt2_global); }
 
 // live rows per global tile layer into counts[nt2_global] (synchronises; nt2_global counters cross the bus)
 static int layer_hist(MpmbEngine *h, int64_t *counts) {
   int rc = recut_reserve(h);
   if (rc != MPMB_OK) return rc;
   const int nl = h->nt2_global;
-  CUDA_TRY(h, cudaMemsetAsync(h->recut_buf, 0, sizeof(unsigned long long) * nl, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->recut_buf.get(), 0, sizeof(unsigned long long) * nl, h->stream));
   if (h->cap > 0) {
-    k_layer_hist<<<h->num_sms * 4, 256, 0, h->stream>>>(h->keys[h->cur], h->q[h->cur][0], h->special_min, h->P.inv_dx, nl, h->cnt, h->recut_buf);
+    k_layer_hist<<<h->num_sms * 4, 256, 0, h->stream>>>(h->keys[h->cur].get(), h->q[h->cur][0].get(), h->special_min, h->P.inv_dx, nl, h->cnt.get(), h->recut_buf.get());
     h->launches++;
   }
   static_assert(sizeof(int64_t) == sizeof(unsigned long long), "64-bit counters");
-  CUDA_TRY(h, cudaMemcpyAsync(counts, h->recut_buf, sizeof(int64_t) * nl, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(counts, h->recut_buf.get(), sizeof(int64_t) * nl, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
   return MPMB_OK;
@@ -4845,11 +4804,11 @@ int mpmb_recut_pack(MpmbHandle h, const int32_t *cuts, void *dev_buf, int64_t ca
   int64_t off = 0;
   for (int d = 0; d < world; d++) {   // grouped by destination in ascending rank order, storage order within a destination
     if (counts[d] == 0) continue;
-    k_layer_flags<<<(ns + 255) / 256, 256, 0, h->stream>>>(h->keys[h->cur], h->q[h->cur][0], ns, h->special_min, h->P.inv_dx, cuts[d], cuts[d + 1], h->scan_a);
+    k_layer_flags<<<(ns + 255) / 256, 256, 0, h->stream>>>(h->keys[h->cur].get(), h->q[h->cur][0].get(), ns, h->special_min, h->P.inv_dx, cuts[d], cuts[d + 1], h->scan_a.get());
     int got = 0;
     if ((rc = scan_flags(h, (size_t)ns, &got)) != MPMB_OK) return rc;
     if (got != counts[d]) return fail(h, MPMB_ERR_STATE, "rank %d: %d rows flagged, %lld counted", d, got, (long long)counts[d]);
-    k_recut_pack<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, ns, h->scan_b, (float4 *)dev_buf + (size_t)off * N_Q);
+    k_recut_pack<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, ns, h->scan_b.get(), (float4 *)dev_buf + (size_t)off * N_Q);
     h->launches += 2;
     off += counts[d];
   }
@@ -4877,7 +4836,7 @@ int mpmb_recut_apply(MpmbHandle h, int32_t tile_z0, int32_t tile_z1, int64_t n_i
   // checks first: what stays, whether every arrival belongs here, whether a configured capacity holds both
   if (ns > 0) {
     if ((rc = scan_reserve(h, (size_t)ns)) != MPMB_OK) return rc;
-    k_layer_flags<<<(ns + 255) / 256, 256, 0, h->stream>>>(h->keys[h->cur], h->q[h->cur][0], ns, h->special_min, h->P.inv_dx, tile_z0, tile_z1, h->scan_a);
+    k_layer_flags<<<(ns + 255) / 256, 256, 0, h->stream>>>(h->keys[h->cur].get(), h->q[h->cur][0].get(), ns, h->special_min, h->P.inv_dx, tile_z0, tile_z1, h->scan_a.get());
     h->launches++;
     if ((rc = scan_flags(h, (size_t)ns, &kept)) != MPMB_OK) return rc;
   }
@@ -4905,7 +4864,7 @@ int mpmb_recut_apply(MpmbHandle h, int32_t tile_z0, int32_t tile_z1, int64_t n_i
   h->cfg.tile_z1 = tile_z1;
   if (h->cap > 0) {
     if (kept > 0) {   // the staying rows, compacted in storage order into the other buffer, re-keyed; departing rows are left behind
-      k_recut_keep<<<std::min((ns + 255) / 256, h->num_sms * 8), 256, 0, h->stream>>>(make_view(h), h->P, ns, h->scan_b, ints + 1);
+      k_recut_keep<<<std::min((ns + 255) / 256, h->num_sms * 8), 256, 0, h->stream>>>(make_view(h), h->P, ns, h->scan_b.get(), ints + 1);
       h->launches++;
     }
     h->cur ^= 1;
@@ -4940,19 +4899,12 @@ static int async_check(MpmbEngine *h, bool need_init) {
 // room for `need` records in both buffers of a pool, keeping the current records (grows by at least half, as
 // grow_keeping_rows does for the resident set)
 static int apool_reserve(MpmbEngine *h, MpmbEngine::APool &p, int64_t need) {
-  if (need <= p.cap) return MPMB_OK;
-  const int64_t want = std::max<int64_t>(need, p.cap + p.cap / 2);
-  void *nb[2] = {};
-  for (int b = 0; b < 2; b++) {
-    cudaError_t e = cudaMalloc(&nb[b], sizeof(float) * AREC_WORDS * (size_t)want);
-    if (e != cudaSuccess) {
-      cudaFree(nb[0]);
-      h->sticky_cuda = true;
-      return fail(h, MPMB_ERR_CUDA, "cudaMalloc of an AsyncMPM pool failed: %s", cudaGetErrorString(e));
-    }
-  }
-  ARec n0 = arec_layout(nb[0], want);
-  const ARec &o = p.r[p.cur];
+  const int64_t cap = arec_cap(p.buf[0]);
+  if (need <= cap) return MPMB_OK;
+  const int64_t want = std::max<int64_t>(need, cap + cap / 2);
+  DevBuf<float> nb[2];
+  for (auto &b : nb) CUDA_TRY(h, b.alloc((size_t)AREC_WORDS * want));
+  const ARec n0 = arec_of(nb[0]), o = p.rec(p.cur);
   const size_t n = (size_t)p.n;
   if (n > 0) {
     const struct { void *d; const void *s; size_t w; } cp[] = {{n0.x, o.x, 3}, {n0.v, o.v, 3}, {n0.F, o.F, 9}, {n0.b, o.b, 9}, {n0.mass, o.mass, 1},
@@ -4961,13 +4913,8 @@ static int apool_reserve(MpmbEngine *h, MpmbEngine::APool &p, int64_t need) {
     for (const auto &c : cp) CUDA_TRY(h, cudaMemcpyAsync(c.d, c.s, 4 * c.w * n, cudaMemcpyDeviceToDevice, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   }
-  for (int b = 0; b < 2; b++) cudaFree(p.buf[b]);
-  p.buf[0] = nb[0];
-  p.buf[1] = nb[1];
-  p.r[0] = n0;
-  p.r[1] = arec_layout(nb[1], want);
+  for (int b = 0; b < 2; b++) p.buf[b] = std::move(nb[b]);
   p.cur = 0;
-  p.cap = want;
   return MPMB_OK;
 }
 
@@ -4979,13 +4926,13 @@ static int apool_split(MpmbEngine *h, MpmbEngine::APool &p, int bit, MpmbEngine:
   if (n == 0) return MPMB_OK;
   int rc, moved = 0;
   if ((rc = scan_reserve(h, (size_t)n)) != MPMB_OK) return rc;
-  k_async_rec_flags<<<nblocks(n), 256, 0, h->stream>>>(p.r[p.cur].block, n, h->a_bfl, bit, h->scan_a);
+  k_async_rec_flags<<<nblocks(n), 256, 0, h->stream>>>(p.rec(p.cur).block, n, h->a_bfl.get(), bit, h->scan_a.get());
   h->launches++;
   if ((rc = scan_flags(h, (size_t)n, &moved)) != MPMB_OK) return rc;
   if (moved == 0) return MPMB_OK;
   if (to && (rc = apool_reserve(h, *to, to->n + moved)) != MPMB_OK) return rc;
-  k_async_split<<<nblocks(n), 256, 0, h->stream>>>(p.r[p.cur], n, h->scan_a, h->scan_b, to ? to->r[to->cur] : ARec{}, to ? (int)to->n : 0, to ? 1 : 0,
-                                                    p.r[p.cur ^ 1], 0, 1);
+  k_async_split<<<nblocks(n), 256, 0, h->stream>>>(p.rec(p.cur), n, h->scan_a.get(), h->scan_b.get(), to ? to->rec(to->cur) : ARec{}, to ? (int)to->n : 0,
+                                                    to ? 1 : 0, p.rec(p.cur ^ 1), 0, 1);
   h->launches++;
   CUDA_TRY(h, cudaGetLastError());
   p.cur ^= 1;
@@ -5007,17 +4954,22 @@ int mpmb_async_init(MpmbHandle h, const int32_t nb[3], float inv_dx) {
   const int64_t nblk = (int64_t)nb[0] * nb[1] * nb[2];
   if (nblk >= (1ll << 30)) return fail(h, MPMB_ERR_INVALID, "too many scheduler blocks");
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  async_free(h);
+  // empty pools and no gather scratch: every capacity starts again from nothing
+  for (auto &p : h->apool) p = MpmbEngine::APool{};
+  h->a_gbuf.reset(); h->a_sbuf.reset(); h->a_rowk.reset(); h->a_cub.reset();
+  for (auto &k : h->a_key) k.reset();
+  for (auto &u : h->a_u) u.reset();
+  h->async_on = false;
   for (int d = 0; d < 3; d++) h->anb[d] = nb[d];
   h->nblk = (int)nblk;
   h->a_inv_dx = inv_dx;
-  CUDA_TRY(h, cudaMalloc(&h->a_bfl, (size_t)nblk));
-  CUDA_TRY(h, cudaMalloc(&h->a_bflag, sizeof(uint32_t) * nblk));
-  CUDA_TRY(h, cudaMalloc(&h->a_bmin, sizeof(int) * nblk));
-  CUDA_TRY(h, cudaMalloc(&h->a_bmax, sizeof(int) * nblk));
-  CUDA_TRY(h, cudaMalloc(&h->a_blk, sizeof(int) * nblk));
-  CUDA_TRY(h, cudaMalloc(&h->a_lim, sizeof(float) * 2 * nblk));
-  CUDA_TRY(h, cudaMalloc(&h->a_bad, sizeof(int)));
+  CUDA_TRY(h, h->a_bfl.alloc(nblk));
+  CUDA_TRY(h, h->a_bflag.alloc(nblk));
+  CUDA_TRY(h, h->a_bmin.alloc(nblk));
+  CUDA_TRY(h, h->a_bmax.alloc(nblk));
+  CUDA_TRY(h, h->a_blk.alloc(nblk));
+  CUDA_TRY(h, h->a_lim.alloc(2 * nblk));
+  CUDA_TRY(h, h->a_bad.alloc(1));
   for (auto &p : h->apool)
     if ((rc = apool_reserve(h, p, 1024)) != MPMB_OK) return rc;
   h->async_on = true;
@@ -5035,17 +4987,17 @@ int mpmb_async_add(MpmbHandle h, int32_t which, int64_t n, const float *x, const
   MpmbEngine::APool &p = h->apool[which];
   if (p.n + n >= (1ll << 30)) return fail(h, MPMB_ERR_CAPACITY, "an AsyncMPM pool holds fewer than 2^30 records");
   if ((rc = apool_reserve(h, p, p.n + n)) != MPMB_OK) return rc;
-  const ARec &r = p.r[p.cur];
+  const ARec r = p.rec(p.cur);
   const size_t o = (size_t)p.n;
   const struct { void *d; const void *s; size_t w; } cp[] = {{r.x + 3 * o, x, 3}, {r.v + 3 * o, v, 3}, {r.F + 9 * o, F, 9}, {r.b + 9 * o, b, 9},
                                                             {r.mass + o, mass, 1}, {r.vol + o, vol, 1}, {r.scalar + o, scalar, 1}, {r.group + o, group, 1},
                                                             {r.id + o, id, 1}};
   for (const auto &c : cp) CUDA_TRY(h, cudaMemcpyAsync(c.d, c.s, 4 * c.w * (size_t)n, cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->a_bad, 0, sizeof(int), h->stream));
-  k_async_blocks<<<nblocks(n), 256, 0, h->stream>>>(r.x + 3 * o, (int)n, h->a_inv_dx, h->anb[0], h->anb[1], h->anb[2], r.block + o, h->a_bad);
+  CUDA_TRY(h, cudaMemsetAsync(h->a_bad.get(), 0, sizeof(int), h->stream));
+  k_async_blocks<<<nblocks(n), 256, 0, h->stream>>>(r.x + 3 * o, (int)n, h->a_inv_dx, h->anb[0], h->anb[1], h->anb[2], r.block + o, h->a_bad.get());
   h->launches++;
   int bad = 0;
-  CUDA_TRY(h, cudaMemcpyAsync(&bad, h->a_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(&bad, h->a_bad.get(), sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
   if (bad) return fail(h, MPMB_ERR_INVALID, "%d records lie outside the %d x %d x %d scheduler blocks", bad, h->anb[0], h->anb[1], h->anb[2]);
@@ -5061,31 +5013,31 @@ int mpmb_async_block_limits(MpmbHandle h, int32_t with_limits, int64_t cap, int6
   *n_blocks = 0;
   const int nblk = h->nblk;
   const MpmbEngine::APool &p = h->apool[0];
-  CUDA_TRY(h, cudaMemsetAsync(h->a_bflag, 0, sizeof(uint32_t) * nblk, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->a_bad, 0, sizeof(int), h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->a_bflag.get(), 0, sizeof(uint32_t) * nblk, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->a_bad.get(), 0, sizeof(int), h->stream));
   if (with_limits) {
-    k_fill_u32<<<nblocks(nblk), 256, 0, h->stream>>>((uint32_t *)h->a_bmin, nblk, 0x3dcccccdu);   // 0.1f
-    k_fill_u32<<<nblocks(nblk), 256, 0, h->stream>>>((uint32_t *)h->a_bmax, nblk, 0x2539705fu);   // 1e-16f
+    k_fill_u32<<<nblocks(nblk), 256, 0, h->stream>>>((uint32_t *)h->a_bmin.get(), nblk, 0x3dcccccdu);   // 0.1f
+    k_fill_u32<<<nblocks(nblk), 256, 0, h->stream>>>((uint32_t *)h->a_bmax.get(), nblk, 0x2539705fu);   // 1e-16f
     h->launches += 2;
   }
   if (p.n > 0) {
-    k_async_limits<<<nblocks(p.n), 256, 0, h->stream>>>(p.r[p.cur], (int)p.n, h->P, with_limits ? 1 : 0, h->a_bflag, h->a_bmin, h->a_bmax, h->a_bad);
+    k_async_limits<<<nblocks(p.n), 256, 0, h->stream>>>(p.rec(p.cur), (int)p.n, h->P, with_limits ? 1 : 0, h->a_bflag.get(), h->a_bmin.get(), h->a_bmax.get(), h->a_bad.get());
     h->launches++;
   }
   int bad = 0, total = 0;
-  CUDA_TRY(h, cudaMemcpyAsync(&bad, h->a_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(&bad, h->a_bad.get(), sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   if ((rc = scan_reserve(h, (size_t)nblk)) != MPMB_OK) return rc;
-  k_async_occupied<<<nblocks(nblk), 256, 0, h->stream>>>(h->a_bflag, nblk, h->scan_a);
+  k_async_occupied<<<nblocks(nblk), 256, 0, h->stream>>>(h->a_bflag.get(), nblk, h->scan_a.get());
   h->launches++;
   if ((rc = scan_flags(h, (size_t)nblk, &total)) != MPMB_OK) return rc;
   if (bad) return fail(h, MPMB_ERR_INVALID, "%d pool particles are of a type without a time-step limit (linear / jelly)", bad);
   *n_blocks = total;
   if (total > cap) return fail(h, MPMB_ERR_CAPACITY, "%d occupied blocks do not fit in the %lld entries provided", total, (long long)cap);
   if (total == 0) return MPMB_OK;
-  float *dmin = h->a_lim, *dmax = h->a_lim + nblk;
-  k_async_block_out<<<nblocks(nblk), 256, 0, h->stream>>>(h->a_bflag, h->a_bmin, h->a_bmax, nblk, h->scan_b, h->a_blk, dmin, dmax);
+  float *dmin = h->a_lim.get(), *dmax = h->a_lim.get() + nblk;
+  k_async_block_out<<<nblocks(nblk), 256, 0, h->stream>>>(h->a_bflag.get(), h->a_bmin.get(), h->a_bmax.get(), nblk, h->scan_b.get(), h->a_blk.get(), dmin, dmax);
   h->launches++;
-  CUDA_TRY(h, cudaMemcpyAsync(block, h->a_blk, sizeof(int) * total, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(block, h->a_blk.get(), sizeof(int) * total, cudaMemcpyDeviceToHost, h->stream));
   if (with_limits) {
     CUDA_TRY(h, cudaMemcpyAsync(min_dt, dmin, sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaMemcpyAsync(max_v2, dmax, sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
@@ -5109,59 +5061,51 @@ int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_
     any_swap |= (flags[i] & MPMB_ASYNC_SWAP) != 0;
     any_clear |= (flags[i] & MPMB_ASYNC_CLEAR) != 0;
   }
-  CUDA_TRY(h, cudaMemcpyAsync(h->a_bfl, flags, (size_t)nblk, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(h->a_bfl.get(), flags, (size_t)nblk, cudaMemcpyHostToDevice, h->stream));
 
   // 1. gather: flagged candidates -> sort by (part, page index) -> first copy of every id -> the set, in that order
   const int np = (int)P0.n, nbk = (int)B0.n;
   const int64_t nc_all = 2 * (int64_t)np + nbk;
   int nc = 0, ng = 0;
+  ARec G{}, S{};   // the gathered set and its survivors
   if (nc_all > 0) {
     if ((rc = scan_reserve(h, (size_t)nc_all)) != MPMB_OK) return rc;
-    k_async_cand_flags<<<nblocks(nc_all), 256, 0, h->stream>>>(P0.r[P0.cur].block, np, B0.r[B0.cur].block, nbk, h->a_bfl, h->scan_a);
+    k_async_cand_flags<<<nblocks(nc_all), 256, 0, h->stream>>>(P0.rec(P0.cur).block, np, B0.rec(B0.cur).block, nbk, h->a_bfl.get(), h->scan_a.get());
     h->launches++;
     if ((rc = scan_flags(h, (size_t)nc_all, &nc)) != MPMB_OK) return rc;
   }
   if (nc > 0) {
-    if (nc > h->a_ccap) {
-      const int64_t want = std::max<int64_t>(nc, h->a_ccap + h->a_ccap / 2);
-      for (int k = 0; k < 2; k++) { cudaFree(h->a_key[k]); h->a_key[k] = nullptr; }
-      for (auto &u : h->a_u) { cudaFree(u); u = nullptr; }
-      cudaFree(h->a_rowk); cudaFree(h->a_cub);
-      h->a_rowk = nullptr; h->a_cub = nullptr; h->a_ccap = 0; h->a_cub_bytes = 0;
-      for (int k = 0; k < 2; k++) CUDA_TRY(h, cudaMalloc(&h->a_key[k], sizeof(unsigned long long) * want));
-      for (auto &u : h->a_u) CUDA_TRY(h, cudaMalloc(&u, sizeof(uint32_t) * want));
-      CUDA_TRY(h, cudaMalloc(&h->a_rowk, sizeof(int) * want));
+    const int64_t ccap = (int64_t)h->a_rowk.size();   // the candidate capacity
+    if (nc > ccap) {
+      const int64_t want = std::max<int64_t>(nc, ccap + ccap / 2);
+      for (auto &k : h->a_key) k.reset();   // the old candidate scratch goes before the new comes
+      for (auto &u : h->a_u) u.reset();
+      h->a_rowk.reset(); h->a_cub.reset();
+      for (auto &k : h->a_key) CUDA_TRY(h, k.alloc(want));
+      for (auto &u : h->a_u) CUDA_TRY(h, u.alloc(want));
+      CUDA_TRY(h, h->a_rowk.alloc(want));
       size_t b1 = 0, b2 = 0;
-      cub::DeviceRadixSort::SortPairs(nullptr, b1, h->a_key[0], h->a_key[1], h->a_u[0], h->a_u[1], (int)want, 0, 38, h->stream);
-      cub::DeviceRadixSort::SortPairs(nullptr, b2, h->a_u[2], h->a_u[3], h->a_u[0], h->a_u[0], (int)want, 0, 32, h->stream);
-      h->a_cub_bytes = std::max(b1, b2);
-      CUDA_TRY(h, cudaMalloc(&h->a_cub, h->a_cub_bytes));
-      h->a_ccap = want;
+      cub::DeviceRadixSort::SortPairs(nullptr, b1, h->a_key[0].get(), h->a_key[1].get(), h->a_u[0].get(), h->a_u[1].get(), (int)want, 0, 38, h->stream);
+      cub::DeviceRadixSort::SortPairs(nullptr, b2, h->a_u[2].get(), h->a_u[3].get(), h->a_u[0].get(), h->a_u[0].get(), (int)want, 0, 32, h->stream);
+      CUDA_TRY(h, h->a_cub.alloc(std::max(b1, b2)));
     }
     // keys and candidate indices; once sorted, the unsorted candidate list holds the positions sorted by id, and a_rowk
     // (rewritten by the routing) the unsorted positions
-    unsigned long long *key = h->a_key[0], *key_s = h->a_key[1];
-    uint32_t *cand = h->a_u[0], *cand_s = h->a_u[1], *ids = h->a_u[2], *ids_s = h->a_u[3];
-    uint32_t *pos = (uint32_t *)h->a_rowk, *pos_s = h->a_u[0];
-    k_async_cand_keys<<<nblocks(nc_all), 256, 0, h->stream>>>(P0.r[P0.cur].block, np, B0.r[B0.cur].block, nbk, h->scan_a, h->scan_b, h->anb[1], h->anb[2], key, cand);
-    size_t bytes = h->a_cub_bytes;
-    cub::DeviceRadixSort::SortPairs(h->a_cub, bytes, key, key_s, cand, cand_s, nc, 0, 38, h->stream);
-    k_async_cand_ids<<<nblocks(nc), 256, 0, h->stream>>>(cand_s, nc, P0.r[P0.cur].id, np, B0.r[B0.cur].id, ids, pos);
-    bytes = h->a_cub_bytes;
-    cub::DeviceRadixSort::SortPairs(h->a_cub, bytes, ids, ids_s, pos, pos_s, nc, 0, 32, h->stream);
-    k_async_first<<<nblocks(nc), 256, 0, h->stream>>>(ids_s, pos_s, nc, h->scan_a);
+    unsigned long long *key = h->a_key[0].get(), *key_s = h->a_key[1].get();
+    uint32_t *cand = h->a_u[0].get(), *cand_s = h->a_u[1].get(), *ids = h->a_u[2].get(), *ids_s = h->a_u[3].get();
+    uint32_t *pos = (uint32_t *)h->a_rowk.get(), *pos_s = h->a_u[0].get();
+    k_async_cand_keys<<<nblocks(nc_all), 256, 0, h->stream>>>(P0.rec(P0.cur).block, np, B0.rec(B0.cur).block, nbk, h->scan_a.get(), h->scan_b.get(), h->anb[1], h->anb[2], key, cand);
+    size_t bytes = h->a_cub.size();
+    cub::DeviceRadixSort::SortPairs(h->a_cub.get(), bytes, key, key_s, cand, cand_s, nc, 0, 38, h->stream);
+    k_async_cand_ids<<<nblocks(nc), 256, 0, h->stream>>>(cand_s, nc, P0.rec(P0.cur).id, np, B0.rec(B0.cur).id, ids, pos);
+    bytes = h->a_cub.size();
+    cub::DeviceRadixSort::SortPairs(h->a_cub.get(), bytes, ids, ids_s, pos, pos_s, nc, 0, 32, h->stream);
+    k_async_first<<<nblocks(nc), 256, 0, h->stream>>>(ids_s, pos_s, nc, h->scan_a.get());
     h->launches += 5;
     if ((rc = scan_flags(h, (size_t)nc, &ng)) != MPMB_OK) return rc;
-    if (ng > h->a_gcap) {
-      cudaFree(h->a_gbuf);
-      h->a_gbuf = nullptr;
-      h->a_gcap = 0;
-      const int64_t want = std::max<int64_t>(ng, 3 * (int64_t)ng / 2);
-      CUDA_TRY(h, cudaMalloc(&h->a_gbuf, sizeof(float) * AREC_WORDS * (size_t)want));
-      h->a_gcap = want;
-    }
-    h->a_G = arec_layout(h->a_gbuf, h->a_gcap);
-    k_async_gather<<<nblocks(nc), 256, 0, h->stream>>>(cand_s, nc, h->scan_a, h->scan_b, P0.r[P0.cur], np, B0.r[B0.cur], h->a_G);
+    if (ng > arec_cap(h->a_gbuf)) CUDA_TRY(h, h->a_gbuf.alloc((size_t)AREC_WORDS * std::max<int64_t>(ng, 3 * (int64_t)ng / 2)));
+    G = arec_of(h->a_gbuf);
+    k_async_gather<<<nblocks(nc), 256, 0, h->stream>>>(cand_s, nc, h->scan_a.get(), h->scan_b.get(), P0.rec(P0.cur), np, B0.rec(B0.cur), G);
     h->launches++;
     CUDA_TRY(h, cudaGetLastError());
   }
@@ -5179,7 +5123,6 @@ int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_
   if (ng > 0) {
     apply_delta_t(h, dt);
     h->aos_host_pool = nullptr;
-    const ARec &G = h->a_G;
     if ((rc = pack_rows(h, ng, G.x, G.v, G.F, G.b, G.mass, G.vol, G.scalar, G.group, 0, 0)) != MPMB_OK) return rc;
     if ((rc = finish_upload(h, ng)) != MPMB_OK) return rc;
     if ((rc = mpmb_substep(h, 1)) != MPMB_OK) return rc;
@@ -5187,19 +5130,11 @@ int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_
     int ns = 0;
     if ((rc = read_n_store(h, &ns)) != MPMB_OK) return rc;
     if (ns > 0 && (rc = live_prefix(h, ns, &alive)) != MPMB_OK) return rc;
-    if (alive > h->a_scap) {
-      cudaFree(h->a_sbuf);
-      h->a_sbuf = nullptr;
-      h->a_scap = 0;
-      const int64_t want = std::max<int64_t>(alive, h->a_gcap);
-      CUDA_TRY(h, cudaMalloc(&h->a_sbuf, sizeof(float) * AREC_WORDS * (size_t)want));
-      h->a_scap = want;
-    }
-    h->a_S = arec_layout(h->a_sbuf, h->a_scap);
-    const ARec &S = h->a_S;
+    if (alive > arec_cap(h->a_sbuf)) CUDA_TRY(h, h->a_sbuf.alloc((size_t)AREC_WORDS * std::max<int64_t>(alive, arec_cap(h->a_gbuf))));
+    S = arec_of(h->a_sbuf);
     if (alive > 0) {
       unpack_live(h, ns, S.id, S.x, S.v, S.F, S.b, S.mass, S.vol, S.scalar, S.group);
-      k_async_blocks<<<nblocks(alive), 256, 0, h->stream>>>(S.x, (int)alive, h->a_inv_dx, h->anb[0], h->anb[1], h->anb[2], S.block, h->a_bad);
+      k_async_blocks<<<nblocks(alive), 256, 0, h->stream>>>(S.x, (int)alive, h->a_inv_dx, h->anb[0], h->anb[1], h->anb[2], S.block, h->a_bad.get());
       h->launches++;
     }
   }
@@ -5209,19 +5144,19 @@ int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_
 
   // 5. survivors, in gather order, to the pool of their new block (EQUAL) or to the backup (CLEAR, not EQUAL)
   if (alive > 0) {
-    k_fill_u32<<<nblocks(ng), 256, 0, h->stream>>>((uint32_t *)h->a_rowk, ng, 0xffffffffu);
-    k_async_rank<<<nblocks(alive), 256, 0, h->stream>>>(h->a_S.id, (int)alive, h->a_rowk);
+    k_fill_u32<<<nblocks(ng), 256, 0, h->stream>>>((uint32_t *)h->a_rowk.get(), ng, 0xffffffffu);
+    k_async_rank<<<nblocks(alive), 256, 0, h->stream>>>(S.id, (int)alive, h->a_rowk.get());
     h->launches += 2;
     if ((rc = scan_reserve(h, (size_t)ng)) != MPMB_OK) return rc;
     for (int to_backup = 0; to_backup < 2; to_backup++) {
       MpmbEngine::APool &D = to_backup ? B0 : P0;
       int cnt = 0;
-      k_async_route_flags<<<nblocks(ng), 256, 0, h->stream>>>(h->a_rowk, ng, h->a_S.block, h->a_bfl, to_backup, h->scan_a);
+      k_async_route_flags<<<nblocks(ng), 256, 0, h->stream>>>(h->a_rowk.get(), ng, S.block, h->a_bfl.get(), to_backup, h->scan_a.get());
       h->launches++;
       if ((rc = scan_flags(h, (size_t)ng, &cnt)) != MPMB_OK) return rc;
       if (cnt == 0) continue;
       if ((rc = apool_reserve(h, D, D.n + cnt)) != MPMB_OK) return rc;
-      k_async_route<<<nblocks(ng), 256, 0, h->stream>>>(h->a_rowk, ng, h->scan_a, h->scan_b, h->a_S, h->a_G.id, D.r[D.cur], (int)D.n);
+      k_async_route<<<nblocks(ng), 256, 0, h->stream>>>(h->a_rowk.get(), ng, h->scan_a.get(), h->scan_b.get(), S, G.id, D.rec(D.cur), (int)D.n);
       h->launches++;
       D.n += cnt;
     }
@@ -5251,7 +5186,7 @@ int mpmb_async_download(MpmbHandle h, int32_t which, int64_t cap, int64_t *n_out
   const MpmbEngine::APool &p = h->apool[which];
   *n_out = p.n;
   if (p.n > cap) return fail(h, MPMB_ERR_CAPACITY, "%lld records do not fit in the %lld rows provided", (long long)p.n, (long long)cap);
-  const ARec &r = p.r[p.cur];
+  const ARec r = p.rec(p.cur);
   const size_t n = (size_t)p.n;
   const struct { void *d; const void *s; size_t w; } cp[] = {{id, r.id, 1}, {block, r.block, 1}, {x, r.x, 3}, {v, r.v, 3}, {F, r.F, 9}, {b, r.b, 9},
                                                             {mass, r.mass, 1}, {vol, r.vol, 1}, {scalar, r.scalar, 1}, {group, r.group, 1}};

@@ -135,6 +135,19 @@ void warp_release(unsigned mask) {
 }
 }  // namespace simt
 
+// emulated device allocations (simt.h): the live count; simt_fail_allocation(k) makes the k-th cudaMalloc from now fail
+// (k = 0: none) and returns how many allocations the previous setting still had to go (0: it has fired, or there was none)
+namespace simt {
+long long g_live_allocs = 0;
+long long g_fail_in = 0;
+}  // namespace simt
+extern "C" long long simt_device_allocations() { return simt::g_live_allocs; }
+extern "C" long long simt_fail_allocation(long long k) {
+  const long long left = simt::g_fail_in;
+  simt::g_fail_in = k > 0 ? k : 0;
+  return left;
+}
+
 void __syncthreads() {
   simt::Block *b = simt::g_blk;
   simt::Thread &t = b->th[b->cur];

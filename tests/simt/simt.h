@@ -210,8 +210,25 @@ enum cudaMemcpyKind { cudaMemcpyHostToHost = 0, cudaMemcpyHostToDevice = 1, cuda
 struct cudaDeviceProp { char name[256]; int multiProcessorCount; size_t totalGlobalMem; int major, minor; };
 struct cudaIpcMemHandle_t { char reserved[64]; };
 enum { cudaIpcMemLazyEnablePeerAccess = 1 };
-template <class T> static inline cudaError_t cudaMalloc(T **p, size_t n) { void *q = nullptr; if (posix_memalign(&q, 256, n ? n : 256)) return cudaErrorMemoryAllocation; memset(q, 0xCD, n); *p = (T *)q; return cudaSuccess; }
-static inline cudaError_t cudaFree(void *p) { free(p); return cudaSuccess; }
+// live allocations are counted, and one allocation can be made to fail (simt_fail_allocation below), so that tests can check
+// that every allocation is freed, on every error path too
+namespace simt {
+extern long long g_live_allocs;   // device allocations not freed yet
+extern long long g_fail_in;       // > 0: the g_fail_in-th cudaMalloc from now fails
+}
+template <class T> static inline cudaError_t cudaMalloc(T **p, size_t n) {
+  if (simt::g_fail_in > 0 && --simt::g_fail_in == 0) return cudaErrorMemoryAllocation;
+  void *q = nullptr;
+  if (posix_memalign(&q, 256, n ? n : 256)) return cudaErrorMemoryAllocation;
+  memset(q, 0xCD, n);
+  *p = (T *)q;
+  simt::g_live_allocs++;
+  return cudaSuccess;
+}
+static inline cudaError_t cudaFree(void *p) {
+  if (p) { free(p); simt::g_live_allocs--; }
+  return cudaSuccess;
+}
 static inline cudaError_t cudaMemcpy(void *d, const void *s, size_t n, cudaMemcpyKind) { memcpy(d, s, n); return cudaSuccess; }
 static inline cudaError_t cudaMemcpyAsync(void *d, const void *s, size_t n, cudaMemcpyKind, cudaStream_t = nullptr) { memcpy(d, s, n); return cudaSuccess; }
 static inline cudaError_t cudaMemcpy2DAsync(void *d, size_t dp, const void *s, size_t sp, size_t w, size_t h, cudaMemcpyKind, cudaStream_t = nullptr) {
