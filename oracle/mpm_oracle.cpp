@@ -1105,6 +1105,23 @@ template <class R> void g2p_coupled(const Scene<R> &sc, Rigid<R> &rg, Particles<
   rigid_apply_tmp(rg);                                                                          // 967-969
 }
 
+// The first half of the coupled substep: ordering, rigid pages, the colour field, gather_cdf and the coupled rasterize into a
+// zeroed grid (src/mpm.cpp:464-487).  velocity / angular_velocity return with the rasterize's impulses; the visit order is
+// returned for the resample.
+template <class R>
+std::vector<int64_t> rasterize_coupled(const Scene<R> &sc, Rigid<R> &rg, Particles<R> &P, const uint8_t *alive, R *grid, uint32_t *node_state_out,
+                                       R *node_dist_out) {
+  std::fill(grid, grid + sc.n_nodes() * 4, R(0));
+  auto order = visit_order(sc, P, alive);
+  rigid_pages(sc, rg);
+  cdf_rasterize(sc, rg);
+  if (node_state_out) std::memcpy(node_state_out, rg.node_state.data(), sizeof(uint32_t) * sc.n_nodes());
+  if (node_dist_out) std::memcpy(node_dist_out, rg.node_dist.data(), sizeof(R) * sc.n_nodes());
+  gather_cdf(sc, rg, P, alive);
+  p2g_coupled(sc, rg, P, order, grid);
+  return order;
+}
+
 // MPM<3>::substep with rigid bodies (src/mpm.cpp:452-575), without the host-side rigid dynamics (rigidify, articulate,
 // advect_rigid_bodies): one substep at a fixed pose; velocity / angular_velocity return with the impulses of both transfers.
 template <class R>
@@ -1113,14 +1130,7 @@ void substep_coupled(const Scene<R> &sc, Rigid<R> &rg, Particles<R> &P, uint8_t 
   std::vector<R> grid_local;
   R *grid = grid_out;
   if (!grid) { grid_local.assign(sc.n_nodes() * 4, R(0)); grid = grid_local.data(); }
-  else std::fill(grid, grid + sc.n_nodes() * 4, R(0));
-  auto order = visit_order(sc, P, alive);
-  rigid_pages(sc, rg);
-  cdf_rasterize(sc, rg);
-  if (node_state_out) std::memcpy(node_state_out, rg.node_state.data(), sizeof(uint32_t) * sc.n_nodes());
-  if (node_dist_out) std::memcpy(node_dist_out, rg.node_dist.data(), sizeof(R) * sc.n_nodes());
-  gather_cdf(sc, rg, P, alive);
-  p2g_coupled(sc, rg, P, order, grid);
+  auto order = rasterize_coupled(sc, rg, P, alive, grid, node_state_out, node_dist_out);
   if (grid_rast_out) std::memcpy(grid_rast_out, grid, sizeof(R) * sc.n_nodes() * 4);
   grid_update(sc, grid);
   g2p_coupled(sc, rg, P, order, grid);
@@ -1587,6 +1597,18 @@ template <class R> Scene<R> make_scene(const int *res, R dx, R dt, const R *grav
   return sc;
 }
 
+template <class R> Rigid<R> make_rigid(int n_rigid, const R *position, const R *rot, R *velocity, R *angular_velocity, const R *inv_mass,
+                                       const R *inv_inertia, const R *frictions, int64_t n_samples, const R *s_offset, const R *s_tri,
+                                       const int32_t *s_rigid, R penalty, R pushing_force, uint32_t *states, R *bnormal, R *bdist,
+                                       uint8_t *near) {
+  Rigid<R> rg;
+  rg.n_rigid = n_rigid; rg.position = position; rg.rot = rot; rg.velocity = velocity; rg.angular_velocity = angular_velocity;
+  rg.inv_mass = inv_mass; rg.inv_inertia = inv_inertia; rg.frictions = frictions;
+  rg.n_samples = n_samples; rg.offset = s_offset; rg.tri = s_tri; rg.sample_rigid = s_rigid;
+  rg.penalty = penalty; rg.pushing_force = pushing_force; rg.states = states; rg.bnormal = bnormal; rg.bdist = bdist; rg.near = near;
+  return rg;
+}
+
 }  // namespace
 
 // =================================================================================
@@ -1632,13 +1654,29 @@ template <class R> Scene<R> make_scene(const int *res, R dx, R dt, const R *grav
     (void)n_groups;                                                                                                            \
     Scene<R> sc = make_scene<R>(res, dx, dt, gravity, particle_gravity, mat_kind, mat_params, sdf, friction);                  \
     Particles<R> P{n, x, v, F, b, mass, vol, ps, group};                                                                       \
-    Rigid<R> rg;                                                                                                               \
-    rg.n_rigid = n_rigid; rg.position = r_position; rg.rot = r_rot; rg.velocity = r_velocity;                                  \
-    rg.angular_velocity = r_angular_velocity; rg.inv_mass = r_inv_mass; rg.inv_inertia = r_inv_inertia;                        \
-    rg.frictions = r_frictions; rg.n_samples = n_samples; rg.offset = s_offset; rg.tri = s_tri; rg.sample_rigid = s_rigid;     \
-    rg.penalty = penalty; rg.pushing_force = pushing_force; rg.states = states; rg.bnormal = bnormal; rg.bdist = bdist;        \
-    rg.near = near;                                                                                                            \
+    Rigid<R> rg = make_rigid<R>(n_rigid, r_position, r_rot, r_velocity, r_angular_velocity, r_inv_mass, r_inv_inertia,         \
+                                r_frictions, n_samples, s_offset, s_tri, s_rigid, penalty, pushing_force, states, bnormal,     \
+                                bdist, near);                                                                                  \
     substep_coupled<R>(sc, rg, P, alive, grid_vel, grid_rast, node_state, node_dist);                                          \
+  }                                                                                                                            \
+  /* Only the coupled rasterize of the substep above (same arguments, no grid_vel): grid_rast, the particle colours and  */    \
+  /* boundary reconstruction, the bodies' velocities after the rasterize's impulses; v of the rigid pages' particles     */    \
+  /* returns with the gravity kick the rasterize stores back.                                                            */    \
+  ORACLE_API void oracle_p2g_coupled_##SUF(const int *res, R dx, R dt, const R *gravity, int particle_gravity, int n_groups,   \
+                                       const int32_t *mat_kind, const R *mat_params, const R *sdf, R friction, int64_t n,      \
+                                       R *x, R *v, R *F, R *b, const R *mass, const R *vol, R *ps, const int32_t *group,       \
+                                       uint8_t *alive, R *grid_rast, int n_rigid, const R *r_position,                         \
+                                       const R *r_rot, R *r_velocity, R *r_angular_velocity, const R *r_inv_mass,              \
+                                       const R *r_inv_inertia, const R *r_frictions, int64_t n_samples, const R *s_offset,     \
+                                       const R *s_tri, const int32_t *s_rigid, R penalty, R pushing_force, uint32_t *states,   \
+                                       R *bnormal, R *bdist, uint8_t *near, uint32_t *node_state, R *node_dist) {              \
+    (void)n_groups;                                                                                                            \
+    Scene<R> sc = make_scene<R>(res, dx, dt, gravity, particle_gravity, mat_kind, mat_params, sdf, friction);                  \
+    Particles<R> P{n, x, v, F, b, mass, vol, ps, group};                                                                       \
+    Rigid<R> rg = make_rigid<R>(n_rigid, r_position, r_rot, r_velocity, r_angular_velocity, r_inv_mass, r_inv_inertia,         \
+                                r_frictions, n_samples, s_offset, s_tri, s_rigid, penalty, pushing_force, states, bnormal,     \
+                                bdist, near);                                                                                  \
+    rasterize_coupled<R>(sc, rg, P, alive, grid_rast, node_state, node_dist);                                                  \
   }                                                                                                                            \
   ORACLE_API void oracle_mpm88_advance_##SUF(int n, R dt, R E, R nu, R hardening, R gravity_y, int plastic, int64_t np, R *x,  \
                                              R *v, R *F, R *C, R *Jp, R *grid) {                                               \

@@ -159,6 +159,20 @@ def substep_coupled(scene, state, rigid, dtype=np.float64):
     state additionally carries "states"[N] uint32 (MPMParticle::states; zeros if absent).
     Returns (new_state, grid_rast, grid_vel, rigid_out, cdf) with new_state["states"/"bnormal"/"bdist"/"near"],
     rigid_out = dict(velocity, angular_velocity) after both transfers, cdf = dict(node_state, node_dist)."""
+    return _coupled("oracle_substep_coupled_", scene, state, rigid, dtype, True)
+
+
+def p2g_coupled(scene, state, rigid, dtype=np.float64):
+    """Only the coupled rasterize of substep_coupled(): ordering, rigid pages, the colour field, gather_cdf and the coupled P2G
+    with its impulses (apply_tmp_velocity after rasterize, src/transfer.cpp:578-580).  Same arguments.
+    Returns (state, grid_rast, rigid_out, cdf): state carries "states"/"bnormal"/"bdist"/"near" and, for the particles of rigid
+    pages, v with the gravity kick the rasterize stores back; rigid_out = dict(velocity, angular_velocity) after the rasterize's
+    impulses only."""
+    st, grid_rast, _, rig, cdf = _coupled("oracle_p2g_coupled_", scene, state, rigid, dtype, False)
+    return st, grid_rast, rig, cdf
+
+
+def _coupled(entry, scene, state, rigid, dtype, with_grid_vel):
     res = np.asarray(scene["res"], np.int32)
     st = {k: np.ascontiguousarray(np.asarray(state[k], dtype)).copy() for k in ("x", "v", "F", "b", "mass", "vol", "ps")}
     st["group"] = np.ascontiguousarray(state["group"], np.int32)
@@ -172,20 +186,21 @@ def substep_coupled(scene, state, rigid, dtype=np.float64):
     sdf = None if sdf is None else np.ascontiguousarray(sdf, dtype)
     g = np.ascontiguousarray(scene["gravity"], dtype)
     nn = tuple(int(r) + 1 for r in res)
-    grid_rast, grid_vel = np.zeros(nn + (4,), dtype), np.zeros(nn + (4,), dtype)
+    grid_rast = np.zeros(nn + (4,), dtype)
+    grid_vel = np.zeros(nn + (4,), dtype) if with_grid_vel else None
     node_state, node_dist = np.zeros(nn, np.uint32), np.zeros(nn, dtype)
     r = {k: np.ascontiguousarray(np.asarray(rigid[k], dtype)).copy() for k in ("position", "rot", "velocity", "angular_velocity", "inv_mass",
                                                                              "inv_inertia", "frictions", "sample_offset", "sample_tri")}
     sr = np.ascontiguousarray(rigid["sample_rigid"], np.int32)
     sc = _scalar(dtype)
-    getattr(lib(), "oracle_substep_coupled_" + _suf(dtype))(
+    getattr(lib(), entry + _suf(dtype))(
         _p(res), sc(scene["dx"]), sc(scene["dt"]), _p(g), C.c_int(int(scene.get("particle_gravity", 1))), C.c_int(len(mk)),
         _p(mk), _p(mp), _p(sdf), sc(scene.get("friction", 0.0)), C.c_int64(n),
         _p(st["x"]), _p(st["v"]), _p(st["F"]), _p(st["b"]), _p(st["mass"]), _p(st["vol"]), _p(st["ps"]), _p(st["group"]),
-        _p(st["alive"]), _p(grid_rast), _p(grid_vel), C.c_int(len(r["inv_mass"])), _p(r["position"]), _p(r["rot"]), _p(r["velocity"]),
-        _p(r["angular_velocity"]), _p(r["inv_mass"]), _p(r["inv_inertia"]), _p(r["frictions"]), C.c_int64(len(sr)), _p(r["sample_offset"]),
-        _p(r["sample_tri"]), _p(sr), sc(rigid.get("penalty", 0.0)), sc(rigid.get("pushing_force", 20000.0)), _p(st["states"]),
-        _p(st["bnormal"]), _p(st["bdist"]), _p(st["near"]), _p(node_state), _p(node_dist))
+        _p(st["alive"]), _p(grid_rast), *([_p(grid_vel)] if with_grid_vel else []), C.c_int(len(r["inv_mass"])), _p(r["position"]), _p(r["rot"]),
+        _p(r["velocity"]), _p(r["angular_velocity"]), _p(r["inv_mass"]), _p(r["inv_inertia"]), _p(r["frictions"]), C.c_int64(len(sr)),
+        _p(r["sample_offset"]), _p(r["sample_tri"]), _p(sr), sc(rigid.get("penalty", 0.0)), sc(rigid.get("pushing_force", 20000.0)),
+        _p(st["states"]), _p(st["bnormal"]), _p(st["bdist"]), _p(st["near"]), _p(node_state), _p(node_dist))
     return st, grid_rast, grid_vel, dict(velocity=r["velocity"], angular_velocity=r["angular_velocity"]), dict(node_state=node_state, node_dist=node_dist)
 
 

@@ -433,9 +433,12 @@ class Engine:
     def get_rigid_state(self, n_bodies):
         arr = (MpmbRigidBody * n_bodies)()
         self._check(self.L.mpmb_get_rigid_state(self.h, C.c_int32(n_bodies), arr))
+        # rot and inv_inertia also column-major flattened, the layout of scenes.make_rigid (what the next substep reads)
         return dict(velocity=np.array([list(a.velocity) for a in arr], np.float32), angular_velocity=np.array([list(a.angular_velocity) for a in arr], np.float32),
                     position=np.array([list(a.position) for a in arr], np.float32),
-                    rotation=np.array([np.reshape(list(a.rot), (3, 3)).T for a in arr], np.float32))
+                    rotation=np.array([np.reshape(list(a.rot), (3, 3)).T for a in arr], np.float32),
+                    rot=np.array([list(a.rot) for a in arr], np.float32), inv_mass=np.array([a.inv_mass for a in arr], np.float32),
+                    inv_inertia=np.array([list(a.inv_inertia) for a in arr], np.float32), frictions=np.array([list(a.frictions) for a in arr], np.float32))
 
     def set_rigid_motion(self, motion, levelset_collision=False):
         """Device advection of the bodies (mpmb_set_rigid_motion).  motion: one dict per body, row 0 = the background body

@@ -20,12 +20,16 @@ from tests import common as T  # noqa: E402
 VARIANTS = ["kinematic", "dynamic", "two_bodies", "sand_preset"]
 
 
-def golden_scene(variant):
-    """A stirred block cut by a tilted plate (and, for two_bodies, a small free box inside it)."""
+def golden_scene(variant, kind=None, vel=0.3):
+    """A stirred block cut by a tilted plate (and, for two_bodies, a small free box inside it).  `kind`: the block of another
+    material instead, perturbed at its T.KIND_KW strain (T.perturbed_scene's default otherwise) — not a golden scene."""
     res = 32
     dx = 1.0 / res
-    kind = scenes.MAT_SAND if variant == "sand_preset" else scenes.MAT_JELLY
-    scene, st = T.perturbed_scene(kind, res=res, cells=6, seed=3, strain=0.005, vel=0.3)
+    if kind is None:
+        kind = scenes.MAT_SAND if variant == "sand_preset" else scenes.MAT_JELLY
+        scene, st = T.perturbed_scene(kind, res=res, cells=6, seed=3, strain=0.005, vel=vel)
+    else:
+        scene, st = T.perturbed_scene(kind, res=res, cells=6, seed=3, vel=vel, **T.KIND_KW.get(kind, {}))
     c = st["x"].mean(0)
     rot = scenes.euler_rotation((7.0, 13.0, -5.0))     # generic orientation: no grid node sits on a triangle edge
     plate = dict(tris=scenes.plate_mesh(0.21, 0.19, axis=1), position=c + np.array([0.004, 0.011, -0.003]), rotation=rot,

@@ -7,8 +7,8 @@ the oracle's rasterize of the same state with F = I and the fresh plastic scalar
 engine's error is measured against max |G_ref - G_free| instead of against the whole grid.  A probe with one particle
 per tile also solves the next P2G for A particle by particle, at the branch edges of every material, and follows 20
 substeps of those particles against 20 fp64 oracle substeps.  Runs on the SIMT emulator too
-(tests/test_next_p2g_simt.py).  Out of scope: the rigid-coupled path (k_g2p_rigid, whose P2G needs the colour state
-and the coupled oracle) and the AsyncMPM pools (they rebuild A from the rows on every advance)."""
+(tests/test_next_p2g_simt.py).  The rigid-coupled path (k_g2p_rigid) is checked the same way in
+tests/test_gpu_rigid_parity.py; out of scope: the AsyncMPM pools (they rebuild A from the rows on every advance)."""
 import numpy as np
 import pytest
 

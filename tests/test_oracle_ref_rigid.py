@@ -64,15 +64,59 @@ def test_oracle_cpic_matches_golden_run_of_reference(variant):
     _compare(scene, st, rigid, _golden(variant, scene))
 
 
+KINDS = [("linear", 0), ("jelly", 1), ("snow", 2), ("water", 3), ("sand", 4), ("elastic", 5), ("von_mises", 6), ("visco", 7)]
+
+
 @pytest.mark.skipif(not O.ref_transfer_available(), reason="reference build (oracle/_ref) not available")
-@pytest.mark.parametrize("variant", ["dynamic", "sand_preset"])
+@pytest.mark.parametrize("variant", ["dynamic", "sand_preset"] + ["dynamic_" + name for name, _ in KINDS])
 def test_oracle_cpic_matches_reference_live(variant):
-    scene, st, rigid = G.golden_scene(variant)
+    # the golden scenes, and the dynamic one with the block of each of the eight kinds (the reference harness registers all
+    # of them: oracle/transfer_ref.cpp, reft_add_particle), at the kind's T.KIND_KW strain
+    kind = dict(KINDS).get(variant[len("dynamic_"):]) if variant.startswith("dynamic_") else None
+    scene, st, rigid = G.golden_scene("dynamic" if kind is not None else variant, kind=kind)
     st["x"] = st["x"] + np.float32(0.0037)                     # not the golden positions
     new, grid_rast, grid_vel, rs, cdf = O.ref_substep_coupled(scene, st, rigid)
     ref = dict(new, grid_rast=grid_rast, grid_vel=grid_vel, node_state=cdf["node_state"], node_dist=cdf["node_dist"], rigid_v=rs["velocity"],
                rigid_w=rs["angular_velocity"])
     _compare(scene, st, rigid, ref)
+
+
+@pytest.mark.skipif(not O.ref_transfer_available(), reason="reference build (oracle/_ref) not available")
+@pytest.mark.parametrize("variant", ["dynamic", "two_bodies", "sand_preset", "dynamic_snow", "dynamic_von_mises"])
+def test_oracle_p2g_coupled_matches_reference_live(variant):
+    # pyoracle.p2g_coupled, the coupled rasterize alone, against the reference's ordering + rigid pages + CDF + gather_cdf
+    # (coupled_stage 0) and rasterize_optimized (coupled_stage 1): the grid, the colours and boundary reconstruction, and the
+    # bodies' velocities after the rasterize's impulses only
+    kind = dict(KINDS).get(variant[len("dynamic_"):]) if variant.startswith("dynamic_") else None
+    scene, st, rigid = G.golden_scene("dynamic" if kind is not None else variant, kind=kind)
+    st["x"] = st["x"] + np.float32(0.0021)
+    new, grid, rs, cdf = O.p2g_coupled(scene, st, rigid, np.float64)
+    s = O.RefSolver(scene, st)
+    try:
+        s.set_rigid(rigid)
+        if st.get("states") is not None:
+            s.set_states(st["states"])
+        s.coupled_stage(0)
+        rcdf, pc = s.cdf_grid(), s.cdf_particles()
+        s.coupled_stage(1)
+        rgrid, rrs = s.get_grid(), s.rigid_state()
+    finally:
+        s.close()
+    assert np.array_equal(cdf["node_state"], rcdf["node_state"]) and (cdf["node_state"] >> 24 != 0).sum() > 200
+    assert np.array_equal(new["states"], pc["states"]) and np.array_equal(new["near"], pc["near"]) and 0 < pc["near"].sum()
+    assert np.abs(new["bdist"] - pc["bdist"]).max() <= 1e-6 and np.abs(new["bnormal"] - pc["bnormal"]).max() <= 1e-4
+    pmax = max(np.abs(grid[..., :3]).max(), grid[..., 3].max())
+    assert np.abs(grid - rgrid).max() <= 3e-6 * pmax
+    free = rigid["inv_mass"] > 0
+    for b in range(1, len(rigid["inv_mass"])):
+        dv, dw = rs["velocity"][b] - rigid["velocity"][b], rs["angular_velocity"][b] - rigid["angular_velocity"][b]
+        print(variant, "body", b, "dv", dv, "dw", dw)
+        assert np.abs(dv - (rrs["velocity"][b] - rigid["velocity"][b])).max() <= 1e-4 * np.abs(dv).max() + 1e-7
+        assert np.abs(dw - (rrs["angular_velocity"][b] - rigid["angular_velocity"][b])).max() <= 1e-4 * np.abs(dw).max() + 1e-6
+        assert (np.abs(dv).max() > 1e-4) == bool(free[b])
+    # the rasterize alone is the first half of substep_coupled: the same grid, colours and reconstruction
+    full, grid_rast, _, _, _ = O.substep_coupled(scene, st, rigid, np.float64)
+    assert np.array_equal(grid, grid_rast) and np.array_equal(new["states"], full["states"]) and np.array_equal(new["bdist"], full["bdist"])
 
 
 @pytest.mark.skipif(not O.ref_transfer_available(), reason="reference build (oracle/_ref) not available")
