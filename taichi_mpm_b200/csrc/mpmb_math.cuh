@@ -189,6 +189,61 @@ struct Material {
 #define MPMB_EIG_SWEEPS 3
 #endif
 
+__device__ __forceinline__ float det3(const Mat3 &A) {
+  return A.m[0] * (A.m[4] * A.m[8] - A.m[7] * A.m[5]) - A.m[3] * (A.m[1] * A.m[8] - A.m[7] * A.m[2]) + A.m[6] * (A.m[1] * A.m[5] - A.m[4] * A.m[2]);
+}
+
+// Inverted elements (det F < 0).  The eigen-system of F F^T - I gives |sigma| only; the convention of the
+// reference's polar_decomp()/svd() with rotations U, V in SO(3) (DESIGN.md §2) puts the sign of det F on the
+// smallest singular value: F = U diag(s^) V^T with s^_k = -s_k on that axis.  Returns k, or -1 for det F >= 0.
+__device__ __forceinline__ int argmin3(const float e[3]) { return e[0] <= e[1] ? (e[0] <= e[2] ? 0 : 2) : (e[1] <= e[2] ? 1 : 2); }
+__device__ __forceinline__ int reflected_axis(const Mat3 &F, const float e[3]) { return det3(F) < 0.f ? argmin3(e) : -1; }
+
+// Fixed-corotated Kirchhoff stress in principal space from en_i = s_i^2 - 1 (s_i >= 0) and the reflected axis
+// `flip` (-1: none):  tau_i = 2 mu s^_i (s^_i - 1) + lambda (J-1) J,  J = prod s^ (signed).
+// Kept axes use s - 1 = e/(s+1) and J - 1 = (J^2-1)/(J+1) (no cancellation near I); on the reflected axis
+// s^(s^-1) = s(s+1) and J <= 0, where those forms would divide by zero at s^ = -1, J = -1.
+__device__ __forceinline__ void fixed_corotated_tau(float mu, float la, const float en[3], int flip, float tau[3]) {
+  const float s[3] = {sqrtf(fmaxf(1.f + en[0], 0.f)), sqrtf(fmaxf(1.f + en[1], 0.f)), sqrtf(fmaxf(1.f + en[2], 0.f))};
+  float J = s[0] * s[1] * s[2];
+  float Jm1;
+  if (flip >= 0) {
+    J = -J;
+    Jm1 = J - 1.f;
+  } else {
+    const float J2m1 = (en[0] + en[1] + en[2]) + fmaf(en[0], en[1], fmaf(en[0], en[2], en[1] * en[2])) + en[0] * en[1] * en[2];
+    Jm1 = J2m1 / (J + 1.f);
+  }
+  const float vol_term = la * Jm1 * J;
+#pragma unroll
+  for (int i = 0; i < 3; i++) tau[i] = fmaf(2.f * mu * s[i], i == flip ? s[i] + 1.f : en[i] / (s[i] + 1.f), vol_term);
+}
+
+// F' = U diag(r) U^T Ft with the part along axis k rebuilt as sig_k u_k v_k^T.  With m = U^T Ft (rows s^_i v_i^T)
+// and U, V in SO(3), v_k = v_i x v_j = unit(m_i x m_j) for (i,j,k) cyclic, whatever s^_k is: the return maps
+// take this for the smallest axis where the ratio sig_k / s_k would divide by a vanishing (or 1e-4-clamped)
+// singular value that F F^T - I resolves only to ~1e-7 / s_k.  Needs s_i, s_j > 0 (rank >= 2).
+// Arguments by value (see ViscoOut below): out of line, on a path physical states never take.
+MPMB_NOINLINE_DEVICE Mat3 rebuild_small_axis(Mat3 U, float r0, float r1, float r2, int k, float sig_k, Mat3 Ft) {
+  const float r[3] = {k == 0 ? 0.f : r0, k == 1 ? 0.f : r1, k == 2 ? 0.f : r2};
+  Mat3 F = sym_mul(sym_from_eig(U, r), Ft);
+  const int i = k == 2 ? 0 : k + 1, j = k == 0 ? 2 : k - 1;
+  float mi[3], mj[3];
+#pragma unroll
+  for (int c = 0; c < 3; c++) {  // m_i[c] = sum_r U(r,i) Ft(r,c)
+    mi[c] = fmaf(U.m[i * 3], Ft.m[c * 3], fmaf(U.m[i * 3 + 1], Ft.m[c * 3 + 1], U.m[i * 3 + 2] * Ft.m[c * 3 + 2]));
+    mj[c] = fmaf(U.m[j * 3], Ft.m[c * 3], fmaf(U.m[j * 3 + 1], Ft.m[c * 3 + 1], U.m[j * 3 + 2] * Ft.m[c * 3 + 2]));
+  }
+  const float v[3] = {mi[1] * mj[2] - mi[2] * mj[1], mi[2] * mj[0] - mi[0] * mj[2], mi[0] * mj[1] - mi[1] * mj[0]};
+  const float n2 = fmaf(v[0], v[0], fmaf(v[1], v[1], v[2] * v[2]));
+  const float sc = n2 > 0.f ? sig_k / sqrtf(n2) : 0.f;
+#pragma unroll
+  for (int c = 0; c < 3; c++)
+#pragma unroll
+    for (int rr = 0; rr < 3; rr++) F.m[c * 3 + rr] = fmaf(sc * U.m[k * 3 + rr], v[c], F.m[c * 3 + rr]);
+  return F;
+}
+
 // -vol * P(F) F^T  ==  the value of Particle::calculate_force() (src/particles.cpp:216-218,
 // 335-337,409-411,463-467,628-637), returned as a symmetric tensor where it is one (all kinds
 // except LINEAR, whose P F^T is not symmetric for finite strain).
@@ -240,21 +295,14 @@ __device__ __forceinline__ void calculate_force(const Material &mat, const Mat3 
     tau[2] = fmaf(2.f * mu, l2, tr);
   } else {
     // fixed corotated (jelly 391-398, snow 207-214, visco 69-82): P F^T = 2mu (F-R)F^T + lambda (J-1) J I
-    //   (F-R)F^T = U diag(s(s-1)) U^T ;  s-1 = e/(s+1) ;  J^2-1 = sum e + sum e e + e e e
+    //   (F-R)F^T = U diag(s^(s^-1)) U^T with R in SO(3) and J = det F signed (fixed_corotated_tau)
     float mu = mat.p[0], la = mat.p[1];
     if (mat.kind == MAT_SNOW) {
       float h = __expf(mat.p[2] * (1.0f - ps));  // 244-252
       mu *= h;
       la *= h;
     }
-    float s0 = sqrtf(1.f + e[0]), s1 = sqrtf(1.f + e[1]), s2 = sqrtf(1.f + e[2]);
-    float J = s0 * s1 * s2;
-    float J2m1 = (e[0] + e[1] + e[2]) + fmaf(e[0], e[1], fmaf(e[0], e[2], e[1] * e[2])) + e[0] * e[1] * e[2];
-    float Jm1 = J2m1 / (J + 1.f);
-    float vol_term = la * Jm1 * J;
-    tau[0] = fmaf(2.f * mu * s0, e[0] / (s0 + 1.f), vol_term);
-    tau[1] = fmaf(2.f * mu * s1, e[1] / (s1 + 1.f), vol_term);
-    tau[2] = fmaf(2.f * mu * s2, e[2] / (s2 + 1.f), vol_term);
+    fixed_corotated_tau(mu, la, e, reflected_axis(F, e), tau);
   }
   tau[0] *= -vol; tau[1] *= -vol; tau[2] *= -vol;
   Sym3 T = sym_from_eig(U, tau);
@@ -284,21 +332,6 @@ __device__ __forceinline__ bool von_mises_return(const Material &mat, const floa
   return yield;
 }
 
-// Fixed-corotated Kirchhoff stress in principal space from en_i = s_i^2 - 1: tau_i = 2 mu s_i (s_i - 1) + lambda (J-1) J
-__device__ __forceinline__ void fixed_corotated_tau(float mu, float la, const float en[3], float tau[3]) {
-  const float s0 = sqrtf(1.f + en[0]), s1 = sqrtf(1.f + en[1]), s2 = sqrtf(1.f + en[2]);
-  const float J = s0 * s1 * s2;
-  const float J2m1 = (en[0] + en[1] + en[2]) + fmaf(en[0], en[1], fmaf(en[0], en[2], en[1] * en[2])) + en[0] * en[1] * en[2];
-  const float vol_term = la * (J2m1 / (J + 1.f)) * J;
-  tau[0] = fmaf(2.f * mu * s0, en[0] / (s0 + 1.f), vol_term);
-  tau[1] = fmaf(2.f * mu * s1, en[1] / (s1 + 1.f), vol_term);
-  tau[2] = fmaf(2.f * mu * s2, en[2] / (s2 + 1.f), vol_term);
-}
-
-__device__ __forceinline__ float det3(const Mat3 &A) {
-  return A.m[0] * (A.m[4] * A.m[8] - A.m[7] * A.m[5]) - A.m[3] * (A.m[1] * A.m[8] - A.m[7] * A.m[2]) + A.m[6] * (A.m[1] * A.m[5] - A.m[4] * A.m[2]);
-}
-
 // ViscoParticle::plasticity (src/particles.cpp:104-137) + the fixed-corotated stress of the new state (69-82).
 // ps = visco_tau.  Kept out of line: a rarely used material must not shape the register allocation of k_g2p.
 //   F^ = approximate_exponent(dt_p, (cdg - I)/dt_p) F   (89-102: (s/2 + I) s + I, halving while det <= 0)
@@ -319,7 +352,9 @@ MPMB_NOINLINE_DEVICE ViscoOut visco_step_impl(float mu, float la, float nu, floa
     Mat3 U0;
     float e0[3];
     eig_sym3<MPMB_EIG_SWEEPS>(left_strain(F), U0, e0);
-    const float s0 = sqrtf(1.f + e0[0]), s1 = sqrtf(1.f + e0[1]), s2 = sqrtf(1.f + e0[2]);
+    const int fk = reflected_axis(F, e0);  // P of an inverted F with R in SO(3): signed s^, J
+    const float s0 = (fk == 0 ? -1.f : 1.f) * sqrtf(fmaxf(1.f + e0[0], 0.f)), s1 = (fk == 1 ? -1.f : 1.f) * sqrtf(fmaxf(1.f + e0[1], 0.f)),
+                s2 = (fk == 2 ? -1.f : 1.f) * sqrtf(fmaxf(1.f + e0[2], 0.f));
     const float J = s0 * s1 * s2;
     const float vt = la * (J - 1.f) * J;
     const float p0 = fmaf(2.f * mu, s0 - 1.f, vt / s0), p1 = fmaf(2.f * mu, s1 - 1.f, vt / s1), p2 = fmaf(2.f * mu, s2 - 1.f, vt / s2);
@@ -352,19 +387,23 @@ MPMB_NOINLINE_DEVICE ViscoOut visco_step_impl(float mu, float la, float nu, floa
   float sg[3] = {sqrtf(fmaxf(1.f + e[0], 0.f)), sqrtf(fmaxf(1.f + e[1], 0.f)), sqrtf(fmaxf(1.f + e[2], 0.f))};
   const float det = sg[0] * sg[1] * sg[2];
   const float scale = fabsf(det) > 1e-5f ? 1.0f / cbrtf(det) : 1.0f;
-  float ratio[3], en[3];
+  float ratio[3], en[3], sn[3];
 #pragma unroll
   for (int i = 0; i < 3; i++) {
     const float mid = powf(sg[i] * scale, gamma);
     const float mid_inv = fabsf(mid) > 1e-5f ? 1.0f / mid : 1.0f;
-    const float sn = fminf(fmaxf(sg[i] * mid_inv, 0.1f), 10.0f);
-    ratio[i] = sn / sg[i];
-    en[i] = fmaf(sn, sn, -1.f);
+    sn[i] = fminf(fmaxf(sg[i] * mid_inv, 0.1f), 10.0f);
+    ratio[i] = sn[i] / sg[i];
+    en[i] = fmaf(sn[i], sn[i], -1.f);
   }
   ps = fmaf(kappa * gamma, pnorm, ps);
-  F = sym_mul(sym_from_eig(U, ratio), Fh);
+  // the return map reads |sigma| (the reference's pow(det, 1/3) and log of a negative sigma are NaN, DESIGN.md §2):
+  // an inverted F^ stays inverted, on the same (smallest) axis
+  const int k = argmin3(e), flip = det3(Fh) < 0.f ? k : -1;
+  if (1.f + e[k] < 1e-2f) F = rebuild_small_axis(U, ratio[0], ratio[1], ratio[2], k, flip >= 0 ? -sn[k] : sn[k], Fh);
+  else F = sym_mul(sym_from_eig(U, ratio), Fh);
   float tau[3];
-  fixed_corotated_tau(mu, la, en, tau);
+  fixed_corotated_tau(mu, la, en, flip, tau);
   tau[0] *= -vol; tau[1] *= -vol; tau[2] *= -vol;
   const Sym3 T = sym_from_eig(U, tau);
   force.m[0] = T.xx; force.m[1] = T.xy; force.m[2] = T.xz;
@@ -404,22 +443,25 @@ __device__ __forceinline__ void plasticity(const Material &mat, const Mat3 &cdg,
   Mat3 U;
   float e[3];
   eig_sym3<MPMB_EIG_SWEEPS>(left_strain(Ft), U, e);
-  float ratio[3];
+  float ratio[3], sig_k = 0.f;
   bool changed;
+  const int k = argmin3(e), flip = det3(Ft) < 0.f ? k : -1;
   if (mat.kind == MAT_VON_MISES) {
     changed = von_mises_return(mat, e, ratio, nullptr);
+    sig_k = (flip >= 0 ? -1.f : 1.f) * sqrtf(fmaxf(1.f + e[k], 0.f)) * ratio[k];
   } else if (mat.kind == MAT_SNOW) {
-    // sigma clamped to [1-theta_c, 1+theta_s]; Jp <- clamp(Jp * prod(s)/prod(s'))   (222-242)
+    // signed sigma^ clamped to [1-theta_c, 1+theta_s]; Jp <- clamp(Jp * prod(s^)/prod(s'))   (222-242)
     float lo = 1.f - mat.p[3], hi = 1.f + mat.p[4];
     float prod = 1.f;
     changed = false;
 #pragma unroll
     for (int i = 0; i < 3; i++) {
-      float s = sqrtf(fmaxf(1.f + e[i], 0.f));
+      float s = (i == flip ? -1.f : 1.f) * sqrtf(fmaxf(1.f + e[i], 0.f));
       float sc = fminf(fmaxf(s, lo), hi);
       ratio[i] = sc / s;
       prod *= s / sc;
       changed |= (sc != s);
+      if (i == k) sig_k = sc;
     }
     float Jp = ps * prod;
     if (!(Jp <= mat.p[6])) Jp = mat.p[6];
@@ -432,9 +474,8 @@ __device__ __forceinline__ void plasticity(const Material &mat, const Mat3 &cdg,
     float sum = 0.f;
 #pragma unroll
     for (int i = 0; i < 3; i++) {
-      // ln max(|s|,1e-4) with s = sqrt(1+e) >= 0
-      float ec = fmaxf(e[i], 1e-8f - 1.f);
-      ls[i] = 0.5f * log1pf(ec);
+      // ln max(|s|,1e-4) with s = sqrt(1+e) >= 0 (clamped after the log: 1e-8f - 1.f rounds to -1.f)
+      ls[i] = fmaxf(0.5f * log1pf(e[i]), -9.21034037f);
       eps[i] = ls[i] - coh;
       sum += eps[i];
     }
@@ -447,29 +488,34 @@ __device__ __forceinline__ void plasticity(const Material &mat, const Mat3 &cdg,
       for (int i = 0; i < 3; i++) ratio[i] = __expf(coh - ls[i]);
       ps = fmaf(beta, sum, ps);
       changed = true;
+      sig_k = __expf(coh);
     } else {
       ps = 0.f;
       float dg = hn + (3.f * la + 2.f * mu) / (2.f * mu) * tr * alpha;
       if (dg <= 0.f) {
 #pragma unroll
         for (int i = 0; i < 3; i++) ratio[i] = 1.f;
-        changed = false;
-        // NB the reference still rebuilds F = U exp(eps+c) V^T here, which equals cdg F up to
-        // rounding unless a singular value was clamped at 1e-4 (never for physical states).
-        if (e[0] < 1e-8f - 1.f || e[1] < 1e-8f - 1.f || e[2] < 1e-8f - 1.f) {
-#pragma unroll
-          for (int i = 0; i < 3; i++) ratio[i] = __expf(ls[i]) * rsqrtf(fmaxf(1.f + e[i], 1e-30f));
-          changed = true;
-        }
+        // NB the reference still rebuilds F = U exp(eps+c) V^T here, which equals cdg F up to rounding
+        // unless a singular value was clamped at 1e-4 (the smallest axis, rebuilt below) or F is inverted
+        changed = ls[k] <= -9.21034037f;
+        sig_k = __expf(ls[k]);
       } else {
-        float k = dg / hn;
+        float kp = dg / hn;
 #pragma unroll
-        for (int i = 0; i < 3; i++) ratio[i] = expf(-k * hat[i]);
+        for (int i = 0; i < 3; i++) ratio[i] = expf(-kp * hat[i]);
         changed = true;
+        sig_k = __expf(ls[k] - kp * hat[k]);
       }
     }
+    // project() reads |sigma| and returns sigma' > 0: an inverted F comes out un-inverted
+    if (flip >= 0) {
+      ratio[k] = -ratio[k];
+      changed = true;
+    }
   }
-  if (changed) {
+  if (changed && 1.f + e[k] < 1e-2f) {
+    F = rebuild_small_axis(U, ratio[0], ratio[1], ratio[2], k, sig_k, Ft);
+  } else if (changed) {
     Sym3 M = sym_from_eig(U, ratio);
     F = sym_mul(M, Ft);
   } else {
@@ -586,7 +632,9 @@ __device__ __forceinline__ Sym3 sym_exp_series(const Sym3 &X, float nrm2) {
 __device__ __forceinline__ bool sand_step_series(const Material &mat, const Mat3 &Ft, Mat3 &F, float &ps, float vol, Mat3 &force) {
   const Sym3 E = left_strain(Ft);
   const float nE2 = sym_norm2(E);
-  const bool small = nE2 <= 0.0225f;
+  // log(I + E) is the log strain only for det Ft > 0: a reflection (E = 0 for F = diag(1,1,-1)) must take the
+  // eigen path, which un-inverts it as project() does
+  const bool small = nE2 <= 0.0225f && det3(Ft) > 0.f;
   const float mu = mat.p[0], la = mat.p[1], alpha = mat.p[2], coh = mat.p[3], beta = mat.p[4];
   Sym3 L = sym_log1p_series(E, small ? nE2 : 0.f);
   L.xx *= 0.5f; L.yy *= 0.5f; L.zz *= 0.5f; L.xy *= 0.5f; L.xz *= 0.5f; L.yz *= 0.5f;
@@ -670,12 +718,18 @@ __device__ __forceinline__ void material_step(const Material &mat, const Mat3 &c
   eig_sym3<MPMB_EIG_SWEEPS>(left_strain(Ft), U, e);
   float ratio[3], tau[3];
   bool changed = false;
+  // the smallest axis carries the sign of det Ft (-1: not inverted) and, for the return maps, is rebuilt from the
+  // other two where its singular value is too small to divide by (rebuild_small_axis); sig_k is its new s^
+  const int k = argmin3(e), flip = reflected_axis(Ft, e);
+  float sig_k = 0.f;
   if (EXT && (mat.kind == MAT_ELASTIC || mat.kind == MAT_VON_MISES)) {
-    // Hencky elasticity (src/particles.cpp:800-814) with the von Mises return map (714-734) where asked for
+    // Hencky elasticity (src/particles.cpp:800-814) with the von Mises return map (714-734) where asked for.
+    // Both read |sigma| (the reference's log of a negative sigma is NaN): an inverted element stays inverted.
     const float mu = mat.p[0], la = mat.p[1];
     float lsn[3];
     if (mat.kind == MAT_VON_MISES) {
       changed = von_mises_return(mat, e, ratio, lsn);
+      sig_k = (flip >= 0 ? -1.f : 1.f) * sqrtf(fmaxf(1.f + e[k], 0.f)) * ratio[k];
     } else {
 #pragma unroll
       for (int i = 0; i < 3; i++) lsn[i] = 0.5f * log1p_strain(e[i]);
@@ -689,8 +743,8 @@ __device__ __forceinline__ void material_step(const Material &mat, const Mat3 &c
     float sum = 0.f;
 #pragma unroll
     for (int i = 0; i < 3; i++) {
-      const float ec = fmaxf(e[i], 1e-8f - 1.f);  // ln max(|s|,1e-4), s = sqrt(1+e)
-      ls[i] = 0.5f * log1p_strain(ec);
+      // ln max(|s|,1e-4), s = sqrt(1+e); clamped after the log (1e-8f - 1.f rounds to -1.f, log1p(-1) = -inf; fmaxf drops a NaN)
+      ls[i] = fmaxf(0.5f * log1p_strain(e[i]), -9.21034037f);
       eps[i] = ls[i] - coh;
       sum += eps[i];
     }
@@ -709,39 +763,48 @@ __device__ __forceinline__ void material_step(const Material &mat, const Mat3 &c
       if (dg <= 0.f) {
 #pragma unroll
         for (int i = 0; i < 3; i++) { ratio[i] = 1.f; lsn[i] = ls[i]; }
-        if (e[0] < 1e-8f - 1.f || e[1] < 1e-8f - 1.f || e[2] < 1e-8f - 1.f) {  // a singular value was clamped at 1e-4
-#pragma unroll
-          for (int i = 0; i < 3; i++) ratio[i] = __expf(ls[i]) * rsqrtf(fmaxf(1.f + e[i], 1e-30f));
-          changed = true;
-        }
+        // the reference rebuilds F = U exp(eps+c) V^T, which equals Ft up to rounding unless the smallest singular
+        // value was clamped at 1e-4 (rebuilt below) or Ft is inverted
+        changed = ls[k] <= -9.21034037f;
       } else {
-        const float k = dg / hn;
+        const float kp = dg / hn;
 #pragma unroll
-        for (int i = 0; i < 3; i++) { ratio[i] = __expf(-k * hat[i]); lsn[i] = fmaf(-k, hat[i], ls[i]); }
+        for (int i = 0; i < 3; i++) { ratio[i] = __expf(-kp * hat[i]); lsn[i] = fmaf(-kp, hat[i], ls[i]); }
         changed = true;
       }
     }
+    // project() reads |sigma| and returns sigma' > 0: an inverted element comes out un-inverted
+    if (flip >= 0) {
+      ratio[k] = -ratio[k];
+      changed = true;
+    }
+    sig_k = __expf(lsn[k]);
     const float trl = la * (lsn[0] + lsn[1] + lsn[2]);
 #pragma unroll
     for (int i = 0; i < 3; i++) tau[i] = -vol * fmaf(2.f * mu, lsn[i], trl);
   } else {
-    // fixed corotated family.  JELLY: no return map; SNOW: clamp + hardening with the NEW Jp.
+    // fixed corotated family.  JELLY: no return map; SNOW: clamp of the signed s^ + hardening with the NEW Jp.
     float mu = mat.p[0], la = mat.p[1];
     float en[3] = {e[0], e[1], e[2]};  // s'^2 - 1 of the new state
+    int flip_new = flip;
     if (mat.kind == MAT_SNOW) {
       const float lo = 1.f - mat.p[3], hi = 1.f + mat.p[4];
       float prod = 1.f;
 #pragma unroll
       for (int i = 0; i < 3; i++) {
-        const float s = sqrtf(fmaxf(1.f + e[i], 0.f));
+        const float s = (i == flip ? -1.f : 1.f) * sqrtf(fmaxf(1.f + e[i], 0.f));
         const float sc = fminf(fmaxf(s, lo), hi);
         if (sc != s) {
           changed = true;
           ratio[i] = sc / s;
-          prod *= s / sc;
+          prod *= s / sc;  // < 0 on a reflected axis: Jp lands on min_Jp, as src/particles.cpp:225-238 does
           en[i] = fmaf(sc, sc, -1.f);
         } else {
           ratio[i] = 1.f;
+        }
+        if (i == k) {
+          sig_k = sc;
+          if (sc > 0.f) flip_new = -1;
         }
       }
       float Jp = ps * prod;
@@ -752,15 +815,11 @@ __device__ __forceinline__ void material_step(const Material &mat, const Mat3 &c
       mu *= hgain;
       la *= hgain;
     }
-    const float s0 = sqrtf(1.f + en[0]), s1 = sqrtf(1.f + en[1]), s2 = sqrtf(1.f + en[2]);
-    const float J = s0 * s1 * s2;
-    const float J2m1 = (en[0] + en[1] + en[2]) + fmaf(en[0], en[1], fmaf(en[0], en[2], en[1] * en[2])) + en[0] * en[1] * en[2];
-    const float vol_term = la * (J2m1 / (J + 1.f)) * J;
-    tau[0] = -vol * fmaf(2.f * mu * s0, en[0] / (s0 + 1.f), vol_term);
-    tau[1] = -vol * fmaf(2.f * mu * s1, en[1] / (s1 + 1.f), vol_term);
-    tau[2] = -vol * fmaf(2.f * mu * s2, en[2] / (s2 + 1.f), vol_term);
+    fixed_corotated_tau(mu, la, en, flip_new, tau);
+    tau[0] *= -vol; tau[1] *= -vol; tau[2] *= -vol;
   }
-  if (changed) F = sym_mul(sym_from_eig(U, ratio), Ft);
+  if (changed && 1.f + e[k] < 1e-2f) F = rebuild_small_axis(U, ratio[0], ratio[1], ratio[2], k, sig_k, Ft);
+  else if (changed) F = sym_mul(sym_from_eig(U, ratio), Ft);
   else F = Ft;
   store_sym(sym_from_eig(U, tau), force);
 }

@@ -246,3 +246,109 @@ def test_device_friction_project_cases(hm):
         hm.hm_friction_project0(C.c_int64(n), _p(v), _p(nn), C.c_float(fr), _p(out))
         ref = np.array([O.friction_project(v[i], np.zeros(3), nn[i], fr, np.float64) for i in range(n)])
         assert np.abs(out - ref).max() <= 2e-6, fr
+
+
+# ---- the edges of the constitutive models (tests/material_states.py): rotated, large, degenerate, near-singular and
+# inverted deformation gradients, against the fp64 oracle (or, where the reference is undefined, against
+# material_states.expected_step's statement of the device's convention, DESIGN.md §2)
+from tests import common as T  # noqa: E402
+from tests import material_states as MS  # noqa: E402
+
+
+def edge_cases():
+    """(kind, regime, strain) of every batch the three consumers of material_states run"""
+    out = []
+    for kind in MS.KINDS:
+        for strain in MS.ROTATED_STRAIN[kind]:
+            out.append((kind, "rotated", strain))
+        for regime in MS.REGIMES[1:]:
+            out.append((kind, regime, None))
+    return out
+
+
+def edge_batch(kind, regime, strain, n=128, seed=0):
+    """states of one batch with their fp64 expectation.  Near-singular states keep s_min only where the reference's
+    own result is finite: the Hencky stress (elastic, von Mises) and visco's |P(F_old)| hold ln s_min and 1/s_min."""
+    F, cdg, ps, vol = MS.states(kind, regime, n, seed, strain)
+    if regime == "near_singular":
+        floor = 1e-3 if kind in (scenes.MAT_ELASTIC, scenes.MAT_VON_MISES, scenes.MAT_VISCO) else (1e-4 if kind == scenes.MAT_JELLY else 0.0)
+        keep = MS.min_abs_sigma(F) >= floor * 0.5
+        F, cdg, ps, vol = F[keep], cdg[keep], ps[keep], vol[keep]
+    prm = _params8(kind)
+    Fo, pso, fo = MS.expected_batch(kind, prm, cdg, F, ps, vol)
+    return F, cdg, ps, vol, prm, Fo, pso, fo
+
+
+def edge_errors(kind, regime, F, cdg, Fd, psd, fd, Fo, pso, fo):
+    """worst errors of one batch: F (relative to max(1, |F'|)), ps (T.ps_err) and force (relative to the batch's
+    stress scale).  Near-singular states compare what is unique there: det F', tr(force), ps."""
+    assert np.isfinite(Fd).all() and np.isfinite(psd).all() and np.isfinite(fd).all(), (kind, regime)
+    assert np.isfinite(Fo).all() and np.isfinite(fo).all(), (kind, regime)
+    Fd, fd = Fd.astype(np.float64), fd.astype(np.float64)
+    scale = max(np.abs(fo).max(), 1e-30)
+    err = {"ps": T.ps_err(psd, pso)}
+    if regime == "near_singular":
+        # e = s^2 - 1 from F F^T - I holds s_min^2 to ~1e-7 absolute, i.e. s_min to ~3e-4: det F' and tr(force) are
+        # compared from s_min = 1e-2 on; below it every output must be finite and ps must match, while det F' and the
+        # stress (ln s_min, 1/s_min) are not resolved -- except for snow, whose clamp rebuilds that axis from the
+        # other two (rebuild_small_axis), and the kinds that need no eigen-system (DESIGN.md §2)
+        m = (MS.min_abs_sigma(F) >= 5e-3) | (kind in (scenes.MAT_SNOW, scenes.MAT_LINEAR, scenes.MAT_WATER))
+        F, Fd, fd, Fo, fo = F[m], Fd[m], fd[m], Fo[m], fo[m]
+        dd, do = np.linalg.det(Fd), np.linalg.det(Fo)
+        # at s_min = 0 the sign of det F' is the free sign of the reference's null vector
+        dd, do = np.where(MS.min_abs_sigma(F) == 0, np.abs(dd), dd), np.where(MS.min_abs_sigma(F) == 0, np.abs(do), do)
+        err["detF"] = float((np.abs(dd - do) / np.maximum(np.abs(do), 1e-4)).max())
+        err["trforce"] = float(np.abs(np.trace(fd, axis1=1, axis2=2) - np.trace(fo, axis1=1, axis2=2)).max() / scale)
+    else:
+        err["F"] = float((np.abs(Fd - Fo).reshape(len(F), -1).max(1) / np.maximum(1.0, np.abs(Fo).reshape(len(F), -1).max(1))).max())
+        err["force"] = float(np.abs(fd - fo).max() / scale)
+    if kind == scenes.MAT_WATER:
+        err.pop("F", None), err.pop("detF", None)                 # water carries no F (src/particles.cpp:469-478)
+    return err
+
+
+# worst errors allowed per regime.  F and ps: TOL_F_ABS and TOL_PS_ABS as everywhere; stress: 2e-4 of the batch's
+# scale (the floor of the moderate-strain cases above), except where fp32 itself cannot do better -- large stretches
+# (sigma up to 5: the eigen-system of F F^T - I resolves e to 1e-7 |F|^2) and near-singular states (e = s^2 - 1 of
+# s_min <= 1e-2 is ~ -1 + 1e-4; s_min itself comes from the other two axes, rebuild_small_axis)
+EDGE_TOL = {
+    "rotated": {"F": T.TOL_F_ABS, "ps": T.TOL_PS_ABS, "force": 2e-4},
+    "large": {"F": T.TOL_F_ABS, "ps": T.TOL_PS_ABS, "force": 2e-4},
+    "degenerate": {"F": T.TOL_F_ABS, "ps": T.TOL_PS_ABS, "force": 2e-4},
+    "near_singular": {"detF": 1e-3, "ps": T.TOL_PS_ABS, "trforce": 1e-3},
+    "inverted": {"F": T.TOL_F_ABS, "ps": T.TOL_PS_ABS, "force": 2e-4},
+}
+
+
+def rotated_force_tol(kind, prm, cdg, F, ps, vol, fo):
+    """force tolerance of a rotated batch, relative to its stress scale.  fp32 holds F = R S to ~6e-8 per entry, so
+    a strain under a half turn is known to ~1e-7 in sigma whatever the arithmetic after it: 2e-4 of the scale plus
+    1e-7 x 5 (a few roundings) of the stiffness.  Where the reference runs, the device must also stay within 2x of
+    the error of the reference's own fp32 plasticity() + calculate_force() on the same states, plus 2e-5."""
+    scale = np.abs(fo).max()
+    stiff = float(prm[0] * prm[1]) if kind == scenes.MAT_WATER else float(2 * prm[0] + 3 * prm[1])
+    tol = 2e-4 + 5e-7 * stiff * float(vol.max()) / scale
+    if O.ref_particles_available():
+        fr = np.array([O.ref_particle_step(kind, prm, cdg[i], F[i], ps[i], float(vol[i]))[2] for i in range(len(F))])
+        tol = min(tol, 2.0 * np.abs(fr - fo).max() / scale + 2e-5)
+    return tol
+
+
+def run_host_step(hm, kind, prm, F, cdg, ps, vol):
+    n = len(F)
+    Fd, psd, force = _cm(F), ps.copy(), np.zeros((n, 9), np.float32)
+    hm.hm_material_step(C.c_int64(n), C.c_int(kind), _p(prm), _p(_cm(cdg)), _p(Fd), _p(psd), _p(vol), _p(force))
+    return _math(Fd), psd, _math(force)
+
+
+@pytest.mark.parametrize("kind,regime,strain", edge_cases())
+def test_device_material_step_edges_match_oracle(hm, kind, regime, strain):
+    F, cdg, ps, vol, prm, Fo, pso, fo = edge_batch(kind, regime, strain)
+    Fd, psd, fd = run_host_step(hm, kind, prm, F, cdg, ps, vol)
+    err = edge_errors(kind, regime, F, cdg, Fd, psd, fd, Fo, pso, fo)
+    tol = dict(EDGE_TOL[regime])
+    if regime == "rotated":
+        tol["force"] = rotated_force_tol(kind, prm, cdg, F, ps, vol, fo)
+    print("host", kind, regime, strain, {k: "%.2e" % v for k, v in err.items()})
+    for k, v in err.items():
+        assert v <= tol[k], (k, v, tol[k])

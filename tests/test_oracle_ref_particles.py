@@ -5,8 +5,8 @@ friction_project of src/mpm_fwd.h:25-57, compiled where they lie (oracle/particl
 stand-in for the un-vendored taichi core headers (oracle/taichi_stub/taichi/*.h — VectorND/MatrixND,
 Config, svd/polar; its header says what is restated and which SVD convention it takes).  Golden
 vectors of that run are committed (tests/golden/particles_ref.npz); where the reference tree is
-present the code is also run live.  det F > 0 only: inverted elements depend on the SVD's sign
-convention (DESIGN.md §2)."""
+present the code is also run live, for det F > 0 and, where the reference is defined there (jelly, snow, sand), for
+inverted elements under the convention of DESIGN.md §2 (U, V in SO(3), the sign on the smallest singular value)."""
 import importlib.util
 import os
 
@@ -84,3 +84,28 @@ def test_sand_alpha_and_defaults_live():
         assert abs(L.ref_sand_alpha(O.C.c_float(phi)) - scenes.material_params(scenes.MAT_SAND, friction_angle=phi)[2]) <= 1e-7
     for kind in range(5):
         assert np.allclose(O.ref_default_params(kind), scenes.material_params(kind), rtol=3e-7, atol=0)
+
+
+@pytest.mark.skipif(not O.ref_particles_available(), reason="reference tree absent")
+@pytest.mark.parametrize("kind", [scenes.MAT_JELLY, scenes.MAT_SNOW, scenes.MAT_SAND])
+def test_oracle_constitutive_matches_reference_particles_live_inverted(kind):
+    # det F < 0 with distinct |sigma| (tests/material_states.py "inverted"): the reference's polar_decomp / svd with
+    # rotations U, V in SO(3) (the stand-in's svd_rot puts the sign on the smallest singular value, as the oracle's svd3
+    # does) and its signed j = determinant(dg_e) (src/particles.cpp:208, 392).  Jelly and snow keep the fixed-corotated
+    # stress of the reflected state; snow's clamp and sand's project() return positive singular values (un-inverted F)
+    from tests import material_states as MS
+    prm = O.ref_default_params(kind)
+    F, cdg, ps, _ = MS.states(kind, "inverted", 60, 11)
+    ref = [O.ref_particle_step(kind, prm, cdg[i], F[i], ps[i], G.VOL) for i in range(len(F))]
+    scale = max(np.abs(r[2]).max() for r in ref)
+    for i, (Fr, psr, fr) in enumerate(ref):
+        F1, ps1, force = _oracle_step(kind, prm, cdg[i], F[i], ps[i], np.float64)
+        assert np.isfinite(fr).all() and np.isfinite(Fr).all()
+        assert np.abs(F1 - Fr).max() <= 2e-6 * max(1.0, np.abs(Fr).max()), i
+        assert abs(ps1 - psr) <= 3e-6 * max(1.0, abs(psr)), i
+        assert np.abs(force - fr).max() <= FORCE_TOL[kind] * scale, i
+        if kind != scenes.MAT_JELLY:
+            assert np.linalg.det(F1) > 0                        # un-inverted
+        _, _, f0 = O.ref_particle_step(kind, prm, cdg[i], F[i], ps[i], G.VOL, do_plasticity=False)
+        if kind != scenes.MAT_SAND:                             # the Hencky stress of an inverted F is log of a negative sigma
+            assert np.abs(O.calculate_force(kind, prm.astype(np.float64), F[i].astype(np.float64), float(ps[i]), G.VOL, np.float64) - f0).max() <= FORCE_TOL[kind] * max(np.abs(f0).max(), scale)
