@@ -77,6 +77,9 @@ struct Counters {  // device-resident
   int n_live;         // scratch of k_count_live (mpmb_num_particles)
   unsigned long long updates;  // sum over substeps of the particles binned: the reference's update_counter (src/mpm.cpp:436)
   int g2p_done;       // CTAs of the running k_g2p that have finished (the last one commits the substep)
+  // tiles handed out beyond the first gridDim.x by the substep's k_p2g [0] / k_g2p [1] launch of each part (tile_in_part):
+  // each launch has its own counter, zeroed by the ordering that precedes the launches
+  int claim[2][3];
   int xstep;          // substeps completed since the peers were connected: the sequence number of the peer exchange
                       // (kept on the device so that a captured CUDA graph of a substep stays valid from replay to replay)
   int chk[8];         // MPMB_CHECKED builds: first violated index check {site, a, b, c, ...}
@@ -90,6 +93,38 @@ struct Counters {  // device-resident
 #define MPMB_CHK(cnt, cond, site, a, b, c) true
 #endif
 enum { DEVERR_TILE_CAPACITY = 1, DEVERR_MIGRATE_CAPACITY = 2, DEVERR_PARTICLE_CAPACITY = 4, DEVERR_PEER_TIMEOUT = 8, DEVERR_BAD_INPUT = 16 };
+
+// Tile-scheduling trace (-DMPMB_TILE_TRACE, read by bench_tail.py through mpmb_debug_tile_trace): every CTA of k_p2g,
+// k_grid and k_g2p records when it started and ended (%globaltimer, ns), its SM and the tiles and particle rows it
+// processed.  Each kernel keeps the records of its last launch.
+#ifdef MPMB_TILE_TRACE
+struct CtaTrace { unsigned long long t0, t1; int sm, tiles, rows, pad; };
+enum { TRACE_P2G = 0, TRACE_GRID = 1, TRACE_G2P = 2, TRACE_CTAS = 4096 };
+__device__ CtaTrace g_trace[3][TRACE_CTAS];
+#ifndef MPMB_SIMT_HOST
+__device__ __forceinline__ unsigned long long trace_clock() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ int trace_smid() {
+  int s;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+  return s;
+}
+#else
+__device__ __forceinline__ unsigned long long trace_clock() { return 0; }
+__device__ __forceinline__ int trace_smid() { return 0; }
+#endif
+#define MPMB_TRACE_BEGIN const unsigned long long trace_t0 = trace_clock(); int trace_tiles = 0, trace_rows = 0
+#define MPMB_TRACE_TILE(rows) (trace_tiles++, trace_rows += (rows))
+#define MPMB_TRACE_END(k) \
+  if (threadIdx.x == 0 && blockIdx.x < TRACE_CTAS) g_trace[k][blockIdx.x] = CtaTrace{trace_t0, trace_clock(), trace_smid(), trace_tiles, trace_rows, 0}
+#else
+#define MPMB_TRACE_BEGIN
+#define MPMB_TRACE_TILE(rows)
+#define MPMB_TRACE_END(k)
+#endif
 
 struct TileMeta {  // one 32-byte record per active tile (slot)
   int tile, run_begin, run_len, arr_off, arr_len, out_begin, xy, z;  // xy = tile x | y << 16, z = GLOBAL tile layer
@@ -664,6 +699,7 @@ __global__ void __launch_bounds__(1024) k_order_b(View V, int nblocks) {
     V.cnt->updates += (unsigned long long)carry[0];
     V.cnt->n_tiles = carry[2];
     V.cnt->n_ghost = 0;
+    for (int k = 0; k < 6; k++) (&V.cnt->claim[0][0])[k] = 0;
     if (carry[2] > V.cap_tiles) atomicOr(&V.cnt->error, DEVERR_TILE_CAPACITY);
     if (carry[0] > V.cap_particles) atomicOr(&V.cnt->error, DEVERR_PARTICLE_CAPACITY);
   }
@@ -891,13 +927,31 @@ __global__ void __launch_bounds__(P2G_T, 4) k_p2g(View V, Params P, int part) {
   const int own = tid & 63, half = tid >> 6;  // my cell, and which half of its stencil I accumulate (warp-uniform)
   const int cx = own >> 4, cy = (own >> 2) & 3, cz = own & 3;
   const int n_tiles = V.cnt->n_tiles;
-  for (int slot = blockIdx.x; slot < n_tiles; slot += gridDim.x) {
+  MPMB_TRACE_BEGIN;
+  // Tiles are handed out in slot order from the launch's counter (the first gridDim.x by block index): a CTA that drew
+  // small tiles takes more, so the launch ends at most one tile after its average CTA instead of with its most loaded
+  // one.  Thread 0 claims the next tile at the top of the current one and publishes it with the tile's last barrier,
+  // in s_claim[cp ^ 1] while everyone reads this tile's s_claim[cp].
+  __shared__ int s_claim[2];
+  int *const counter = &V.cnt->claim[0][part];
+  auto claim = [&](int slot) {  // the first tile of the part at or after `slot`, drawing replacements from the counter
+    while (slot < n_tiles && part != 0 && !tile_in_part(P, V.meta[slot].tile, part)) slot = (int)gridDim.x + atomicAdd(counter, 1);
+    return slot;
+  };
+  if (tid == 0) s_claim[0] = claim(blockIdx.x);
+  __syncthreads();
+  for (int slot = s_claim[0], cp = 0; slot < n_tiles; cp ^= 1, slot = s_claim[cp]) {
+    int ahead = 0;
+    if (tid == 0) ahead = (int)gridDim.x + atomicAdd(counter, 1);  // consumed after the tile's work: the latency is hidden
     const TileMeta tm = V.meta[slot];
-    const int tile = tm.tile;
-    if (!tile_in_part(P, tile, part)) continue;  // uniform per CTA
     const int nrow_tile = tm.run_len + tm.arr_len;
     if (!MPMB_CHK(V.cnt, tm.run_begin >= 0 && tm.run_len >= 0 && tm.arr_len >= 0 && tm.run_begin + tm.run_len <= V.cap_particles && tm.arr_off + tm.arr_len <= V.cap_particles &&
-                             tm.out_begin + nrow_tile <= V.cap_particles, 3, slot, tm.run_begin, tm.run_len)) continue;
+                             tm.out_begin + nrow_tile <= V.cap_particles, 3, slot, tm.run_begin, tm.run_len)) {
+      if (tid == 0) s_claim[cp ^ 1] = claim(ahead);
+      __syncthreads();
+      continue;
+    }
+    MPMB_TRACE_TILE(nrow_tile);
     MPMB_TILE_XYZ(P, tm, tx, ty, tz);
     const float fbx = (float)(tx * 4 + cx), fby = (float)(ty * 4 + cy), fbz = (float)(tz * 4 + cz);
     F4 acc[P2G_SPLIT];  // (p_x, p_y | p_z, m) of my half of my cell's stencil
@@ -1047,8 +1101,10 @@ __global__ void __launch_bounds__(P2G_T, 4) k_p2g(View V, Params P, int part) {
       out[n] = make_float4(s_arena[0][node] + ar1[0][node], s_arena[1][node] + ar1[1][node], s_arena[2][node] + ar1[2][node],
                            s_arena[3][node] + ar1[3][node]);
     }
+    if (tid == 0) s_claim[cp ^ 1] = claim(ahead);
     __syncthreads();
   }
+  MPMB_TRACE_END(TRACE_P2G);
 }
 
 
@@ -1109,10 +1165,17 @@ __global__ void __launch_bounds__(256, 1) k_grid(View V, Params P, float4 *vel, 
   const int lane = threadIdx.x & 31;
   const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
   const int n_tiles = V.cnt->n_tiles;
+  MPMB_TRACE_BEGIN;
+#ifdef MPMB_TILE_TRACE
+  __shared__ int s_trace[2];  // tiles and rows of the CTA's warps
+  if (threadIdx.x == 0) s_trace[0] = s_trace[1] = 0;
+  __syncthreads();
+#endif
   for (int slot = gw; slot < n_tiles; slot += nw) {
     const TileMeta tmg = V.meta[slot];
     const int tile = tmg.tile;
     if (!tile_in_part(P, tile, part)) continue;  // uniform per warp
+    MPMB_TRACE_TILE(tmg.run_len + tmg.arr_len);
     MPMB_TILE_XYZ(P, tmg, tx, ty, tz);
     int my_nb = -1;
     if (lane < 27) {
@@ -1138,6 +1201,13 @@ __global__ void __launch_bounds__(256, 1) k_grid(View V, Params P, float4 *vel, 
       if (n0 + lane < ARENA) vel[(size_t)slot * ARENA + n] = g;
     }
   }
+#ifdef MPMB_TILE_TRACE
+  if (lane == 0) { atomicAdd(&s_trace[0], trace_tiles); atomicAdd(&s_trace[1], trace_rows); }
+  __syncthreads();
+  trace_tiles = s_trace[0];
+  trace_rows = s_trace[1];
+#endif
+  MPMB_TRACE_END(TRACE_GRID);
 }
 
 // ------------------------------------------------------------------------------ G2P
@@ -1169,15 +1239,25 @@ __global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4
   constexpr int KPT = G2P_CH / BLOCK;
   const int tid = threadIdx.x;
   const int n_tiles = V.cnt->n_tiles;
+  MPMB_TRACE_BEGIN;
   const float scale = -4.0f * P.inv_dx * P.dt;  // src/transfer.cpp:938
+  // Tiles are handed out in slot order from the launch's counter (the first gridDim.x by block index), as in k_p2g.  The
+  // pipeline puts a tile's first chunk in flight while the previous tile's last chunk is computed, so thread 0 claims
+  // ONE TILE AHEAD: s_ahead[sp ^ 1] is the CTA's next tile, read by everyone at the tile change; thread 0 then claims the
+  // one after it into s_ahead[sp], which the end-of-chunk barrier publishes (sp alternates per tile, as for s_stay).  A
+  // tile's chunks stay with its CTA.  (No pointer or index of its own is kept live: the loop is at the register limit.)
+  __shared__ int s_ahead[2];
+  auto next_claim = [&]() { return (int)gridDim.x + atomicAdd(&V.cnt->claim[1][part], 1); };
+  auto claim = [&](int slot) {  // the first tile at or after `slot` this kernel processes, drawing replacements from the counter
+    // z-slab parts: tiles of the other part; CPIC scenes: tiles of rigid pages belong to k_g2p_rigid
+    while (slot < n_tiles && ((part != 0 && !tile_in_part(P, V.meta[slot].tile, part)) || (V.rigid_flag && V.rigid_flag[slot]))) slot = next_claim();
+    return slot;
+  };
+  int sp = 0;
   struct Item { int slot, rb, first; TileMeta tm; };
   auto first_item = [&](int slot) {
     Item it;
     it.rb = 0; it.first = 1;
-    if (part != 0)  // next tile of this CTA's round-robin share that belongs to the part
-      while (slot < n_tiles && !tile_in_part(P, V.meta[slot].tile, part)) slot += (int)gridDim.x;
-    if (V.rigid_flag)  // CPIC scenes: tiles of rigid pages belong to k_g2p_rigid
-      while (slot < n_tiles && V.rigid_flag[slot]) slot += (int)gridDim.x;
     it.slot = slot;
     if (slot < n_tiles) it.tm = V.meta[slot];
     else {
@@ -1188,7 +1268,7 @@ __global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4
   };
   auto next_item = [&](const Item &it) {
     if (it.rb + G2P_CH < it.tm.run_len + it.tm.arr_len) { Item n = it; n.rb += G2P_CH; n.first = 0; return n; }
-    return first_item(it.slot + (int)gridDim.x);
+    return first_item(s_ahead[sp ^ 1]);
   };
   // rows of the chunk that lie inside the tile's run (unit stride in storage) / alignment shift of their outpos words
   auto run_rows = [&](const Item &it) { return max(0, min(G2P_CH, it.tm.run_len - it.rb)); };
@@ -1241,16 +1321,20 @@ __global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4
     mbar_init_fence();
     s_stay[0] = 0;
     s_stay[1] = 0;
+    s_ahead[0] = claim(blockIdx.x);
+    s_ahead[1] = s_ahead[0] < n_tiles ? claim(next_claim()) : n_tiles;
   }
   __syncthreads();
-  Item cur = first_item(blockIdx.x);
-  int buf = 0, vbuf = 0, sp = 0;
+  Item cur = first_item(s_ahead[0]);
+  __syncthreads();  // s_ahead[0] is claimed into again at the first tile change
+  int buf = 0, vbuf = 0;
   unsigned phase = 0;  // bit b = parity of the phase stage b's barrier is in
   prefetch(cur, 0, 0);
   while (cur.slot < n_tiles) {
     const Item nxt = next_item(cur);
     const int nvbuf = nxt.first ? (vbuf ^ 1) : vbuf;
     prefetch(nxt, buf ^ 1, nvbuf);
+    if (tid == 0 && nxt.first && nxt.slot < n_tiles) s_ahead[sp] = claim(next_claim());  // nxt took the tile claimed ahead
     asm volatile("cp.async.wait_group 1;\n" ::: "memory");  // my arrival rows of the current item have landed; the next item stays in flight
     mbar_wait(&s_bar[buf], (phase >> buf) & 1u);              // ... and so have its bulk copies (every thread reads only rows it waited for)
     phase ^= 1u << buf;
@@ -1349,12 +1433,14 @@ __global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4
     if (nxt.slot != cur.slot) {
       if (tid == 0) { V.stay_next[cur.tm.tile] = s_stay[sp]; s_stay[sp] = 0; }
       sp ^= 1;
+      MPMB_TRACE_TILE(cur.tm.run_len + cur.tm.arr_len);
     }
     cur = nxt;
     buf ^= 1;
     vbuf = nvbuf;
   }
   cp_async_wait_all();
+  MPMB_TRACE_END(TRACE_G2P);
   // end of the substep: the lists and runs this kernel produced become the current ones — done by the last CTA to
   // finish (no separate 1-thread launch)
   if (commit) {
@@ -4452,6 +4538,19 @@ extern "C" int mpmb_debug_rows(MpmbHandle h, int n, uint32_t *keys, float *mass4
   return MPMB_OK;
 }
 #endif  // MPMB_DEBUG_EXPORTS
+#ifdef MPMB_TILE_TRACE
+// the per-CTA records of the last launch of kernel `which` (TRACE_P2G / TRACE_GRID / TRACE_G2P) as 32-byte
+// {t0, t1, sm, tiles, rows, -}; returns the launch's CTA count (records copied: at most cap)
+extern "C" int mpmb_debug_tile_trace(MpmbHandle h, int which, void *out, int cap) {
+  CHECK_HANDLE(h);
+  if (which < 0 || which > 2) return fail(h, MPMB_ERR_INVALID, "which must be 0 (k_p2g), 1 (k_grid) or 2 (k_g2p)");
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  const int ctas = which == TRACE_P2G ? h->grid_p2g : which == TRACE_GRID ? h->num_sms * 8 : h->grid_g2p;
+  const int n = std::min(std::min(ctas, cap), (int)TRACE_CTAS);
+  CUDA_TRY(h, cudaMemcpyFromSymbol(out, g_trace, sizeof(CtaTrace) * n, sizeof(CtaTrace) * TRACE_CTAS * which));
+  return ctas;
+}
+#endif  // MPMB_TILE_TRACE
 
 // ------------------------------------------------------------------------------ profiling
 int mpmb_set_profiling(MpmbHandle h, int32_t enabled) {
