@@ -586,6 +586,16 @@ class Engine:
         self._check(self.L.mpmb_get_ordering_stats(self.h, C.byref(a), C.byref(b), C.byref(c)))
         return dict(rows=a.value, movers=b.value, ghost_tiles=c.value)
 
+    def debug_check(self):
+        """Bounds-checked builds only (-DMPMB_CHECKED, build.CHECKED_LIB): [site, a, b, c] of the first index check that
+        failed (site 0: none failed), then n_store, n_alive, n_movers, n_tiles."""
+        f = getattr(self.L, "mpmb_debug_check", None)
+        if f is None:
+            raise RuntimeError("mpmb_debug_check is exported by the bounds-checked build only")
+        out = (C.c_int32 * 8)()
+        self._check(f(self.h, out))
+        return list(out)
+
     def get_counters(self):
         a, b, c = C.c_int64(0), C.c_int64(0), C.c_int64(0)
         self._check(self.L.mpmb_get_counters(self.h, C.byref(a), C.byref(b), C.byref(c)))
