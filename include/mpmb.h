@@ -294,7 +294,9 @@ int mpmb_download_grid(MpmbHandle h, int32_t which, float *dense4);
  *   - on the device, after mpmb_set_rigid_motion: every substep ends with advect_rigid_bodies (and, if asked for,
  *     rigid_body_levelset_collision) on an fp64 master state per body, scripted parts taken from a table the host uploads
  *     with mpmb_set_rigid_script.  mpmb_substep(h, n) then runs n whole coupled substeps and replays CUDA graphs.
- * Rigid-rigid collisions (rigidify) and articulation are not implemented.  Single-GPU engines only (world == 1).
+ * Rigid-rigid collisions (rigidify) and articulation are not implemented.  z-slab runs (world > 1): every rank holds every
+ * body and every boundary sample and rasterises the colour field over the whole node grid; each transfer's impulses are summed
+ * over the ranks in rank order (mpmb_rigid_* below), so the bodies are bit-identical on every rank.
  * What the device assumes of the core's RigidBody (it cannot be read here; SURVEY appendix C):
  *   get_velocity_at(p) = velocity + angular_velocity x (p - position);
  *   apply_tmp_impulse(j, p): tmp_velocity += inv_mass j, tmp_angular_velocity += inv_inertia ((p - position) x j);
@@ -360,7 +362,9 @@ int mpmb_set_rigid_motion(MpmbHandle h, int32_t n_bodies, const MpmbRigidMotion 
  * MPMB_ERR_INVALID.  The table is copied (synchronises).                                                               */
 int mpmb_set_rigid_script(MpmbHandle h, int32_t n_substeps, const double *poses);
 /* MPMParticle::states (src/particles.h) by particle id - id_base: set (default 0 for uploaded particles) / read together
- * with boundary_normal, boundary_distance and near_boundary_ of the last substep.  Any pointer may be NULL.            */
+ * with boundary_normal, boundary_distance and near_boundary_ of the last substep.  Any pointer may be NULL.
+ * z-slab ranks index both by the ABSOLUTE particle id (entry k = id k); only the entries of the particles the rank owns
+ * are meaningful.                                                                                                     */
 int mpmb_set_particle_states(MpmbHandle h, int64_t n, const uint32_t *states);
 int mpmb_get_particle_cdf(MpmbHandle h, int64_t n, uint32_t *states, float *normal3, float *distance, uint8_t *near_boundary);
 /* Parity/debug: the node colour field of the last substep, dense [res0+1][res1+1][res2+1]: GridState::states
@@ -483,9 +487,42 @@ int mpmb_recut_pack(MpmbHandle h, const int32_t *cuts, void *dev_buf, int64_t ca
  * largest id held), so the next free id of the run is unchanged; the whole set is ordered again from scratch.  Exchange
  * sequence numbers, the exchange buffers and the peers mapped into them (mpmb_xchg_connect) are untouched (their size
  * does not depend on the slab thickness): peer-connected ranks go on with mpmb_substep(h, n), whose first substep after
- * the re-cut runs outside the graph.  A rank may end with no particles.  Rigid bodies and AsyncMPM pools do not exist on
- * z-slab ranks.                                                                                                         */
+ * the re-cut runs outside the graph.  A rank may end with no particles.  With rigid coupling the records carry each
+ * particle's colour state (see below).  AsyncMPM pools do not exist on z-slab ranks.                                    */
 int mpmb_recut_apply(MpmbHandle h, int32_t tile_z0, int32_t tile_z1, int64_t n_in, const void *dev_records);
+
+/* Rigid bodies on z-slab ranks (world > 1, after mpmb_set_rigid_samples with the same samples, bodies and states on every
+ * rank).  A rank's transfers rewrite only its own tiles (those of the part being run) and sum only its own particles'
+ * impulses.  After each of the two transfers of a substep (mpmb_rasterize, or both of its parts; mpmb_resample, or both of
+ * its parts) every rank gathers all ranks' partial sums, adds them in rank order 0..world-1 and applies the sum; after the
+ * second one device-advanced bodies take their step.  Until then the next stage returns MPMB_ERR_STATE (mpmb_resample /
+ * mpmb_resample_part after the P2G transfer, mpmb_sort_particles_and_populate_grid, the slab edits, the re-cut and the
+ * rigid set-up calls after either).
+ * A particle's colour state (MPMParticle::states) travels with it: the migration and re-cut records carry it in row 9 .y
+ * (that row holds only apic_b[8] in .x), so record sizes are unchanged, and runs without rigid coupling move the same bytes
+ * as before.  The by-id colour arrays of a slab rank are indexed by ABSOLUTE id up to its id end (24 B per id per rank: state, normal + distance, mark):
+ * after per-rank uploads, raise every rank's id end to the run's (the maximum of mpmb_id_end over the ranks) with
+ * mpmb_append_owned_particles(n = 0, first_id = that maximum; taichi_mpm_b200/slab.py share_id_end does it, and
+ * connect_peers and SlabRunner call it); an immigrant past it raises the device error flag.
+ *
+ * Host transport: mpmb_rigid_impulse_pack writes this rank's partial sums (mpmb_rigid_impulse_bytes bytes) into a DEVICE
+ * buffer; the host all-gathers them into world consecutive blocks in rank order and every rank calls
+ * mpmb_rigid_impulse_apply on that gathered buffer.                                                                    */
+int64_t mpmb_rigid_impulse_bytes(MpmbHandle h);
+int mpmb_rigid_impulse_pack(MpmbHandle h, void *dev_buf);
+int mpmb_rigid_impulse_apply(MpmbHandle h, const void *dev_all);
+/* Peer transport: every rank owns a small mailbox that every other rank maps (CUDA IPC handle between processes, the
+ * pointer inside one process; mpmb_rigid_connect once per other rank).  mpmb_rigid_send stores this rank's partial sums
+ * into every mailbox and releases a sequence number system-wide; mpmb_rigid_recv waits for all ranks (a bounded spin: a
+ * missing peer raises the device error flag instead of hanging) and applies the sum.  With the halo peers and every
+ * mailbox connected, mpmb_substep(h, n) does both reductions itself and, with device-advanced bodies, replays graphs;
+ * with a mailbox unconnected it returns MPMB_ERR_STATE and enqueues nothing.  Hosts that drive the stages on one stream
+ * issue every rank's mpmb_rigid_send before any rank's mpmb_rigid_recv.                                               */
+int mpmb_rigid_mailbox(MpmbHandle h, void **dev_ptr);
+int mpmb_rigid_mailbox_ipc_handle(MpmbHandle h, void *out64);
+int mpmb_rigid_connect(MpmbHandle h, int32_t rank, const void *handle64, void *same_process_ptr);
+int mpmb_rigid_send(MpmbHandle h);
+int mpmb_rigid_recv(MpmbHandle h);
 
 #ifdef __cplusplus
 }

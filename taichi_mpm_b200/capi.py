@@ -34,6 +34,8 @@ EXPORTS = [
     "mpmb_xchg_buffer", "mpmb_xchg_ipc_handle", "mpmb_xchg_connect", "mpmb_halo_send", "mpmb_halo_recv", "mpmb_migrate_send", "mpmb_migrate_recv",
     "mpmb_async_init", "mpmb_async_add", "mpmb_async_block_limits", "mpmb_async_advance", "mpmb_async_size", "mpmb_async_download",
     "mpmb_layer_counts", "mpmb_recut_pack", "mpmb_recut_apply",
+    "mpmb_rigid_impulse_bytes", "mpmb_rigid_impulse_pack", "mpmb_rigid_impulse_apply", "mpmb_rigid_mailbox", "mpmb_rigid_mailbox_ipc_handle",
+    "mpmb_rigid_connect", "mpmb_rigid_send", "mpmb_rigid_recv",
 ]
 ASYNC_SMALLER, ASYNC_EQUAL, ASYNC_LARGER, ASYNC_SWAP, ASYNC_CLEAR = 1, 2, 4, 8, 16   # per-block flags of mpmb_async_advance
 RECORD_BYTES = 160   # one particle record of mpmb_recut_pack / mpmb_recut_apply (and of the migration messages)
@@ -112,6 +114,8 @@ def lib():
         L.mpmb_migrate_bytes.restype = C.c_int64
         L.mpmb_halo_bytes.argtypes = [C.c_void_p]
         L.mpmb_migrate_bytes.argtypes = [C.c_void_p]
+        L.mpmb_rigid_impulse_bytes.restype = C.c_int64
+        L.mpmb_rigid_impulse_bytes.argtypes = [C.c_void_p]
         L.mpmb_create.argtypes = [C.POINTER(MpmbConfig), C.POINTER(C.c_void_p)]
         for name in EXPORTS:
             getattr(L, name)  # AttributeError if a declared symbol is not exported
@@ -422,6 +426,7 @@ class Engine:
         off, tri = _f32(rigid["sample_offset"], (-1, 3)), _f32(rigid["sample_tri"], (-1, 9))
         rid = np.ascontiguousarray(rigid["sample_rigid"], np.int32)
         self._check(self.L.mpmb_set_rigid_samples(self.h, C.c_int32(len(rigid["inv_mass"])), C.c_int64(len(rid)), _ptr(off), _ptr(tri), _ptr(rid)))
+        self.rigid_coupled = len(rid) > 0
         if len(rid):
             self._check(self.L.mpmb_set_rigid_coupling(self.h, C.c_float(rigid.get("penalty", 0.0)), C.c_float(rigid.get("pushing_force", 20000.0))))
             self.set_rigid_state(rigid)
@@ -544,6 +549,38 @@ class Engine:
 
     def migrate_recv(self, face):
         self._check(self.L.mpmb_migrate_recv(self.h, C.c_int32(face)))
+
+    # --- rigid impulses of z-slab ranks: summed over the ranks after each transfer
+    def rigid_impulse_bytes(self):
+        return int(self.L.mpmb_rigid_impulse_bytes(self.h))
+
+    def rigid_impulse_pack(self, dev_ptr):
+        """This rank's partial impulse sums of the last transfer into a device buffer of rigid_impulse_bytes()."""
+        self._check(self.L.mpmb_rigid_impulse_pack(self.h, C.c_void_p(int(dev_ptr))))
+
+    def rigid_impulse_apply(self, dev_ptr):
+        """Sums the world ranks' partials (consecutive blocks in rank order, device memory) and applies them."""
+        self._check(self.L.mpmb_rigid_impulse_apply(self.h, C.c_void_p(int(dev_ptr))))
+
+    def rigid_mailbox(self):
+        p = C.c_void_p()
+        self._check(self.L.mpmb_rigid_mailbox(self.h, C.byref(p)))
+        return p.value
+
+    def rigid_mailbox_ipc_handle(self):
+        buf = (C.c_ubyte * 64)()
+        self._check(self.L.mpmb_rigid_mailbox_ipc_handle(self.h, buf))
+        return bytes(buf)
+
+    def rigid_connect(self, rank, handle=None, ptr=None):
+        hb = (C.c_ubyte * 64).from_buffer_copy(handle) if handle is not None else None
+        self._check(self.L.mpmb_rigid_connect(self.h, C.c_int32(rank), hb, C.c_void_p(ptr) if ptr else None))
+
+    def rigid_send(self):
+        self._check(self.L.mpmb_rigid_send(self.h))
+
+    def rigid_recv(self):
+        self._check(self.L.mpmb_rigid_recv(self.h))
 
     # --- re-cut of a z-slab run (device buffers: anything with data_ptr(), numel() and element_size(), e.g. torch tensors)
     def tile_range(self):

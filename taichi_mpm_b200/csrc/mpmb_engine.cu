@@ -1749,7 +1749,8 @@ __device__ __forceinline__ void load_tile_words(const RigidView &R, const Params
 
 // block_op_rigid of rasterize_optimized (src/transfer.cpp:367-463) for the tiles of rigid pages: rewrites the tile's arena
 // (k_p2g ran on it first and provided the output rows).  One CTA per tile, one thread per row, shared float atomics.
-__global__ void __launch_bounds__(128) k_p2g_rigid(View V, Params P, RigidView R) {
+// Owned tiles only (slots below n_tiles; a ghost slot holds a neighbour's partial sums), those of `part` (tile_in_part).
+__global__ void __launch_bounds__(128) k_p2g_rigid(View V, Params P, RigidView R, int part) {
   __shared__ float s_arena[4][ARENA];
   __shared__ uint32_t s_word[ARENA];
   __shared__ float s_acc[RIGID_MAX][6];
@@ -1759,6 +1760,7 @@ __global__ void __launch_bounds__(128) k_p2g_rigid(View V, Params P, RigidView R
     for (int slot = blockIdx.x; slot < n_tiles; slot += gridDim.x) {
     if (!R.tile_flag[slot]) continue;
     const TileMeta tm = V.meta[slot];
+    if (!tile_in_part(P, tm.tile, part)) continue;
     MPMB_TILE_XYZ(P, tm, tx, ty, tz);
     for (int n = tid; n < ARENA; n += blockDim.x) { s_arena[0][n] = 0.f; s_arena[1][n] = 0.f; s_arena[2][n] = 0.f; s_arena[3][n] = 0.f; }
     for (int n = tid; n < RIGID_MAX * 6; n += blockDim.x) (&s_acc[0][0])[n] = 0.f;
@@ -1850,6 +1852,30 @@ __global__ void k_rigid_apply(RigidView R) {
   }
   for (int k = 0; k < 6; k++) B.acc[k] = 0.f;
 }
+
+// z-slab ranks: each rank's transfers sum only its own particles' impulses.  Every rank sums the partials of all `world`
+// ranks (RIGID_IMPULSE_FLOATS floats each, rank r's at parts + r * stride floats) in rank order 0..world-1 and applies the
+// sum as k_rigid_apply does, so the bodies stay bit-identical on every rank.  One thread per body.
+constexpr int RIGID_IMPULSE_FLOATS = RIGID_MAX * 6;
+__device__ __forceinline__ void rigid_sum_apply(RigidView R, const float *parts, size_t stride, int world) {
+  const int b = threadIdx.x;
+  if (b >= R.n_bodies) return;
+  float s[6];
+  for (int k = 0; k < 6; k++) s[k] = parts[b * 6 + k];
+  for (int w = 1; w < world; w++)
+    for (int k = 0; k < 6; k++) s[k] += parts[(size_t)w * stride + b * 6 + k];
+  RigidDev &B = R.bodies[b];
+  for (int k = 0; k < 3; k++) {
+    B.vel[k] += B.inv_mass * s[k];
+    B.ang[k] += B.inv_inertia[k] * s[3] + B.inv_inertia[3 + k] * s[4] + B.inv_inertia[6 + k] * s[5];
+  }
+  for (int k = 0; k < 6; k++) B.acc[k] = 0.f;
+}
+// this rank's partial sums of the running transfer into out[RIGID_IMPULSE_FLOATS]
+__global__ void k_rigid_impulse_pack(RigidView R, float *out) {
+  for (int n = threadIdx.x; n < RIGID_IMPULSE_FLOATS; n += blockDim.x) out[n] = R.bodies[n / 6].acc[n % 6];
+}
+__global__ void k_rigid_impulse_apply(RigidView R, const float *parts, int world) { rigid_sum_apply(R, parts, RIGID_IMPULSE_FLOATS, world); }
 
 // Bodies advanced on the device (mpmb_set_rigid_motion): advect_rigid_bodies (src/mpm_rigid_body.cpp:273-287) and
 // rigid_body_levelset_collision (:347-384) with the arithmetic of HostRigidBody.advect / levelset_collision
@@ -2014,8 +2040,9 @@ __global__ void k_rigid_advance(RigidView R, MotionView M, Params P, float3 grav
 }
 
 // block_op_rigid of resample_optimized (src/transfer.cpp:706-835) + what k_g2p does for the ordering (output rows, keys,
-// movers, stay counts), for the tiles of rigid pages.  Launched BEFORE k_g2p, which commits the substep.
-__global__ void __launch_bounds__(128) k_g2p_rigid(View V, Params P, RigidView R, const float4 *vel) {
+// movers, stay counts), for the tiles of rigid pages.  Launched BEFORE k_g2p, which commits the substep.  Owned tiles of
+// `part` only, as k_p2g_rigid.
+__global__ void __launch_bounds__(128) k_g2p_rigid(View V, Params P, RigidView R, const float4 *vel, int part) {
   __shared__ float4 s_vel[ARENA];
   __shared__ uint32_t s_word[ARENA];
   __shared__ float s_acc[RIGID_MAX][6];
@@ -2028,6 +2055,7 @@ __global__ void __launch_bounds__(128) k_g2p_rigid(View V, Params P, RigidView R
     if (!R.tile_flag[slot]) continue;
     const TileMeta tm = V.meta[slot];
     const int tile = tm.tile;
+    if (!tile_in_part(P, tile, part)) continue;
     MPMB_TILE_XYZ(P, tm, tx, ty, tz);
     for (int n = tid; n < ARENA; n += blockDim.x) s_vel[n] = vel[(size_t)slot * ARENA + n];
     for (int n = tid; n < RIGID_MAX * 6; n += blockDim.x) (&s_acc[0][0])[n] = 0.f;
@@ -2270,10 +2298,36 @@ __global__ void k_halo_unpack(View V, Params P, int layer_z, int cap_xy, const i
   }
 }
 
+// CPIC colour state of the particles that change rank (z-slab ranks with rigid coupling; w == nullptr otherwise):
+// MPMParticle::states, kept by ABSOLUTE particle id on z-slab ranks (w[id], id < n), travels in row 9 .y of the record
+// (that row holds only apic_b[8] in .x), so the migration and re-cut records keep their size.  Without rigid coupling
+// the records are the raw rows.
+struct StateWords {
+  uint32_t *w;
+  int n;
+};
+__device__ __forceinline__ void copy_record(const StateWords &S, float4 *const *q, size_t i, float4 *rec, Counters *cnt) {
+#pragma unroll
+  for (int k = 0; k < N_Q - 1; k++) rec[k] = q[k][i];
+  float4 r9 = q[N_Q - 1][i];
+  if (S.w) {
+    const uint32_t id = __float_as_uint(q[6][i].w) & TAG_ID_MASK;
+    if (id < (uint32_t)S.n) r9.y = __uint_as_float(S.w[id]);
+    else { r9.y = 0.f; atomicOr(&cnt->error, DEVERR_BAD_INPUT); }
+  }
+  rec[N_Q - 1] = r9;
+}
+__device__ __forceinline__ void record_state_in(const StateWords &S, const float4 *rec, Counters *cnt) {
+  if (!S.w) return;
+  const uint32_t id = __float_as_uint(rec[6].w) & TAG_ID_MASK;
+  if (id < (uint32_t)S.n) S.w[id] = __float_as_uint(rec[N_Q - 1].y);
+  else atomicOr(&cnt->error, DEVERR_BAD_INPUT);   // an id past the run's id range (include/mpmb.h, mpmb_set_rigid_samples)
+}
+
 // Migration message: int4 header {count,0,0,0} | float4 record[cap][N_Q].  Emigrants are the movers
 // whose destination is the face's special key; their row in the (new) current storage is a hole
 // for everybody else, the key is set dead so that downloads skip it.
-__global__ void k_migrate_pack(View V, uint32_t key_face, uint32_t key_dead, int cap, int *hdr, float4 *rec) {
+__global__ void k_migrate_pack(View V, uint32_t key_face, uint32_t key_dead, int cap, int *hdr, float4 *rec, StateWords S) {
   const int n = V.cnt->n_movers;
   for (int m = blockIdx.x * blockDim.x + threadIdx.x; m < n; m += gridDim.x * blockDim.x) {
     if (V.mover_dst[m] != key_face) continue;
@@ -2282,14 +2336,13 @@ __global__ void k_migrate_pack(View V, uint32_t key_face, uint32_t key_dead, int
     V.keys[i] = key_dead;
     V.mover_dst[m] = key_dead;
     if (idx >= cap) { atomicOr(&V.cnt->error, DEVERR_MIGRATE_CAPACITY); continue; }
-#pragma unroll
-    for (int k = 0; k < N_Q; k++) rec[(size_t)idx * N_Q + k] = V.q[k][i];
+    copy_record(S, V.q, i, rec + (size_t)idx * N_Q, V.cnt);
   }
 }
 
 // Immigrants are appended after the last row of the current storage and enter the mover list, so the
 // next ordering bins them like any other particle that changed tile.
-__global__ void k_migrate_unpack(View V, Params P, int cap, const int *hdr, const float4 *rec) {
+__global__ void k_migrate_unpack(View V, Params P, int cap, const int *hdr, const float4 *rec, StateWords S) {
   const int count = min(hdr[0], cap);
   const int base = V.cnt->n_store, mbase = V.cnt->n_movers;
   for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < count; e += gridDim.x * blockDim.x) {
@@ -2298,6 +2351,7 @@ __global__ void k_migrate_unpack(View V, Params P, int cap, const int *hdr, cons
     float4 r0 = rec[(size_t)e * N_Q];
 #pragma unroll
     for (int k = 0; k < N_Q; k++) V.q[k][dst] = rec[(size_t)e * N_Q + k];
+    record_state_in(S, rec + (size_t)e * N_Q, V.cnt);
     const uint32_t key = make_key(P, r0.x, r0.y, r0.z);
     V.keys[dst] = key;
     V.mover_dst[mbase + e] = key;
@@ -2412,7 +2466,7 @@ __global__ void __launch_bounds__(128) k_halo_recv2(View V, Params P, int cap_xy
   }
 }
 
-__global__ void __launch_bounds__(256) k_migrate_send2(View V, uint32_t key_dead, int cap, XFace f0, XFace f1, int mask, int *xcount, int *done) {
+__global__ void __launch_bounds__(256) k_migrate_send2(View V, uint32_t key_dead, int cap, XFace f0, XFace f1, int mask, int *xcount, int *done, StateWords S) {
   const int n = V.cnt->n_movers;
   const int seq = V.cnt->xstep;  // k_g2p has committed this substep
   for (int m = blockIdx.x * blockDim.x + threadIdx.x; m < n; m += gridDim.x * blockDim.x) {
@@ -2425,15 +2479,14 @@ __global__ void __launch_bounds__(256) k_migrate_send2(View V, uint32_t key_dead
     V.mover_dst[m] = key_dead;
     if (idx >= cap) { atomicOr(&V.cnt->error, DEVERR_MIGRATE_CAPACITY); continue; }
     float4 *rec = (float4 *)((f == 0 ? f0.tx : f1.tx) + 16);
-#pragma unroll
-    for (int k = 0; k < N_Q; k++) rec[(size_t)idx * N_Q + k] = V.q[k][i];
+    copy_record(S, V.q, i, rec + (size_t)idx * N_Q, V.cnt);
   }
   xchg_publish_last(xcount, done, f0, f1, mask, seq);
 }
 
 // one CTA: waits for both neighbours, appends the immigrants of both faces after the last storage row, enters them in the
 // mover list and commits the counts
-__global__ void __launch_bounds__(1024) k_migrate_recv2(View V, Params P, int cap, XFace f0, XFace f1, int mask) {
+__global__ void __launch_bounds__(1024) k_migrate_recv2(View V, Params P, int cap, XFace f0, XFace f1, int mask, StateWords S) {
   __shared__ int s_n[2];
   const int seq = V.cnt->xstep;
   if (threadIdx.x == 0) {
@@ -2454,6 +2507,7 @@ __global__ void __launch_bounds__(1024) k_migrate_recv2(View V, Params P, int ca
     const float4 r0 = rec[0];
 #pragma unroll
     for (int k = 0; k < N_Q; k++) V.q[k][dst] = rec[k];
+    record_state_in(S, rec, V.cnt);
     const uint32_t key = make_key(P, r0.x, r0.y, r0.z);
     V.keys[dst] = key;
     V.mover_dst[mbase + e] = key;
@@ -2471,6 +2525,36 @@ __global__ void k_migrate_commit(Counters *c, const int *hdr, int cap, int cap_p
   const int n = min(min(hdr[0], cap), max(cap_particles - c->n_store, 0));
   c->n_store += n;
   c->n_movers += n;
+}
+
+// ---- rigid impulse mailboxes (z-slab ranks with rigid coupling, peer memory): every rank owns one mailbox of
+// [2 transfers][world] slots that every other rank maps; a slot is {0, seq} (16 B) + one rank's RIGID_IMPULSE_FLOATS
+// partial sums.  After transfer t a rank writes its partials into slot [t][rank] of EVERY mailbox, its own included, and
+// releases seq system-wide; then it waits for all `world` slots [t][*] of its own mailbox and sums them in rank order.
+// seq = the device exchange counter (+1 for the P2G transfer, which precedes k_g2p's commit), so a captured graph stays
+// valid.  A slot is not overwritten before every rank has read it: the next write to [t][r] follows rank r's reduction of
+// the other transfer, which waits for every rank's publication that follows its reduction of t.
+constexpr int RMAIL_SLOT = 320;   // bytes: 16 + 4 * RIGID_IMPULSE_FLOATS, rounded up
+static_assert(16 + 4 * RIGID_IMPULSE_FLOATS <= RMAIL_SLOT, "rigid mailbox slot");
+__global__ void k_rigid_mail_send(RigidView R, char *const *boxes, int world, int rank, int transfer, int seq_off, const Counters *cnt) {
+  const int seq = cnt->xstep + seq_off;
+  const size_t off = ((size_t)transfer * world + rank) * RMAIL_SLOT;
+  for (int j = 0; j < world; j++) {
+    float *dst = (float *)(boxes[j] + off + 16);
+    for (int n = threadIdx.x; n < RIGID_IMPULSE_FLOATS; n += blockDim.x) dst[n] = R.bodies[n / 6].acc[n % 6];
+  }
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (int j = 0; j < world; j++) asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"((int *)(boxes[j] + off) + 1), "r"(seq) : "memory");
+}
+__global__ void k_rigid_mail_recv(RigidView R, const char *mine, int world, int transfer, int seq_off, Counters *cnt) {
+  const int seq = cnt->xstep + seq_off;
+  const char *box = mine + (size_t)transfer * world * RMAIL_SLOT;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < world; w++) xchg_spin((const int *)(box + (size_t)w * RMAIL_SLOT), seq, cnt);
+  __syncthreads();
+  rigid_sum_apply(R, (const float *)(box + 16), RMAIL_SLOT / sizeof(float), world);
 }
 
 // ---- re-cut of the z slabs (mpmb_layer_counts, mpmb_recut_pack, mpmb_recut_apply), between substeps.  The GLOBAL tile layer
@@ -2514,12 +2598,11 @@ __global__ void k_layer_flags(const uint32_t *keys, const float4 *q0, int n, uin
 }
 
 // the rows k_layer_flags marked (prefix = its exclusive scan), in storage order, as migration records: N_Q raw float4 rows
-__global__ void k_recut_pack(View V, int n, const int *prefix, float4 *rec) {
+__global__ void k_recut_pack(View V, int n, const int *prefix, float4 *rec, StateWords S) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n || prefix[i + 1] == prefix[i]) return;
   const size_t o = (size_t)prefix[i];
-#pragma unroll
-  for (int k = 0; k < N_Q; k++) rec[o * N_Q + k] = V.q[k][i];
+  copy_record(S, V.q, i, rec + o * N_Q, V.cnt);
 }
 
 // the rows k_layer_flags marked, compacted in storage order into the other buffer and keyed under the new slicing P;
@@ -2554,12 +2637,13 @@ __global__ void __launch_bounds__(256) k_recut_check(Params P, int n, const floa
 }
 
 // the arriving records after row row0 of the current storage, keyed under P (as k_migrate_recv2 appends immigrants)
-__global__ void k_recut_unpack(View V, Params P, int n, int row0, const float4 *rec) {
+__global__ void k_recut_unpack(View V, Params P, int n, int row0, const float4 *rec, StateWords S) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n) return;
   const int dst = row0 + e;
 #pragma unroll
   for (int k = 0; k < N_Q; k++) V.q[k][dst] = rec[(size_t)e * N_Q + k];
+  record_state_in(S, rec + (size_t)e * N_Q, V.cnt);
   const float4 r0 = rec[(size_t)e * N_Q];
   V.keys[dst] = make_key(P, r0.x, r0.y, r0.z);
 }
@@ -2930,6 +3014,13 @@ struct MpmbEngine {
   DevBuf<int> s_order;                 // sample indices grouped by body; body b owns s_order[s_begin[b] .. s_begin[b + 1])
   int s_begin[RIGID_MAX + 1] = {};
   DevBuf<double> contact;
+  // z-slab ranks: the bodies' impulses are summed over the ranks after each transfer (mpmb_rigid_impulse_* / mpmb_rigid_*)
+  int rigid_pending = 0;               // 1 / 2: the P2G / G2P transfer has run here and its partial impulses await the reduction
+  bool rigid_sent = false;             // ... and were published into the mailboxes (mpmb_rigid_send)
+  DevBuf<char> rmail;                  // my impulse mailbox: [2 transfers][world] slots of RMAIL_SLOT bytes (allocated at create)
+  std::vector<char *> rmail_tx;        // [rank] every rank's mailbox as mapped here ([my rank] = rmail); not owned
+  std::vector<bool> rmail_ipc;         // [rank] rmail_tx was opened from an IPC handle (closed by mpmb_destroy)
+  DevBuf<char *> rmail_dev;            // rmail_tx on the device
   int64_t id_span_pending = 0;
   int64_t id_span = 0;   // ids of the resident particles lie in [id_base, id_base + id_span): uploads number 0..n-1, the seeded
                          // lattice numbers by lattice index (gaps where the boundary band is skipped)
@@ -3040,6 +3131,17 @@ static View make_view(MpmbEngine *h) {
   return V;
 }
 
+// The by-id colour arrays (p_states, p_cdf, p_mark) are indexed by id - rigid_id0 and must cover rigid_ids ids.  One engine:
+// the ids of its resident set, relative to id_base.  z-slab rank: ABSOLUTE ids below the id end, because a rank also holds
+// immigrants whose ids lie below its own id_base; the id end then has to cover the run's ids (include/mpmb.h).
+static uint32_t rigid_id0(const MpmbEngine *h) { return h->cfg.world > 1 ? 0u : h->id_base; }
+static int64_t rigid_ids(const MpmbEngine *h) { return h->cfg.world > 1 ? std::max<int64_t>(h->id_end, h->id_base) : h->id_span; }
+static StateWords state_words(MpmbEngine *h) {   // what the migration and re-cut records carry (nothing without rigid coupling)
+  StateWords S{};
+  if (h->rigid_on && h->p_states.get()) { S.w = h->p_states.get(); S.n = (int)h->p_states.size(); }
+  return S;
+}
+
 // the rigid coupling and the device-advanced bodies as the kernels take them, built at every launch as make_view is
 static RigidView rigid_view(MpmbEngine *h) {
   RigidView R{};
@@ -3055,7 +3157,7 @@ static RigidView rigid_view(MpmbEngine *h) {
   R.tile_flag = h->tile_flag.get();
   R.p_states = h->p_states.get(); R.p_cdf = h->p_cdf.get(); R.p_mark = h->p_mark.get();
   R.epoch = h->epoch.get();
-  R.id_base = h->id_base;
+  R.id_base = rigid_id0(h);
   R.id_cap = (int)h->p_states.size();
   R.penalty = h->penalty;
   R.pushing_force = h->pushing_force;
@@ -3276,6 +3378,12 @@ int mpmb_create(const MpmbConfig *cfg, MpmbHandle *out) {
       }
     if (h->xcount.alloc(32) != cudaSuccess) return bail("cudaMalloc exchange counters");
     cudaMemset(h->xcount.get(), 0, sizeof(int) * 32);  // [0],[4] halo counts, [8],[12] migration counts, [16],[20] finished-CTA counters
+    const size_t mail = (size_t)2 * h->cfg.world * RMAIL_SLOT;
+    if (h->rmail.alloc(mail) != cudaSuccess || h->rmail_dev.alloc(h->cfg.world) != cudaSuccess) return bail("cudaMalloc rigid mailbox");
+    cudaMemset(h->rmail.get(), 0, mail);
+    h->rmail_tx.assign(h->cfg.world, nullptr);
+    h->rmail_ipc.assign(h->cfg.world, false);
+    h->rmail_tx[h->cfg.rank] = h->rmail.get();
   }
   if (cfg->capacity > 0) {
     int rc = alloc_particles(h, cfg->capacity);
@@ -3293,6 +3401,8 @@ int mpmb_destroy(MpmbHandle h) {
   for (int k = 0; k < 2; k++)
     for (int f = 0; f < 2; f++)
       if (h->tx_ipc[k][f] && h->tx[k][f]) cudaIpcCloseMemHandle(h->tx[k][f]);
+  for (size_t r = 0; r < h->rmail_tx.size(); r++)
+    if (h->rmail_ipc[r] && h->rmail_tx[r]) cudaIpcCloseMemHandle(h->rmail_tx[r]);
   for (auto &e : h->events) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
   graph_reset(h);
   if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
@@ -3505,7 +3615,7 @@ static int finish_upload(MpmbEngine *h, int64_t n) {
   h->id_span_pending = 0;
   h->id_end = (int64_t)h->id_base + h->id_span;
   if (h->rigid_on) {  // new particles start with MPMParticle::states = 0 (mpmb_set_particle_states overrides)
-    int rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap));
+    int rc = rigid_reserve_ids(h, std::max<int64_t>(rigid_ids(h), h->cap));
     if (rc != MPMB_OK) return rc;
     CUDA_TRY(h, cudaMemsetAsync(h->p_states.get(), 0, sizeof(uint32_t) * h->p_states.size(), h->stream));
   }
@@ -3599,7 +3709,7 @@ int mpmb_append_particles(MpmbHandle h, int64_t n, const float *x, const float *
   if ((rc = pack_fields(h, n, x, v, F, b, mass, vol, scalar, group, ns, h->id_base + (uint32_t)id0)) != MPMB_OK) return rc;
   h->id_span = id0 + n;
   h->id_end = std::max<int64_t>(h->id_end, (int64_t)h->id_base + h->id_span);
-  if (h->rigid_on && (rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap))) != MPMB_OK) return rc;   // keeps the colours
+  if (h->rigid_on && (rc = rigid_reserve_ids(h, std::max<int64_t>(rigid_ids(h), h->cap))) != MPMB_OK) return rc;   // keeps the colours
   return reorder_from_scratch(h, (int64_t)ns + n);
 }
 
@@ -3613,7 +3723,7 @@ int mpmb_append_owned_particles(MpmbHandle h, int64_t n, const float *x, const f
   if (!n_kept) return fail(h, MPMB_ERR_INVALID, "null argument");
   *n_kept = 0;
   if (n < 0 || (n > 0 && (!x || !v || !mass || !vol))) return fail(h, MPMB_ERR_INVALID, "x, v, mass, vol are required");
-  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "append_owned runs between substeps, not inside one");
+  if (h->stage != 0 || h->rigid_pending) return fail(h, MPMB_ERR_STATE, "append_owned runs between substeps, not inside one");
   const int64_t end = std::max<int64_t>(h->id_end, h->id_base);
   if (first_id < end) return fail(h, MPMB_ERR_INVALID, "first_id %lld lies below the id end %lld", (long long)first_id, (long long)end);
   if (first_id + n > (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_CAPACITY, "particle ids exceed 2^%d", TAG_ID_BITS);
@@ -3637,7 +3747,10 @@ int mpmb_append_owned_particles(MpmbHandle h, int64_t n, const float *x, const f
   h->id_end = std::max<int64_t>(h->id_end, first_id + n);
   h->id_span = std::max<int64_t>(h->id_span, h->id_end - (int64_t)h->id_base);
   *n_kept = kept;
-  if (h->rigid_on && (rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap))) != MPMB_OK) return rc;   // keeps the colours
+  if (h->rigid_on) {   // keeps the colours; the new ids start with MPMParticle::states = 0, as after mpmb_append_particles
+    if ((rc = rigid_reserve_ids(h, std::max<int64_t>(rigid_ids(h), h->cap))) != MPMB_OK) return rc;
+    if (n > 0) CUDA_TRY(h, cudaMemsetAsync(h->p_states.get() + (first_id - rigid_id0(h)), 0, sizeof(uint32_t) * n, h->stream));
+  }
   return kept > 0 ? reorder_from_scratch(h, (int64_t)ns + kept) : MPMB_OK;
 }
 
@@ -3683,7 +3796,7 @@ int mpmb_delete_owned_inside_levelset(MpmbHandle h, int64_t *n_deleted) {
   CHECK_HANDLE(h);
   if (!n_deleted) return fail(h, MPMB_ERR_INVALID, "null argument");
   *n_deleted = 0;
-  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "delete_owned_inside_levelset runs between substeps, not inside one");
+  if (h->stage != 0 || h->rigid_pending) return fail(h, MPMB_ERR_STATE, "delete_owned_inside_levelset runs between substeps, not inside one");
   return delete_inside(h, n_deleted);
 }
 
@@ -3998,7 +4111,7 @@ static int rigid_reserve_ids(MpmbEngine *h, int64_t n_ids) {
 
 // per substep, after the ordering: pages + colour field of this pose, tile flags, particle colours
 static int rigid_prepare(MpmbEngine *h, const View &V, int *nl) {
-  if (!h->p_states.get() || (int64_t)h->p_states.size() < h->id_span) { int rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap)); if (rc != MPMB_OK) return rc; }
+  if (!h->p_states.get() || (int64_t)h->p_states.size() < rigid_ids(h)) { int rc = rigid_reserve_ids(h, std::max<int64_t>(rigid_ids(h), h->cap)); if (rc != MPMB_OK) return rc; }
   const RigidView R = rigid_view(h);
   const int ns = R.n_samples, sb = (ns + 127) / 128;
   k_cdf_clear<<<sb, 128, 0, h->stream>>>(R, h->P);
@@ -4012,7 +4125,7 @@ static int rigid_prepare(MpmbEngine *h, const View &V, int *nl) {
 
 int mpmb_set_rigid_samples(MpmbHandle h, int32_t n_bodies, int64_t n_samples, const float *offset3, const float *tri9, const int32_t *rigid_id) {
   CHECK_HANDLE(h);
-  if (h->cfg.world > 1) return fail(h, MPMB_ERR_STATE, "rigid coupling is implemented for single-GPU engines (world == 1)");
+  if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "rigid samples change between substeps, not inside one");
   if (n_samples == 0) { h->rigid_on = false; h->motion_on = false; graph_reset(h); return MPMB_OK; }
   if (n_bodies < 2 || n_bodies > RIGID_MAX || n_samples < 0 || n_samples > (1 << 24) || !offset3 || !tri9 || !rigid_id)
     return fail(h, MPMB_ERR_INVALID, "need 2..%d bodies (entry 0 is the background body) and their boundary samples", RIGID_MAX);
@@ -4085,6 +4198,7 @@ int mpmb_set_rigid_state(MpmbHandle h, int32_t n_bodies, const MpmbRigidBody *bo
   CHECK_HANDLE(h);
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies: call mpmb_set_rigid_samples first");
   if (n_bodies != h->rigid_bodies || !bodies) return fail(h, MPMB_ERR_INVALID, "expected %d bodies", h->rigid_bodies);
+  if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "z-slab rank: the bodies change after the impulse reduction, not before it");
   RigidDev dev[RIGID_MAX];
   memset(dev, 0, sizeof(dev));
   for (int b = 0; b < n_bodies; b++) {
@@ -4131,7 +4245,7 @@ int mpmb_set_rigid_motion(MpmbHandle h, int32_t n_bodies, const MpmbRigidMotion 
   CHECK_HANDLE(h);
   if (n_bodies == 0) { h->motion_on = false; graph_reset(h); return MPMB_OK; }
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies: call mpmb_set_rigid_samples first");
-  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "rigid motion changes between substeps, not inside one");
+  if (h->stage != 0 || h->rigid_pending) return fail(h, MPMB_ERR_STATE, "rigid motion changes between substeps, not inside one");
   if (n_bodies != h->rigid_bodies || !motion) return fail(h, MPMB_ERR_INVALID, "expected %d motion records", h->rigid_bodies);
   bool scripted = false;
   for (int b = 1; b < n_bodies; b++) {
@@ -4173,7 +4287,7 @@ int mpmb_set_rigid_motion(MpmbHandle h, int32_t n_bodies, const MpmbRigidMotion 
 int mpmb_set_rigid_script(MpmbHandle h, int32_t n_substeps, const double *poses) {
   CHECK_HANDLE(h);
   if (!h->rigid_on || !h->motion_on) return fail(h, MPMB_ERR_STATE, "no device-advanced bodies: call mpmb_set_rigid_motion first");
-  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "the script changes between substeps, not inside one");
+  if (h->stage != 0 || h->rigid_pending) return fail(h, MPMB_ERR_STATE, "the script changes between substeps, not inside one");
   if (n_substeps < 0 || (n_substeps > 0 && !poses)) return fail(h, MPMB_ERR_INVALID, "need n_substeps >= 0 and a table");
   const int nb = h->rigid_bodies;
   const size_t n = (size_t)n_substeps * nb * SCRIPT_STRIDE;
@@ -4268,6 +4382,7 @@ int mpmb_download_cdf(MpmbHandle h, uint32_t *node_states, float *node_distance)
 int mpmb_sort_particles_and_populate_grid(MpmbHandle h) {
   CHECK_HANDLE(h);
   if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "sort must follow resample/upload");
+  if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "z-slab rank: the G2P rigid impulses of the last substep have not been reduced");
   prof_begin(h, 0);
   int nl = 3;
   if (h->cap > 0) {
@@ -4304,10 +4419,14 @@ int mpmb_rasterize(MpmbHandle h) {
   if (h->cap > 0) k_p2g<<<h->grid_p2g, P2G_T, P2G_DYN_BYTES, h->stream>>>(V, h->P, 0);
   h->launches += 1;
   if (h->cap > 0 && h->rigid_on) {  // block_op_rigid for the tiles of rigid pages, then apply_tmp_velocity (src/transfer.cpp:578-580)
-    k_p2g_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h));
-    k_rigid_apply<<<1, 32, 0, h->stream>>>(rigid_view(h));
-    h->launches += 2;
+    k_p2g_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h), 0);
+    h->launches += 1;
+    if (h->cfg.world == 1) {
+      k_rigid_apply<<<1, 32, 0, h->stream>>>(rigid_view(h));
+      h->launches += 1;
+    }
   }
+  if (h->rigid_on && h->cfg.world > 1) h->rigid_pending = 1;   // z-slab rank: the impulses are summed over the ranks first
   prof_end(h, 1);
   CUDA_TRY(h, cudaGetLastError());
   h->stage = 2;
@@ -4330,8 +4449,10 @@ static void launch_g2p(MpmbEngine *h, const View &V, int part, int commit, bool 
 int mpmb_resample(MpmbHandle h) {
   CHECK_HANDLE(h);
   if (h->stage != 2) return fail(h, MPMB_ERR_STATE, "resample must follow rasterize");
+  if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "z-slab rank: reduce the P2G rigid impulses over the ranks before the resample");
   const bool motion = h->rigid_on && h->motion_on;
   if (motion && h->motion_scripted && h->script_left < 1) return fail(h, MPMB_ERR_STATE, "the rigid script has no entry left for this substep");
+  const bool slab_rigid = h->rigid_on && h->cfg.world > 1;   // the G2P impulses, then the advance, follow the reduction
   View V = make_view(h);
   prof_begin(h, 4);
   if (h->cap > 0) k_grid<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, h->vel.get(), 0);
@@ -4339,16 +4460,17 @@ int mpmb_resample(MpmbHandle h) {
   prof_begin(h, 2);
   if (h->cap > 0) {
     if (h->rigid_on) {
-      k_g2p_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h), h->vel.get());
+      k_g2p_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h), h->vel.get(), 0);
       h->launches += 1;
     }
     launch_g2p(h, V, 0, 1, !h->skip_b || h->rigid_on);   // rigid tiles read apic_b back (the impulse needs dt * force)
-    if (h->rigid_on) {
+    if (h->rigid_on && !slab_rigid) {
       k_rigid_apply<<<1, 32, 0, h->stream>>>(rigid_view(h));       // src/transfer.cpp:967-969
       h->launches += 1;
     }
   }
-  if (motion) launch_rigid_motion(h);                    // advect_rigid_bodies (src/mpm_rigid_body.cpp:273-287)
+  if (motion && !slab_rigid) launch_rigid_motion(h);     // advect_rigid_bodies (src/mpm_rigid_body.cpp:273-287)
+  if (slab_rigid) h->rigid_pending = 2;
   h->launches += 2;
   prof_end(h, 1);
   CUDA_TRY(h, cudaGetLastError());
@@ -4361,6 +4483,9 @@ int mpmb_resample(MpmbHandle h) {
 }
 
 static bool peers_connected(MpmbEngine *h);
+static bool rigid_connected(MpmbEngine *h);
+static void rigid_mail_send(MpmbEngine *h);
+static int rigid_mail_recv(MpmbEngine *h);
 static int xchg_halo_fused(MpmbEngine *h);
 static int xchg_migrate_fused(MpmbEngine *h);
 int mpmb_halo_send(MpmbHandle h, int32_t face);
@@ -4378,6 +4503,12 @@ int mpmb_rasterize_part(MpmbHandle h, int32_t part) {
   View V = make_view(h);
   if (h->cap > 0) k_p2g<<<h->grid_p2g, P2G_T, P2G_DYN_BYTES, h->stream>>>(V, h->P, part);
   h->launches += 1;
+  const bool slab_rigid = h->rigid_on && h->cfg.world > 1;
+  if (h->cap > 0 && slab_rigid) {   // the boundary layers' rigid arenas are final before halo_pack / halo_send
+    k_p2g_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h), part);
+    h->launches += 1;
+  }
+  if (slab_rigid && part == 2) h->rigid_pending = 1;
   prof_end(h, 1);
   CUDA_TRY(h, cudaGetLastError());
   h->stage = part == 1 ? 11 : 2;
@@ -4388,17 +4519,26 @@ int mpmb_resample_part(MpmbHandle h, int32_t part) {
   CHECK_HANDLE(h);
   if (part != 1 && part != 2) return fail(h, MPMB_ERR_INVALID, "part must be 1 (boundary) or 2 (interior)");
   if (!((part == 2 && h->stage == 2) || (part == 1 && h->stage == 22))) return fail(h, MPMB_ERR_STATE, "resample_part: interior first, then boundary, after rasterize");
+  if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "z-slab rank: reduce the P2G rigid impulses over the ranks before the resample");
+  const bool slab_rigid = h->rigid_on && h->cfg.world > 1;
+  if (slab_rigid && h->motion_on && h->motion_scripted && h->script_left < 1)
+    return fail(h, MPMB_ERR_STATE, "the rigid script has no entry left for this substep");
   prof_begin(h, 2);
   View V = make_view(h);
   int nl = 2;
   if (h->cap > 0) {
     k_grid<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, h->vel.get(), part);
+    if (slab_rigid) {
+      k_g2p_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h), h->vel.get(), part);
+      nl++;
+    }
     launch_g2p(h, V, part, part == 1 ? 1 : 0, true);
   }
   h->launches += nl;
   prof_end(h, nl);
   CUDA_TRY(h, cudaGetLastError());
   if (part == 2) { h->stage = 22; return MPMB_OK; }
+  if (slab_rigid) h->rigid_pending = 2;
   h->cur ^= 1;
   h->ord ^= 1;
   h->mov ^= 1;
@@ -4412,6 +4552,10 @@ static int substep_once(MpmbEngine *h, bool peers, bool skip_b) {
   int rc;
   if ((rc = mpmb_sort_particles_and_populate_grid(h)) != MPMB_OK) return rc;
   if ((rc = mpmb_rasterize(h)) != MPMB_OK) return rc;
+  if (peers && h->rigid_pending) {   // rigid z-slab rank: the P2G impulses summed over the ranks through the mailboxes
+    rigid_mail_send(h);
+    if ((rc = rigid_mail_recv(h)) != MPMB_OK) return rc;
+  }
   if (peers && (rc = xchg_halo_fused(h)) != MPMB_OK) return rc;  // boundary-layer arenas into the neighbours' memory, theirs in as ghosts
   h->skip_b = skip_b;
 #ifdef MPMB_CHECKED
@@ -4420,6 +4564,10 @@ static int substep_once(MpmbEngine *h, bool peers, bool skip_b) {
   rc = mpmb_resample(h);
   h->skip_b = false;
   if (rc != MPMB_OK) return rc;
+  if (peers && h->rigid_pending) {   // ... and the G2P impulses, then the device advance
+    rigid_mail_send(h);
+    if ((rc = rigid_mail_recv(h)) != MPMB_OK) return rc;
+  }
   if (peers && (rc = xchg_migrate_fused(h)) != MPMB_OK) return rc;
   return MPMB_OK;
 }
@@ -4450,6 +4598,7 @@ static int graph_capture_pair(MpmbEngine *h, bool peers) {
     h->graph_exec[par] = nullptr;
     h->use_graph = false;
     h->cur = cur0; h->ord = ord0; h->mov = mov0; h->xstep = x0; h->stage = 0; h->launches = l0; h->script_left = left0;   // nothing has run
+    h->rigid_pending = 0; h->rigid_sent = false;
     h->sticky_cuda = false;
     return MPMB_OK;
   }
@@ -4462,12 +4611,14 @@ int mpmb_substep(MpmbHandle h, int32_t nsub) {
   CHECK_HANDLE(h);
   const bool peers = peers_connected(h);
   if (h->cfg.world > 1 && !peers) return fail(h, MPMB_ERR_STATE, "z-slab run: connect the peers (mpmb_xchg_connect) or drive the stages and move the buffers yourself");
+  if (h->cfg.world > 1 && h->rigid_on && !rigid_connected(h))
+    return fail(h, MPMB_ERR_STATE, "z-slab run with rigid bodies: connect every rank's rigid mailbox (mpmb_rigid_connect) or drive the stages yourself");
   int s = 0, rc;
   if (nsub > 0 && h->rigid_on && h->motion_on && h->motion_scripted && h->script_left < nsub)
     return fail(h, MPMB_ERR_STATE, "the rigid script has %lld entries left, %d substeps asked", (long long)h->script_left, nsub);
   // the by-id colour arrays cover every id before any capture: allocating them inside one would end graph replay for good
-  if (nsub > 0 && h->rigid_on && h->cap > 0 && (!h->p_states.get() || (int64_t)h->p_states.size() < h->id_span) &&
-      (rc = rigid_reserve_ids(h, std::max<int64_t>(h->id_span, h->cap))) != MPMB_OK)
+  if (nsub > 0 && h->rigid_on && h->cap > 0 && (!h->p_states.get() || (int64_t)h->p_states.size() < rigid_ids(h)) &&
+      (rc = rigid_reserve_ids(h, std::max<int64_t>(rigid_ids(h), h->cap))) != MPMB_OK)
     return rc;
   // the first substep after an upload takes the radix-sorted arrival lists (a different ordering launch): never in a graph
   if (h->fresh && nsub > 0) {
@@ -4665,7 +4816,7 @@ int mpmb_migrate_pack(MpmbHandle h, int32_t face, void *dev_buf) {
   CUDA_TRY(h, cudaMemsetAsync(b, 0, 16, h->stream));
   View V = make_view(h);
   const uint32_t key_face = h->special_min + (face == 0 ? SPECIAL_MIG_DOWN : SPECIAL_MIG_UP);
-  k_migrate_pack<<<h->num_sms * 2, 256, 0, h->stream>>>(V, key_face, h->key_dead, (int)h->mig_cap, (int *)b, (float4 *)(b + 16));
+  k_migrate_pack<<<h->num_sms * 2, 256, 0, h->stream>>>(V, key_face, h->key_dead, (int)h->mig_cap, (int *)b, (float4 *)(b + 16), state_words(h));
   h->launches++;
   prof_end(h, 1);
   CUDA_TRY(h, cudaGetLastError());
@@ -4680,7 +4831,7 @@ int mpmb_migrate_unpack(MpmbHandle h, int32_t face, const void *dev_buf) {
   prof_begin(h, 3);
   const char *b = (const char *)dev_buf;
   View V = make_view(h);
-  k_migrate_unpack<<<64, 256, 0, h->stream>>>(V, h->P, (int)h->mig_cap, (const int *)b, (const float4 *)(b + 16));
+  k_migrate_unpack<<<64, 256, 0, h->stream>>>(V, h->P, (int)h->mig_cap, (const int *)b, (const float4 *)(b + 16), state_words(h));
   k_migrate_commit<<<1, 1, 0, h->stream>>>(h->cnt.get(), (const int *)b, (int)h->mig_cap, (int)h->cap);
   h->launches += 2;
   prof_end(h, 2);
@@ -4728,6 +4879,7 @@ int mpmb_xchg_connect(MpmbHandle h, int32_t kind, int32_t face, const void *hand
   for (int f = 0; f < 2; f++)
     if (h->rx[kind][f].get()) CUDA_TRY(h, cudaMemset(h->rx[kind][f].get(), 0, 16));
   CUDA_TRY(h, cudaMemset(&h->cnt.get()->xstep, 0, sizeof(int)));
+  CUDA_TRY(h, cudaMemset(h->rmail.get(), 0, h->rmail.size()));   // the rigid mailbox's seq words restart with the sequence too
   h->xstep = 0;
   graph_reset(h);
   return MPMB_OK;
@@ -4788,11 +4940,12 @@ static int xchg_migrate_launch(MpmbEngine *h, int mask_send, int mask_recv) {
   View V = make_view(h);
   int nl = 0;
   if (mask_send & mask) {
-    k_migrate_send2<<<h->num_sms * 2, 256, 0, h->stream>>>(V, h->key_dead, (int)h->mig_cap, f[0], f[1], mask_send & mask, h->xcount.get() + 8, h->xcount.get() + 20);
+    k_migrate_send2<<<h->num_sms * 2, 256, 0, h->stream>>>(V, h->key_dead, (int)h->mig_cap, f[0], f[1], mask_send & mask, h->xcount.get() + 8, h->xcount.get() + 20,
+                                                          state_words(h));
     nl++;
   }
   if (mask_recv & mask) {
-    k_migrate_recv2<<<1, 1024, 0, h->stream>>>(V, h->P, (int)h->mig_cap, f[0], f[1], mask_recv & mask);
+    k_migrate_recv2<<<1, 1024, 0, h->stream>>>(V, h->P, (int)h->mig_cap, f[0], f[1], mask_recv & mask, state_words(h));
     nl++;
   }
   h->launches += nl;
@@ -4840,10 +4993,124 @@ int mpmb_migrate_recv(MpmbHandle h, int32_t face) {
   return xchg_migrate_launch(h, 0, 1 << face);
 }
 
+// ------------------------------------------------------------------------------ rigid impulses of z-slab ranks
+static int rigid_reduce_allowed(MpmbEngine *h, const char *what) {
+  if (h->cfg.world <= 1 || !h->rigid_on) return fail(h, MPMB_ERR_STATE, "%s: z-slab ranks with rigid coupling only", what);
+  if (!h->rigid_pending) return fail(h, MPMB_ERR_STATE, "%s follows a whole transfer (rasterize or resample, both parts)", what);
+  return MPMB_OK;
+}
+// the sum is applied: after the G2P transfer the device-advanced bodies take their step (as mpmb_resample does on one engine)
+static int rigid_reduced(MpmbEngine *h) {
+  if (h->rigid_pending == 2 && h->motion_on) launch_rigid_motion(h);
+  h->rigid_pending = 0;
+  h->rigid_sent = false;
+  CUDA_TRY(h, cudaGetLastError());
+  return MPMB_OK;
+}
+static bool rigid_connected(MpmbEngine *h) {
+  for (char *p : h->rmail_tx)
+    if (!p) return false;
+  return !h->rmail_tx.empty();
+}
+static void rigid_mail_send(MpmbEngine *h) {
+  k_rigid_mail_send<<<1, 128, 0, h->stream>>>(rigid_view(h), h->rmail_dev.get(), h->cfg.world, h->cfg.rank, h->rigid_pending - 1, h->rigid_pending == 1 ? 1 : 0, h->cnt.get());
+  h->launches++;
+  h->rigid_sent = true;
+}
+static int rigid_mail_recv(MpmbEngine *h) {
+  k_rigid_mail_recv<<<1, 128, 0, h->stream>>>(rigid_view(h), h->rmail.get(), h->cfg.world, h->rigid_pending - 1, h->rigid_pending == 1 ? 1 : 0, h->cnt.get());
+  h->launches++;
+  return rigid_reduced(h);
+}
+
+int64_t mpmb_rigid_impulse_bytes(MpmbHandle h) {
+  if (!h || h->cfg.world <= 1) return 0;
+  return (int64_t)sizeof(float) * RIGID_IMPULSE_FLOATS;
+}
+
+int mpmb_rigid_impulse_pack(MpmbHandle h, void *dev_buf) {
+  CHECK_HANDLE(h);
+  int rc = rigid_reduce_allowed(h, "rigid_impulse_pack");
+  if (rc != MPMB_OK) return rc;
+  if (!dev_buf) return fail(h, MPMB_ERR_INVALID, "null buffer");
+  k_rigid_impulse_pack<<<1, 128, 0, h->stream>>>(rigid_view(h), (float *)dev_buf);
+  h->launches++;
+  CUDA_TRY(h, cudaGetLastError());
+  return MPMB_OK;
+}
+
+int mpmb_rigid_impulse_apply(MpmbHandle h, const void *dev_all) {
+  CHECK_HANDLE(h);
+  int rc = rigid_reduce_allowed(h, "rigid_impulse_apply");
+  if (rc != MPMB_OK) return rc;
+  if (!dev_all) return fail(h, MPMB_ERR_INVALID, "null buffer");
+  k_rigid_impulse_apply<<<1, 32, 0, h->stream>>>(rigid_view(h), (const float *)dev_all, h->cfg.world);
+  h->launches++;
+  return rigid_reduced(h);
+}
+
+int mpmb_rigid_mailbox(MpmbHandle h, void **dev_ptr) {
+  CHECK_HANDLE(h);
+  if (h->cfg.world <= 1 || !dev_ptr) return fail(h, MPMB_ERR_INVALID, "bad argument");
+  *dev_ptr = h->rmail.get();
+  return MPMB_OK;
+}
+
+int mpmb_rigid_mailbox_ipc_handle(MpmbHandle h, void *out64) {
+  CHECK_HANDLE(h);
+  if (h->cfg.world <= 1 || !out64) return fail(h, MPMB_ERR_INVALID, "bad argument");
+  cudaIpcMemHandle_t hd;
+  CUDA_TRY(h, cudaIpcGetMemHandle(&hd, h->rmail.get()));
+  memcpy(out64, &hd, 64);
+  return MPMB_OK;
+}
+
+int mpmb_rigid_connect(MpmbHandle h, int32_t rank, const void *handle64, void *same_process_ptr) {
+  CHECK_HANDLE(h);
+  if (h->cfg.world <= 1 || rank < 0 || rank >= h->cfg.world || rank == h->cfg.rank) return fail(h, MPMB_ERR_INVALID, "bad rank %d", rank);
+  if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "rigid mailboxes connect between substeps");
+  if (h->rmail_ipc[rank] && h->rmail_tx[rank]) cudaIpcCloseMemHandle(h->rmail_tx[rank]);
+  h->rmail_tx[rank] = nullptr;
+  h->rmail_ipc[rank] = false;
+  if (same_process_ptr) {
+    h->rmail_tx[rank] = (char *)same_process_ptr;
+  } else {
+    if (!handle64) return fail(h, MPMB_ERR_INVALID, "handle or pointer required");
+    cudaIpcMemHandle_t hd;
+    memcpy(&hd, handle64, 64);
+    void *p = nullptr;
+    CUDA_TRY(h, cudaIpcOpenMemHandle(&p, hd, cudaIpcMemLazyEnablePeerAccess));
+    h->rmail_tx[rank] = (char *)p;
+    h->rmail_ipc[rank] = true;
+  }
+  CUDA_TRY(h, cudaMemcpy(h->rmail_dev.get(), h->rmail_tx.data(), sizeof(char *) * h->cfg.world, cudaMemcpyHostToDevice));
+  graph_reset(h);
+  return MPMB_OK;
+}
+
+int mpmb_rigid_send(MpmbHandle h) {
+  CHECK_HANDLE(h);
+  int rc = rigid_reduce_allowed(h, "rigid_send");
+  if (rc != MPMB_OK) return rc;
+  if (!rigid_connected(h)) return fail(h, MPMB_ERR_STATE, "rigid_send: connect every rank's mailbox first (mpmb_rigid_connect)");
+  if (h->rigid_sent) return fail(h, MPMB_ERR_STATE, "rigid_send: this transfer's impulses were sent already");
+  rigid_mail_send(h);
+  CUDA_TRY(h, cudaGetLastError());
+  return MPMB_OK;
+}
+
+int mpmb_rigid_recv(MpmbHandle h) {
+  CHECK_HANDLE(h);
+  int rc = rigid_reduce_allowed(h, "rigid_recv");
+  if (rc != MPMB_OK) return rc;
+  if (!h->rigid_sent) return fail(h, MPMB_ERR_STATE, "rigid_recv follows rigid_send");
+  return rigid_mail_recv(h);
+}
+
 // ------------------------------------------------------------------------------ re-cut of the z slabs
 static int recut_allowed(MpmbEngine *h, const char *what) {
   if (h->cfg.world <= 1) return fail(h, MPMB_ERR_STATE, "%s re-cuts z-slab runs (world > 1)", what);
-  if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "%s runs between substeps, not inside one", what);
+  if (h->stage != 0 || h->rigid_pending) return fail(h, MPMB_ERR_STATE, "%s runs between substeps, not inside one", what);
   return MPMB_OK;
 }
 
@@ -4911,7 +5178,7 @@ int mpmb_recut_pack(MpmbHandle h, const int32_t *cuts, void *dev_buf, int64_t ca
     int got = 0;
     if ((rc = scan_flags(h, (size_t)ns, &got)) != MPMB_OK) return rc;
     if (got != counts[d]) return fail(h, MPMB_ERR_STATE, "rank %d: %d rows flagged, %lld counted", d, got, (long long)counts[d]);
-    k_recut_pack<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, ns, h->scan_b.get(), (float4 *)dev_buf + (size_t)off * N_Q);
+    k_recut_pack<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, ns, h->scan_b.get(), (float4 *)dev_buf + (size_t)off * N_Q, state_words(h));
     h->launches += 2;
     off += counts[d];
   }
@@ -4961,6 +5228,7 @@ int mpmb_recut_apply(MpmbHandle h, int32_t tile_z0, int32_t tile_z1, int64_t n_i
     return fail(h, MPMB_ERR_CAPACITY, "%lld particle rows exceed the configured capacity %lld", (long long)need, (long long)h->cap);
   // the engine changes from here on: a thicker slab grows the tile arrays, the rows grow if they must
   if (sl.ntot > h->cap_tiles && (rc = alloc_tile_arrays(h, sl.ntot)) != MPMB_OK) return rc;
+  if (h->rigid_on && h->tile_flag.size() < (size_t)h->cap_tiles) CUDA_TRY(h, h->tile_flag.alloc(h->cap_tiles));   // rewritten by every ordering
   if (need > 0 && (rc = grow_keeping_rows(h, need, ns)) != MPMB_OK) return rc;
   set_slicing(h, sl);
   h->cfg.tile_z0 = tile_z0;
@@ -4972,7 +5240,7 @@ int mpmb_recut_apply(MpmbHandle h, int32_t tile_z0, int32_t tile_z1, int64_t n_i
     }
     h->cur ^= 1;
     if (n_in > 0) {
-      k_recut_unpack<<<(unsigned)((n_in + 127) / 128), 128, 0, h->stream>>>(make_view(h), h->P, (int)n_in, kept, (const float4 *)dev_records);
+      k_recut_unpack<<<(unsigned)((n_in + 127) / 128), 128, 0, h->stream>>>(make_view(h), h->P, (int)n_in, kept, (const float4 *)dev_records, state_words(h));
       h->launches++;
     }
   }

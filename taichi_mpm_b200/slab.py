@@ -8,6 +8,9 @@ this module only moves two kinds of device buffers between ring neighbours:
                     unpacked by the neighbour as ghost tiles before resample;
   after resample  : particles that left the slab through a face, appended by the neighbour.
 
+With rigid coupling every rank also takes part in two all-gathers per substep: after each transfer the ranks' partial sums
+of the bodies' impulses (engine.rigid_impulse_bytes() each), which every engine sums in rank order and applies.
+
 Messages have a fixed size agreed at start-up (engine.halo_bytes()/migrate_bytes()), so the host
 never waits for a device-side count.  No collective is on the data path: point-to-point only.
 """
@@ -95,6 +98,21 @@ class EngineAdapter:
     def migrate_unpack(self, face, buf):
         self.e.migrate_unpack(face, buf.data_ptr())
 
+    def share_id_end(self, dist):
+        share_id_end(self.e, dist)
+
+    def rigid_on(self):
+        return self.e.rigid_impulse_bytes() > 0 and getattr(self.e, "rigid_coupled", False)
+
+    def rigid_impulse_bytes(self):
+        return self.e.rigid_impulse_bytes()
+
+    def rigid_impulse_pack(self, buf):
+        self.e.rigid_impulse_pack(buf.data_ptr())
+
+    def rigid_impulse_apply(self, buf):
+        self.e.rigid_impulse_apply(buf.data_ptr())
+
 
 class SlabRunner:
     """Runs substeps of one slab and exchanges with the ring neighbours (rank-1 below, rank+1 above)."""
@@ -119,6 +137,21 @@ class SlabRunner:
         self.mig_send = [mk(mb), mk(mb)]
         self.mig_recv = [mk(mb), mk(mb)]
         self.bytes_sent = 0
+        self.device = device
+        self.rig_send = self.rig_all = None   # impulse all-gather buffers, allocated at the first rigid-coupled substep
+        if dist is not None and world > 1 and hasattr(adapter, "share_id_end"):
+            adapter.share_id_end(dist)        # every id of the run has a colour entry on every rank
+
+    def _reduce_impulses(self):
+        """After a whole transfer: every rank's partial impulse sums to every rank (all-gather), summed in rank order."""
+        torch, a = self.torch, self.a
+        if self.rig_send is None:
+            n = a.rigid_impulse_bytes()
+            self.rig_send = torch.empty(n, dtype=torch.uint8, device=self.device)
+            self.rig_all = torch.empty(n * self.world, dtype=torch.uint8, device=self.device)
+        a.rigid_impulse_pack(self.rig_send)
+        self.dist.all_gather(list(self.rig_all.chunk(self.world)), self.rig_send, group=self.group)   # rank r's block r
+        a.rigid_impulse_apply(self.rig_all)
 
     def _exchange(self, send, recv, wait=True):
         """send[0] -> rank-1, send[1] -> rank+1 ; recv[0] <- rank-1, recv[1] <- rank+1.
@@ -143,6 +176,7 @@ class SlabRunner:
 
     def substep(self, n=1):
         a = self.a
+        rigid = self.world > 1 and hasattr(a, "rigid_on") and a.rigid_on()
         for _ in range(n):
             a.sort()
             if self.world == 1:
@@ -159,6 +193,8 @@ class SlabRunner:
                     a.halo_pack(1, self.halo_send[1])
                 works = self._exchange(self.halo_send, self.halo_recv, wait=False)
                 a.rasterize_part(2)
+                if rigid:
+                    self._reduce_impulses()
                 a.resample_part(2)
                 for w in works:
                     w.wait()
@@ -167,8 +203,12 @@ class SlabRunner:
                 if self.has_hi:
                     a.halo_unpack(1, self.halo_recv[1])
                 a.resample_part(1)
+                if rigid:
+                    self._reduce_impulses()
             else:
                 a.rasterize()
+                if rigid:
+                    self._reduce_impulses()
                 if self.has_lo:
                     a.halo_pack(0, self.halo_send[0])
                 if self.has_hi:
@@ -179,6 +219,8 @@ class SlabRunner:
                 if self.has_hi:
                     a.halo_unpack(1, self.halo_recv[1])
                 a.resample()
+                if rigid:
+                    self._reduce_impulses()
             if self.world > 1:
                 if self.has_lo:
                     a.migrate_pack(0, self.mig_send[0])
@@ -225,6 +267,16 @@ def global_id_end(engine, dist=None):
     return _on_all_ranks(engine.id_end, dist, "MAX")
 
 
+def share_id_end(engine, dist=None):
+    """Raises this rank's id end to the run's (global_id_end) and returns it.  A z-slab rank with rigid coupling keeps the
+    particles' colour states by absolute id below its id end, and an immigrant may carry any id of the run: after per-rank
+    uploads (set_id_base + upload, seed_lattice) every rank must know the run's id end.  connect_peers and SlabRunner call it."""
+    end = global_id_end(engine, dist)
+    z3, z1 = np.zeros((0, 3), np.float32), np.zeros(0, np.float32)
+    engine.append_owned(z3, z3, z1, z1, first_id=end)   # no particle: only the id end moves
+    return end
+
+
 def append_particles(engine, batch, first_id, dist=None):
     """Adds a batch of particles to a z-slab run (or to one engine with dist=None) between substeps, keeping every resident
     particle's id and state.  Every rank passes the SAME batch (dict x, v, mass, vol and optionally F, b, ps, group) and the
@@ -244,12 +296,17 @@ def delete_inside_levelset(engine, dist=None):
 
 
 def connect_peers(engine, rank, world, dist):
-    """Maps the ring neighbours' receive buffers into `engine` with CUDA IPC (one process per GPU):
-    afterwards engine.substep(n) runs whole z-slab substeps, halo and migration included, with no
-    host transport.  Handles travel through torch.distributed once."""
+    """Maps the ring neighbours' receive buffers and every rank's rigid impulse mailbox into `engine` with CUDA IPC (one
+    process per GPU): afterwards engine.substep(n) runs whole z-slab substeps, halo, migration and the rigid impulse
+    reductions included, with no host transport.  Handles travel through torch.distributed once."""
+    share_id_end(engine, dist)
     mine = {(k, f): engine.xchg_ipc_handle(k, f) for k in (0, 1) for f in (0, 1)}
+    mine["rigid"] = engine.rigid_mailbox_ipc_handle()
     everyone = [None] * world
     dist.all_gather_object(everyone, mine)
+    for r in range(world):   # the rigid impulse mailboxes: every rank's, for the reductions of rigid-coupled substeps
+        if r != rank:
+            engine.rigid_connect(r, handle=everyone[r]["rigid"])
     for k in (0, 1):
         if rank > 0:
             engine.xchg_connect(k, 0, handle=everyone[rank - 1][(k, 1)])   # my face 0 -> lower neighbour's face-1 buffer
