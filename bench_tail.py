@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench_tail.py — how long the CTAs of k_p2g, k_grid and k_g2p sit idle while the slowest CTA of a launch finishes.
+"""bench_tail.py — how long the CTAs of k_p2g and k_g2p sit idle while the slowest CTA of a launch finishes.
 
     python -m taichi_mpm_b200.build --define MPMB_TILE_TRACE --out build_variants/libmpmb_tile_trace.so
     python bench_tail.py [--lib build_variants/libmpmb_tile_trace.so] [--substeps 10] [--out FILE]
 
 Runs bench.py's flagship scene (sand256, seeded on the device the same way) on one GPU with a library built with
--DMPMB_TILE_TRACE, where every CTA of the three tile kernels records its start and end (%globaltimer), its SM and the
+-DMPMB_TILE_TRACE, where every CTA of the two tile kernels records its start and end (%globaltimer), its SM and the
 tiles and particle rows it processed.  Two states, as bench.py times them: the column at rest (after the 20 warm-up
 substeps) and the developed collapse (after the 20 + 2 * 200 + 20000 + 20 substeps that precede bench.py's flowing
 timed region).  In each state `--substeps` single substeps are traced and, per kernel, averaged:
@@ -29,7 +29,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-KERNELS = ("k_p2g", "k_grid", "k_g2p")
+KERNELS = ("k_p2g", "k_g2p")  # index = the `which` of mpmb_debug_tile_trace
 TRACE = np.dtype([("t0", "<u8"), ("t1", "<u8"), ("sm", "<i4"), ("tiles", "<i4"), ("rows", "<i4"), ("pad", "<i4")])
 
 

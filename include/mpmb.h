@@ -414,7 +414,7 @@ int mpmb_async_download(MpmbHandle h, int32_t which, int64_t cap, int64_t *n_out
                         float *b, float *mass, float *vol, float *scalar, int32_t *group);
 
 /* ------------------------------------------------------------------------------ profiling */
-#define MPMB_N_STAGES 5 /* 0 sort+tiles, 1 P2G, 2 G2P, 3 exchange pack/unpack, 4 grid update */
+#define MPMB_N_STAGES 5 /* 0 sort+tiles, 1 P2G, 2 G2P (with the grid update), 3 exchange pack/unpack, 4 unused: 0 */
 /* When enabled, CUDA events bracket every stage on the engine's stream.                          */
 int mpmb_set_profiling(MpmbHandle h, int32_t enabled);
 /* Accumulated milliseconds and launch counts per stage since the last reset (synchronises).      */

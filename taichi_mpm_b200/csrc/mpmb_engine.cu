@@ -17,7 +17,7 @@
 //     array: run rows are read with unit stride.  The radix sort runs once, at upload.
 //     This replaces sort_particles_and_populate_grid (src/mpm.cpp:770-918).
 //   * grid: no dense grid.  P2G leaves one 6x6x6 float4 "arena" (tile + the +2 stencil halo,
-//     the reference's GridCache footprint src/transfer.cpp:59-63) per active tile; k_grid rebuilds
+//     the reference's GridCache footprint src/transfer.cpp:59-63) per active tile; G2P rebuilds
 //     each node as the fixed-order sum of the <=8 arenas covering it, normalises and applies the
 //     level-set boundary.  No global float atomics, no float atomics at all: single-GPU results
 //     are bit-reproducible run to run.
@@ -94,13 +94,13 @@ struct Counters {  // device-resident
 #endif
 enum { DEVERR_TILE_CAPACITY = 1, DEVERR_MIGRATE_CAPACITY = 2, DEVERR_PARTICLE_CAPACITY = 4, DEVERR_PEER_TIMEOUT = 8, DEVERR_BAD_INPUT = 16 };
 
-// Tile-scheduling trace (-DMPMB_TILE_TRACE, read by bench_tail.py through mpmb_debug_tile_trace): every CTA of k_p2g,
-// k_grid and k_g2p records when it started and ended (%globaltimer, ns), its SM and the tiles and particle rows it
+// Tile-scheduling trace (-DMPMB_TILE_TRACE, read by bench_tail.py through mpmb_debug_tile_trace): every CTA of k_p2g
+// and k_g2p records when it started and ended (%globaltimer, ns), its SM and the tiles and particle rows it
 // processed.  Each kernel keeps the records of its last launch.
 #ifdef MPMB_TILE_TRACE
 struct CtaTrace { unsigned long long t0, t1; int sm, tiles, rows, pad; };
-enum { TRACE_P2G = 0, TRACE_GRID = 1, TRACE_G2P = 2, TRACE_CTAS = 4096 };
-__device__ CtaTrace g_trace[3][TRACE_CTAS];
+enum { TRACE_P2G = 0, TRACE_G2P = 1, TRACE_CTAS = 4096 };
+__device__ CtaTrace g_trace[2][TRACE_CTAS];
 #ifndef MPMB_SIMT_HOST
 __device__ __forceinline__ unsigned long long trace_clock() {
   unsigned long long t;
@@ -132,7 +132,7 @@ struct TileMeta {  // one 32-byte record per active tile (slot)
 // TileMeta::pad0/pad1 carry the tile's (x | y<<16, z) coordinates, decoded once per tile by k_order_c, so the tile
 // kernels skip two runtime integer divisions per CTA per tile/chunk.
 // Alternatives tried and dropped: a 192-thread x-plane P2G (more instructions and three times the row reads) and per-tile
-// level-set flags for k_grid (the band test is not its limiter).
+// level-set flags for the grid update (the band test is not its limiter).
 
 struct View {  // raw pointers handed to kernels
   float4 *q[N_Q];        // current (read) buffer
@@ -1132,9 +1132,17 @@ __device__ __forceinline__ float4 gather_node(const float4 *arena, int zero_slot
   return acc;
 }
 
+// the level set at node (gx, gy, gz), or nothing to project on (no level set, or a node past the grid)
+__device__ __forceinline__ bool node_sdf(const Params &P, const float4 *sdf4, int gx, int gy, int gz, float4 &s) {
+  s = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (!(P.has_sdf && gx < P.nnode[0] && gy < P.nnode[1] && gz < P.nnode[2])) return false;
+  s = sdf4[((size_t)gx * P.nnode[1] + gy) * P.nnode[2] + gz];
+  return true;
+}
+
 // normalize_grid_and_apply_external_force (src/mpm.cpp:277-294) + apply_grid_boundary_conditions
-// (src/mpm.cpp:296-372, static level set) for one node.
-__device__ __forceinline__ float4 node_update(const Params &P, const float4 *sdf4, float4 g, int gx, int gy, int gz, bool use_sdf = true) {
+// (src/mpm.cpp:296-372, static level set) for one node; has_s / s: node_sdf of the node.
+__device__ __forceinline__ float4 node_update(const Params &P, float4 g, bool has_s, float4 s) {
   float m = g.w;
   if (m > 0.f) {
     float inv = 1.0f / m;
@@ -1143,8 +1151,7 @@ __device__ __forceinline__ float4 node_update(const Params &P, const float4 *sdf
     g.y = fmaf(g.y, inv, iy);
     g.z = fmaf(g.z, inv, iz);
   }
-  if (P.has_sdf && use_sdf && m != 0.f && gx < P.nnode[0] && gy < P.nnode[1] && gz < P.nnode[2]) {
-    float4 s = sdf4[((size_t)gx * P.nnode[1] + gy) * P.nnode[2] + gz];
+  if (has_s && m != 0.f) {
     if (!(s.w < -3.0f || 0.0f < s.w)) {
       float3 v = friction_project0(make_float3(g.x, g.y, g.z), make_float3(s.x, s.y, s.z), P.friction);
       g.x = v.x; g.y = v.y; g.z = v.z;
@@ -1155,60 +1162,43 @@ __device__ __forceinline__ float4 node_update(const Params &P, const float4 *sdf
 
 // ------------------------------------------------------------------------------ grid update
 // Replaces normalize_grid_and_apply_external_force (src/mpm.cpp:277-294) + apply_grid_boundary_conditions
-// (src/mpm.cpp:296-372): for every active tile the 6x6x6 nodes its particles gather from are
-// rebuilt (fixed-order sum of the covering arenas), normalised, projected on the level set and
-// stored as one contiguous 3.4 KB block vel[slot][216].  Node-parallel, so the dependent
-// slot_map -> arena -> sdf loads are hidden by occupancy instead of stalling a G2P CTA.
-// launch bound (256, 1): 64 registers; capping at 40 / 32 registers for 6 / 8 CTAs per SM spills
-__global__ void __launch_bounds__(256, 1) k_grid(View V, Params P, float4 *vel, int part) {
-  // one WARP per tile: the 27 neighbour slots live in lanes 0..26 and are fetched with shuffles, so
-  // there is no block barrier and every warp of the grid has its own tile in flight
-  const int lane = threadIdx.x & 31;
-  const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
-  const int n_tiles = V.cnt->n_tiles;
-  MPMB_TRACE_BEGIN;
-#ifdef MPMB_TILE_TRACE
-  __shared__ int s_trace[2];  // tiles and rows of the CTA's warps
-  if (threadIdx.x == 0) s_trace[0] = s_trace[1] = 0;
-  __syncthreads();
-#endif
-  for (int slot = gw; slot < n_tiles; slot += nw) {
-    const TileMeta tmg = V.meta[slot];
-    const int tile = tmg.tile;
-    if (!tile_in_part(P, tile, part)) continue;  // uniform per warp
-    MPMB_TRACE_TILE(tmg.run_len + tmg.arr_len);
-    MPMB_TILE_XYZ(P, tmg, tx, ty, tz);
-    int my_nb = -1;
-    if (lane < 27) {
-      int ox = lane / 9 - 1, oy = (lane / 3) % 3 - 1, oz = lane % 3 - 1;
-      int x = tx + ox, y = ty + oy, z = tz + oz - P.tz_off;  // z: local layer
-      if (x >= 0 && y >= 0 && z >= 0 && x < P.nt[0] && y < P.nt[1] && z < P.nt[2]) my_nb = V.slot_map[(x * P.nt[1] + y) * P.nt[2] + z];
-      if (!MPMB_CHK(V.cnt, my_nb >= -1 && my_nb < V.cap_tiles, 5, slot, my_nb, lane)) my_nb = -1;
-    }
-#pragma unroll 2
-    for (int n0 = 0; n0 < ARENA; n0 += 32) {
-      const int n = min(n0 + lane, ARENA - 1);  // the last pass is partial: clamp, store guarded
-      int a = n / 36, b = (n / 6) % 6, c = n % 6;
-      int wx_ = a >> 2, wy_ = b >> 2, wz_ = c >> 2;  // owner tile offset (0/1)
-      int lx = a & 3, ly = b & 3, lz = c & 3;
-      int sl[8];
+// (src/mpm.cpp:296-372) for the nodes one tile's particles gather from.  Every arena is final once k_p2g (and, on a
+// z-slab rank, the halo exchange) has run, so the G2P kernels build each tile's block themselves, in shared memory,
+// instead of reading it back from a node array that a separate grid pass wrote.
+
+// slot of the neighbour tile k (= (ox+1)*9 + (oy+1)*3 + (oz+1), o in {-1,0,1}^3) of tile (tx, ty, tz); -1: none
+__device__ __forceinline__ int neighbour_slot(const View &V, const Params &P, int slot, int tx, int ty, int tz, int k) {
+  const int x = tx + k / 9 - 1, y = ty + (k / 3) % 3 - 1, z = tz + k % 3 - 1 - P.tz_off;  // z: local layer
+  int nb = -1;
+  if (x >= 0 && y >= 0 && z >= 0 && x < P.nt[0] && y < P.nt[1] && z < P.nt[2]) nb = V.slot_map[(x * P.nt[1] + y) * P.nt[2] + z];
+  if (!MPMB_CHK(V.cnt, nb >= -1 && nb < V.cap_tiles, 5, slot, nb, k)) nb = -1;
+  return nb;
+}
+
+// The 6x6x6 nodes of tile (tx, ty, tz), each the fixed-order sum of the arenas that cover it (nb: the tile's 27
+// neighbour slots), normalised and projected on the level set, into s_vel; the CTA's BLOCK threads share the nodes.
+// The caller puts a block barrier between this and the first read of s_vel.  Every global load of a thread's nodes
+// (arenas and level set) is issued before its first store to s_vel, which the compiler cannot move loads across: the
+// build costs one round trip to L2 / HBM, not two per node with the nodes one after the other.
+template <int BLOCK>
+__device__ __forceinline__ void build_node_block(const View &V, const Params &P, int tx, int ty, int tz, const int *nb, float4 *s_vel) {
+  constexpr int NPT = (ARENA + BLOCK - 1) / BLOCK;  // nodes per thread
+  float4 g[NPT], s[NPT];
+  bool has_s[NPT];
 #pragma unroll
-      for (int o = 0; o < 8; o++) {
-        const int ox = o >> 2, oy = (o >> 1) & 1, oz = o & 1;
-        sl[o] = __shfl_sync(0xffffffffu, my_nb, (wx_ - ox + 1) * 9 + (wy_ - oy + 1) * 3 + (wz_ - oz + 1));
-      }
-      float4 g = gather_node(V.arena, V.cap_tiles, lx, ly, lz, [&](int ox, int oy, int oz) { return sl[ox * 4 + oy * 2 + oz]; });
-      g = node_update(P, V.sdf4, g, tx * 4 + a, ty * 4 + b, tz * 4 + c);
-      if (n0 + lane < ARENA) vel[(size_t)slot * ARENA + n] = g;
-    }
+  for (int k = 0; k < NPT; k++) {
+    const int n = min(k * BLOCK + (int)threadIdx.x, ARENA - 1);  // the last pass is partial: clamp, store guarded
+    const int a = n / 36, b = (n / 6) % 6, c = n % 6;
+    const int wx_ = a >> 2, wy_ = b >> 2, wz_ = c >> 2;  // owner tile offset (0/1)
+    g[k] = gather_node(V.arena, V.cap_tiles, a & 3, b & 3, c & 3,
+                       [&](int ox, int oy, int oz) { return nb[(wx_ - ox + 1) * 9 + (wy_ - oy + 1) * 3 + (wz_ - oz + 1)]; });
+    has_s[k] = node_sdf(P, V.sdf4, tx * 4 + a, ty * 4 + b, tz * 4 + c, s[k]);
   }
-#ifdef MPMB_TILE_TRACE
-  if (lane == 0) { atomicAdd(&s_trace[0], trace_tiles); atomicAdd(&s_trace[1], trace_rows); }
-  __syncthreads();
-  trace_tiles = s_trace[0];
-  trace_rows = s_trace[1];
-#endif
-  MPMB_TRACE_END(TRACE_GRID);
+#pragma unroll
+  for (int k = 0; k < NPT; k++) {
+    const int n = k * BLOCK + (int)threadIdx.x;
+    if (n < ARENA) s_vel[n] = node_update(P, g[k], has_s[k], s[k]);
+  }
 }
 
 // ------------------------------------------------------------------------------ G2P
@@ -1217,16 +1207,21 @@ __global__ void __launch_bounds__(256, 1) k_grid(View V, Params P, float4 *vel, 
 // (calculate_force of the updated state), writes the tile's particles cell-sorted into one contiguous
 // run of the other buffer, and appends the particles whose base node left the tile to the mover list.
 // Persistent CTAs walk their tiles chunk by chunk through a two-stage cp.async pipeline: while the
-// warps compute chunk i out of one shared buffer, the rows (64 B/particle) of chunk i+1 and, at a
-// tile change, that tile's 216 node velocities are already in flight into the other.
+// warps compute chunk i out of one shared buffer, the rows (64 B/particle) of chunk i+1 are already
+// in flight into the other.  At the first chunk of a tile the CTA builds the tile's 216 node
+// velocities from the arenas (build_node_block) while that chunk's successor is in flight.
 constexpr int G2P_CH = 256;  // rows per pipeline stage
 // STORE_B = false skips the apic_b streams (48 B/particle): no kernel reads apic_b — rasterize uses the
 // affine matrix A — so inside mpmb_substep(h, n) only the LAST substep has to leave it behind for the
 // host (downloads, visualize, save).
 // EXT_MATS = false leaves the elastic / von Mises / visco branches of material_step out (see mpmb_math.cuh).
 template <int BLOCK, bool STORE_B, bool EXT_MATS>
-__global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4 *vel, int part, int commit) {
-  __shared__ __align__(16) float4 s_vel[2][ARENA];
+__global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, int part, int commit) {
+  // node block of the current tile: written at its first chunk, after the previous tile's last end-of-chunk barrier
+  __shared__ __align__(16) float4 s_vel[ARENA];
+  // the 27 neighbour slots of the current tile [sp] and of the tile claimed ahead [sp ^ 1], loaded one tile ahead so
+  // that the build's first loads are the arenas'
+  __shared__ int s_nb[2][27];
   __shared__ __align__(16) float4 s_in[2][4][G2P_CH];
   // output row of every staged row: run rows at [sh + r] (sh = 16-byte alignment shift of the run's outpos words),
   // arrival rows at [r + 8] — clear of the up to 3 words by which the bulk copy of the run part is rounded up
@@ -1274,11 +1269,10 @@ __global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4
   // rows of the chunk that lie inside the tile's run (unit stride in storage) / alignment shift of their outpos words
   auto run_rows = [&](const Item &it) { return max(0, min(G2P_CH, it.tm.run_len - it.rb)); };
   auto out_shift = [&](const Item &it) { return run_rows(it) > 0 ? (int)((uint32_t)(it.tm.run_begin + it.rb) & 3u) : 0; };
-  // puts one item in flight: rows of the G2P set (x|mass, F, scalar|vol|tag), their output rows and, for the first
-  // chunk of a tile, the tile's node velocities.  The run part of the chunk and the node block are TMA bulk copies
-  // issued by thread 0 and tracked by the stage's mbarrier; the (few) arrival rows are gathered with 16-byte
-  // LDGSTS copies by the thread that will consume them, tracked by its own copy groups.
-  auto prefetch = [&](const Item &it, int buf, int vbuf) {
+  // puts one item in flight: rows of the G2P set (x|mass, F, scalar|vol|tag) and their output rows.  The run part of
+  // the chunk is TMA bulk copies issued by thread 0 and tracked by the stage's mbarrier; the (few) arrival rows are
+  // gathered with 16-byte LDGSTS copies by the thread that will consume them, tracked by its own copy groups.
+  auto prefetch = [&](const Item &it, int buf) {
     if (it.slot < n_tiles) {
       const int nrow_tile = it.tm.run_len + it.tm.arr_len;
       const int nrows = min(G2P_CH, nrow_tile - it.rb);
@@ -1287,7 +1281,7 @@ __global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4
       if (tid == 0) {
         const uint32_t r0 = (uint32_t)(it.tm.run_begin + it.rb);
         const unsigned row_bytes = (unsigned)nrun * 16u, out_bytes = nrun > 0 ? (((unsigned)(sh + nrun) * 4u + 15u) & ~15u) : 0u;
-        mbar_arrive_expect_tx(&s_bar[buf], 4u * row_bytes + out_bytes + (it.first ? (unsigned)(ARENA * sizeof(float4)) : 0u));
+        mbar_arrive_expect_tx(&s_bar[buf], 4u * row_bytes + out_bytes);
         if (nrun > 0) {
           bulk_g2s(&s_in[buf][0][0], &V.q[0][r0], row_bytes, &s_bar[buf]);
           bulk_g2s(&s_in[buf][1][0], &V.q[4][r0], row_bytes, &s_bar[buf]);
@@ -1295,7 +1289,6 @@ __global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4
           bulk_g2s(&s_in[buf][3][0], &V.q[6][r0], row_bytes, &s_bar[buf]);
           bulk_g2s(&s_out[buf][0], &V.outpos[r0 - (uint32_t)sh], out_bytes, &s_bar[buf]);
         }
-        if (it.first) bulk_g2s(&s_vel[vbuf][0], vel + (size_t)it.slot * ARENA, (unsigned)(ARENA * sizeof(float4)), &s_bar[buf]);
       }
       if (nrun < nrows) {
 #pragma unroll
@@ -1327,15 +1320,22 @@ __global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4
   }
   __syncthreads();
   Item cur = first_item(s_ahead[0]);
+  if (tid < 27 && cur.slot < n_tiles) s_nb[0][tid] = neighbour_slot(V, P, cur.slot, cur.tm.xy & 0xffff, cur.tm.xy >> 16, cur.tm.z, tid);
   __syncthreads();  // s_ahead[0] is claimed into again at the first tile change
-  int buf = 0, vbuf = 0;
+  int buf = 0;
   unsigned phase = 0;  // bit b = parity of the phase stage b's barrier is in
-  prefetch(cur, 0, 0);
+  prefetch(cur, 0);
   while (cur.slot < n_tiles) {
     const Item nxt = next_item(cur);
-    const int nvbuf = nxt.first ? (vbuf ^ 1) : vbuf;
-    prefetch(nxt, buf ^ 1, nvbuf);
-    if (tid == 0 && nxt.first && nxt.slot < n_tiles) s_ahead[sp] = claim(next_claim());  // nxt took the tile claimed ahead
+    prefetch(nxt, buf ^ 1);
+    if (nxt.first && nxt.slot < n_tiles) {  // nxt took the tile claimed ahead
+      if (tid == 0) s_ahead[sp] = claim(next_claim());
+      if (tid < 27) s_nb[sp ^ 1][tid] = neighbour_slot(V, P, nxt.slot, nxt.tm.xy & 0xffff, nxt.tm.xy >> 16, nxt.tm.z, tid);
+    }
+    if (cur.first) {  // the previous tile's last end-of-chunk barrier has retired every read of s_vel
+      build_node_block<BLOCK>(V, P, cur.tm.xy & 0xffff, cur.tm.xy >> 16, cur.tm.z, s_nb[sp], s_vel);
+      __syncthreads();
+    }
     asm volatile("cp.async.wait_group 1;\n" ::: "memory");  // my arrival rows of the current item have landed; the next item stays in flight
     mbar_wait(&s_bar[buf], (phase >> buf) & 1u);              // ... and so have its bulk copies (every thread reads only rows it waited for)
     phase ^= 1u << buf;
@@ -1344,7 +1344,7 @@ __global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4
       const int sh = out_shift(cur), nrun = run_rows(cur);
       MPMB_TILE_XYZ(P, cur.tm, tx, ty, tz);
       const int nrows = min(G2P_CH, cur.tm.run_len + cur.tm.arr_len - cur.rb);
-      const float4 *sv = s_vel[vbuf];
+      const float4 *sv = s_vel;
       int my_stay = 0;
       for (int r = tid; r < nrows; r += BLOCK) {
         const float4 q0 = s_in[buf][0][r];
@@ -1438,7 +1438,6 @@ __global__ void __launch_bounds__(BLOCK, 5) k_g2p(View V, Params P, const float4
     }
     cur = nxt;
     buf ^= 1;
-    vbuf = nvbuf;
   }
   cp_async_wait_all();
   MPMB_TRACE_END(TRACE_G2P);
@@ -2042,8 +2041,9 @@ __global__ void k_rigid_advance(RigidView R, MotionView M, Params P, float3 grav
 // block_op_rigid of resample_optimized (src/transfer.cpp:706-835) + what k_g2p does for the ordering (output rows, keys,
 // movers, stay counts), for the tiles of rigid pages.  Launched BEFORE k_g2p, which commits the substep.  Owned tiles of
 // `part` only, as k_p2g_rigid.
-__global__ void __launch_bounds__(128) k_g2p_rigid(View V, Params P, RigidView R, const float4 *vel, int part) {
+__global__ void __launch_bounds__(128) k_g2p_rigid(View V, Params P, RigidView R, int part) {
   __shared__ float4 s_vel[ARENA];
+  __shared__ int s_nb[27];
   __shared__ uint32_t s_word[ARENA];
   __shared__ float s_acc[RIGID_MAX][6];
   __shared__ int s_stay;
@@ -2057,7 +2057,9 @@ __global__ void __launch_bounds__(128) k_g2p_rigid(View V, Params P, RigidView R
     const int tile = tm.tile;
     if (!tile_in_part(P, tile, part)) continue;
     MPMB_TILE_XYZ(P, tm, tx, ty, tz);
-    for (int n = tid; n < ARENA; n += blockDim.x) s_vel[n] = vel[(size_t)slot * ARENA + n];
+    if (tid < 27) s_nb[tid] = neighbour_slot(V, P, slot, tx, ty, tz, tid);
+    __syncthreads();
+    build_node_block<128>(V, P, tx, ty, tz, s_nb, s_vel);
     for (int n = tid; n < RIGID_MAX * 6; n += blockDim.x) (&s_acc[0][0])[n] = 0.f;
     load_tile_words(R, P, tx, ty, tz, s_word);
     if (tid == 0) s_stay = 0;
@@ -2182,7 +2184,11 @@ __global__ void k_dense_grid(View V, Params P, int which, float4 *dense) {
       if (x < 0 || y < 0 || z < 0 || x >= P.nt[0] || y >= P.nt[1] || z >= P.nt[2]) return -1;
       return V.slot_map[(x * P.nt[1] + y) * P.nt[2] + z];
     });
-    if (which == 1) g = node_update(P, V.sdf4, g, gx, gy, gz);
+    if (which == 1) {
+      float4 s;
+      const bool has_s = node_sdf(P, V.sdf4, gx, gy, gz, s);
+      g = node_update(P, g, has_s, s);
+    }
     dense[i] = g;
   }
 }
@@ -2951,7 +2957,6 @@ struct MpmbEngine {
   DevBuf<int> arr_cnt, arr_off, arr_len, arr_cur, slot_map, blocksum;
   DevBuf<TileMeta> meta;
   DevBuf<float4> arena;
-  DevBuf<float4> vel;  // node velocities per active tile (k_grid -> k_g2p)
   DevBuf<float4> sdf4;
   DevBuf<Counters> cnt;
 
@@ -3264,19 +3269,18 @@ static void set_slicing(MpmbEngine *h, const Slicing &s) {
 }
 
 // Dense per-tile arrays, active-tile records, arenas (plus the all-zero arena read for absent neighbours, past the last
-// slot), node velocities and the ordering's block sums for `cap_tiles` tiles.  All or nothing: on failure the engine keeps
+// slot) and the ordering's block sums for `cap_tiles` tiles.  All or nothing: on failure the engine keeps
 // the arrays it had.
 static int alloc_tile_arrays(MpmbEngine *h, int64_t cap_tiles) {
   DevBuf<int> dense[11], blocksum;
   DevBuf<TileMeta> meta;
-  DevBuf<float4> arena, vel;
+  DevBuf<float4> arena;
   const int64_t blocks = (cap_tiles + ORD_TILE - 1) / ORD_TILE;
   bool ok = true;
   for (auto &d : dense) ok = ok && d.alloc(cap_tiles) == cudaSuccess;
   ok = ok && blocksum.alloc(3 * (blocks + 1)) == cudaSuccess;
   ok = ok && meta.alloc(cap_tiles) == cudaSuccess;
   ok = ok && arena.alloc((size_t)ARENA * (cap_tiles + 1)) == cudaSuccess;
-  ok = ok && vel.alloc((size_t)ARENA * cap_tiles) == cudaSuccess;
   if (!ok) return fail(h, MPMB_ERR_CUDA, "cudaMalloc of the tile arrays (%lld tiles): %s", (long long)cap_tiles, cudaGetErrorString(cudaGetLastError()));
   for (auto &d : dense) cudaMemsetAsync(d.get(), 0, sizeof(int) * cap_tiles, h->stream);
   cudaMemsetAsync(arena.get() + (size_t)ARENA * cap_tiles, 0, sizeof(float4) * ARENA, h->stream);
@@ -3284,7 +3288,7 @@ static int alloc_tile_arrays(MpmbEngine *h, int64_t cap_tiles) {
                          &h->arr_cnt, &h->arr_off, &h->arr_len, &h->arr_cur, &h->slot_map};
   for (int k = 0; k < 11; k++) *mine[k] = std::move(dense[k]);
   cudaMemsetAsync(h->slot_map.get(), 0xFF, sizeof(int) * cap_tiles, h->stream);
-  h->blocksum = std::move(blocksum); h->meta = std::move(meta); h->arena = std::move(arena); h->vel = std::move(vel);
+  h->blocksum = std::move(blocksum); h->meta = std::move(meta); h->arena = std::move(arena);
   h->cap_tiles = (int)cap_tiles;
   return MPMB_OK;
 }
@@ -3347,7 +3351,7 @@ int mpmb_create(const MpmbConfig *cfg, MpmbHandle *out) {
   cudaGetDeviceProperties(&prop, cfg->device);
   h->num_sms = prop.multiProcessorCount;
   // MPMB_NUM_SMS=k (tests): size every persistent and grid-stride launch for min(k, SMs) SMs, so that a small scene
-  // still makes each CTA (each k_grid warp) walk many tiles
+  // still makes each CTA walk many tiles
   if (const char *s = getenv("MPMB_NUM_SMS")) { const int k = atoi(s); if (k > 0) h->num_sms = std::min(k, h->num_sms); }
   {
     int occ = 0;
@@ -4438,11 +4442,11 @@ static void launch_g2p(MpmbEngine *h, const View &V, int part, int commit, bool 
   bool ext = false;
   for (int g = 0; g < MPMB_MAX_GROUPS; g++) ext |= h->P.mats[g].kind > MAT_SAND;
   if (ext) {
-    if (store_b) k_g2p<128, true, true><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel.get(), part, commit);
-    else k_g2p<128, false, true><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel.get(), part, commit);
+    if (store_b) k_g2p<128, true, true><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, part, commit);
+    else k_g2p<128, false, true><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, part, commit);
   } else {
-    if (store_b) k_g2p<128, true, false><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel.get(), part, commit);
-    else k_g2p<128, false, false><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, h->vel.get(), part, commit);
+    if (store_b) k_g2p<128, true, false><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, part, commit);
+    else k_g2p<128, false, false><<<h->grid_g2p, 128, 0, h->stream>>>(V, h->P, part, commit);
   }
 }
 
@@ -4454,13 +4458,10 @@ int mpmb_resample(MpmbHandle h) {
   if (motion && h->motion_scripted && h->script_left < 1) return fail(h, MPMB_ERR_STATE, "the rigid script has no entry left for this substep");
   const bool slab_rigid = h->rigid_on && h->cfg.world > 1;   // the G2P impulses, then the advance, follow the reduction
   View V = make_view(h);
-  prof_begin(h, 4);
-  if (h->cap > 0) k_grid<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, h->vel.get(), 0);
-  prof_end(h, 1);
   prof_begin(h, 2);
   if (h->cap > 0) {
     if (h->rigid_on) {
-      k_g2p_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h), h->vel.get(), 0);
+      k_g2p_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h), 0);
       h->launches += 1;
     }
     launch_g2p(h, V, 0, 1, !h->skip_b || h->rigid_on);   // rigid tiles read apic_b back (the impulse needs dt * force)
@@ -4471,7 +4472,7 @@ int mpmb_resample(MpmbHandle h) {
   }
   if (motion && !slab_rigid) launch_rigid_motion(h);     // advect_rigid_bodies (src/mpm_rigid_body.cpp:273-287)
   if (slab_rigid) h->rigid_pending = 2;
-  h->launches += 2;
+  h->launches += 1;
   prof_end(h, 1);
   CUDA_TRY(h, cudaGetLastError());
   h->cur ^= 1;  // the buffer G2P wrote is the current storage ...
@@ -4525,11 +4526,10 @@ int mpmb_resample_part(MpmbHandle h, int32_t part) {
     return fail(h, MPMB_ERR_STATE, "the rigid script has no entry left for this substep");
   prof_begin(h, 2);
   View V = make_view(h);
-  int nl = 2;
+  int nl = 1;
   if (h->cap > 0) {
-    k_grid<<<h->num_sms * 8, 256, 0, h->stream>>>(V, h->P, h->vel.get(), part);
     if (slab_rigid) {
-      k_g2p_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h), h->vel.get(), part);
+      k_g2p_rigid<<<h->num_sms * 4, 128, 0, h->stream>>>(V, h->P, rigid_view(h), part);
       nl++;
     }
     launch_g2p(h, V, part, part == 1 ? 1 : 0, true);
@@ -4694,13 +4694,13 @@ extern "C" int mpmb_debug_rows(MpmbHandle h, int n, uint32_t *keys, float *mass4
 }
 #endif  // MPMB_DEBUG_EXPORTS
 #ifdef MPMB_TILE_TRACE
-// the per-CTA records of the last launch of kernel `which` (TRACE_P2G / TRACE_GRID / TRACE_G2P) as 32-byte
+// the per-CTA records of the last launch of kernel `which` (TRACE_P2G / TRACE_G2P) as 32-byte
 // {t0, t1, sm, tiles, rows, -}; returns the launch's CTA count (records copied: at most cap)
 extern "C" int mpmb_debug_tile_trace(MpmbHandle h, int which, void *out, int cap) {
   CHECK_HANDLE(h);
-  if (which < 0 || which > 2) return fail(h, MPMB_ERR_INVALID, "which must be 0 (k_p2g), 1 (k_grid) or 2 (k_g2p)");
+  if (which < 0 || which > 1) return fail(h, MPMB_ERR_INVALID, "which must be 0 (k_p2g) or 1 (k_g2p)");
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  const int ctas = which == TRACE_P2G ? h->grid_p2g : which == TRACE_GRID ? h->num_sms * 8 : h->grid_g2p;
+  const int ctas = which == TRACE_P2G ? h->grid_p2g : h->grid_g2p;
   const int n = std::min(std::min(ctas, cap), (int)TRACE_CTAS);
   CUDA_TRY(h, cudaMemcpyFromSymbol(out, g_trace, sizeof(CtaTrace) * n, sizeof(CtaTrace) * TRACE_CTAS * which));
   return ctas;
