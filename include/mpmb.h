@@ -39,7 +39,8 @@ typedef enum MpmbStatus {
   MPMB_ERR_INVALID = -1,   /* bad argument */
   MPMB_ERR_CUDA = -2,      /* a CUDA call failed (sticky per handle) */
   MPMB_ERR_CAPACITY = -3,  /* particle / tile / exchange-buffer capacity exceeded */
-  MPMB_ERR_STATE = -4      /* call not valid in the current state */
+  MPMB_ERR_STATE = -4,     /* call not valid in the current state */
+  MPMB_ERR_LIMIT = -5      /* AsyncMPM: a block's time-step limit is below one unit (mpmb_async_schedule) */
 } MpmbStatus;
 
 /* Material kinds = the registered particle type names of the reference
@@ -373,7 +374,8 @@ int mpmb_download_cdf(MpmbHandle h, uint32_t *node_states, float *node_distance)
 
 /* ------------------------------------------------------------------------------ AsyncMPM pools */
 /* The particle_pool and backup_pool of the reference's AsyncMPM<3> (src/async/async_mpm.h:85-117), kept on the device so that
- * the block scheduler (host code: levels, neighbour masks, the step loop) moves no particle record across the bus.  A record
+ * the block scheduler (levels, neighbour masks: on the host or with mpmb_async_schedule / mpmb_async_advance_level on the
+ * device; the step loop on the host) moves no particle record across the bus.  A record
  * is x, v, F, b, mass, vol, scalar, group, id and the linear index of its 4x4x8-node scheduler block,
  *   base = int(x * inv_dx - 0.5) (fp32, the HOST's inv_dx), block (base_x >> 2, base_y >> 2, base_z >> 3),
  *   linear (bx * nb1 + by) * nb2 + bz.
@@ -412,6 +414,34 @@ int mpmb_async_size(MpmbHandle h, int64_t *n_pool, int64_t *n_backup);
  * written if it exceeds cap).  Synchronises.                                                                              */
 int mpmb_async_download(MpmbHandle h, int32_t which, int64_t cap, int64_t *n_out, uint32_t *id, int32_t *block, float *x, float *v, float *F,
                         float *b, float *mass, float *vol, float *scalar, int32_t *group);
+/* The block scheduler on the device.  mpmb_async_init sets every block's state: level 1 (a power of two, in units),
+ * local_min 1, particle_t 0 and backup_t 0 (clocks in units).  The two calls below make the decisions of
+ * AsyncMPM::update_dt_limits and AsyncMPM::advance (src/async/async_mpm.cpp:90-373) from that state, so that a scheduler
+ * iteration needs no host work per block.
+ *
+ * update_dt_limits at clock t >= 0.  One pass over the particle pool as mpmb_async_block_limits; then every occupied block
+ * whose level divides t (due) takes
+ *   sdl = int64((strength_mul min_dt) inv_unit),  cdl = int64(((cfl_mul dx) inv_unit) (1 / sqrt(max_v2))),
+ *   tmp = min(cdl, sdl, max_units)
+ * (fp32, every operation rounded on its own; int64() truncates, a NaN or |x| >= 2^63 gives INT64_MIN as on x86) and halves
+ * its level while tmp < level, doubles it while tmp >= 2 level and 2 level divides t.  Aligned empty blocks move the same
+ * way toward the occupied blocks' max level (1 if none is occupied).  *min_level / *max_level receive the min / max level
+ * over all blocks; blocks whose level is not that min set local_min to the least particle_t + level of their in-range
+ * 26 neighbours (2^31 if none).  Fails, with no block state changed:
+ *   MPMB_ERR_INVALID  the pool holds a particle of a type without a limit (linear, jelly) while some occupied block is due;
+ *   MPMB_ERR_LIMIT    some due block has tmp < 1 (a NaN limit included).
+ * max_units outside [1, 2^30], t < 0 or a NULL output: MPMB_ERR_INVALID.                                                  */
+int mpmb_async_schedule(MpmbHandle h, int64_t t, float strength_mul, float cfl_mul, float dx, float inv_unit, int64_t max_units, int32_t *min_level,
+                        int32_t *max_level);
+/* advance(limit) at clock t: every block's flags are built from the block state, then mpmb_async_advance's steps 1-5 run
+ * with dt.  EQUAL: level == limit; SWAP: EQUAL and particle_t == t; SMALLER / LARGER: level < / > limit and an in-range
+ * neighbour has level == limit; CLEAR: LARGER and local_min == t + limit.  After the advance, per block: backup_t = t on
+ * SWAP, particle_t = t + limit on EQUAL, backup_t = t + limit on CLEAR.  *n_gathered as mpmb_async_advance.  limit not a
+ * positive power of two, t < 0, dt not positive and finite or NULL n_gathered: MPMB_ERR_INVALID.  A failed advance leaves
+ * the block clocks as they were.                                                                                            */
+int mpmb_async_advance_level(MpmbHandle h, int64_t t, int32_t limit, float dt, int64_t *n_gathered);
+/* Copies the block state out, nb0 * nb1 * nb2 entries each in linear block order; any pointer may be NULL.  Synchronises. */
+int mpmb_async_block_state(MpmbHandle h, int32_t *level, int64_t *local_min, int64_t *particle_t, int64_t *backup_t);
 
 /* ------------------------------------------------------------------------------ profiling */
 #define MPMB_N_STAGES 5 /* 0 sort+tiles, 1 P2G, 2 G2P (with the grid update), 3 exchange pack/unpack, 4 unused: 0 */

@@ -11,6 +11,12 @@ step() are staged in `pool` / `backup` and move into the engine then.  An engine
 stand-in) gets the same pools as numpy record arrays here, gathered and uploaded per advance: the reference the device pools
 are tested against bit for bit.
 
+An engine that also offers mpmb_async_schedule / mpmb_async_advance_level keeps the block state (level, local_min,
+particle_t, backup_t) too and makes the scheduler's decisions per block on the device, the same decisions bit for bit as the
+numpy code here: update_dt_limits is then one call returning the two level bounds, advance one call returning the gathered
+count, and only the step loop and the clock stay on the host.  The numpy scheduler remains the one for every other engine and
+the reference the device scheduler is tested against.
+
 Citations are lines of src/async/async_mpm.cpp unless a file is named.  What cannot be reproduced bit for bit: the reference
 takes 1/sqrt(max |v|^2) with `_mm_rsqrt_ss` (:78-80), a 12-bit hardware approximation; the exact reciprocal square root is used
 here, which can move a block's CFL limit across an integer — and so its level — only when the limit sits within 2e-4 of one."""
@@ -84,6 +90,8 @@ class AsyncMPM(MPM):
         self.backup = None     # backup_pool
         self._next_id = 0
         self._device_pools = hasattr(self.engine, "async_advance")   # the engine keeps the pools (mpmb_async_*)
+        # ... and the block state with the scheduler's decisions (mpmb_async_schedule / mpmb_async_advance_level)
+        self._device_sched = self._device_pools and hasattr(self.engine, "async_schedule")
         self._on_device = False    # the staged records have moved into the engine's pools (first step)
         self.step_counter = 0
         self._async_updates = 0
@@ -139,7 +147,15 @@ class AsyncMPM(MPM):
             if rec is not None and len(rec["id"]):
                 self.engine.async_add(which, rec)
         self.pool = self.backup = None
+        if self._device_sched:      # mpmb_async_init gave the engine's block state these arrays' initial values
+            self.level = self.local_min = self.particle_t = self.backup_t = None
         self._on_device = True
+
+    def block_state(self, fields=("level", "local_min", "particle_t", "backup_t")):
+        """The scheduler's per-block state as int64 arrays of shape nb (read from the engine if it keeps them)."""
+        if self._device_sched and self._on_device:
+            return self.engine.async_block_state(fields)
+        return {k: getattr(self, k).copy() for k in fields}
 
     def pools(self):
         """(particle_pool, backup_pool) as host record dicts in pool order (read from the device pools if the engine keeps them)."""
@@ -218,6 +234,18 @@ class AsyncMPM(MPM):
     def update_dt_limits(self):
         t = self.current_t_int
         inv_unit = np.float32(1.0) / np.float32(self.unit_delta_t)
+        if self._device_sched:
+            self._pools_to_device()
+            try:
+                self.min_delta_t_int, self.max_delta_t_int = self.engine.async_schedule(
+                    t, np.float32(self.strength_dt_mul), np.float32(self.cfl_dt_mul), np.float32(self.delta_x), inv_unit, self.max_units)
+            except capi.MpmbError as e:
+                if e.code == capi.ERR_INVALID:
+                    raise ValueError("particle type without a time-step limit (jelly / linear return 0: the reference stops, :112-124)") from e
+                if e.code == capi.ERR_LIMIT:
+                    raise RuntimeError("a block's time-step limit is below unit_delta_t (the reference stops here, :115-124)") from e
+                raise
+            return
         nonempty, limits = self._pool_scan(t)
         if nonempty.any():
             due = nonempty & ((t & (self.level - 1)) == 0)                  # :95-96
@@ -293,6 +321,10 @@ class AsyncMPM(MPM):
 
     def advance(self, limit):
         t = self.current_t_int
+        if self._device_sched:
+            self._pools_to_device()
+            self._async_updates += self.engine.async_advance_level(t, limit, float(np.float32(self.unit_delta_t) * np.float32(limit)))
+            return
         lg = int(np.log2(limit))
         smaller = self._smaller.get(lg, np.zeros(self.nb, bool))
         larger = self._larger.get(lg, np.zeros(self.nb, bool))
@@ -424,5 +456,6 @@ class AsyncMPM(MPM):
         ne = np.zeros(self.nb, bool)
         if p is not None and len(p["id"]):
             ne[p["block"][:, 0], p["block"][:, 1], p["block"][:, 2]] = True
+        level = self.block_state(("level",))["level"]
         return dict(pool_entries=0 if p is None else len(p["id"]), update_counter=self._async_updates, current_t_int=self.current_t_int,
-                    min_level=int(self.level[ne].min()) if ne.any() else 0, max_level=int(self.level[ne].max()) if ne.any() else 0)
+                    min_level=int(level[ne].min()) if ne.any() else 0, max_level=int(level[ne].max()) if ne.any() else 0)

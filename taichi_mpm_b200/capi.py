@@ -33,11 +33,13 @@ EXPORTS = [
     "mpmb_get_particle_cdf", "mpmb_download_cdf",
     "mpmb_xchg_buffer", "mpmb_xchg_ipc_handle", "mpmb_xchg_connect", "mpmb_halo_send", "mpmb_halo_recv", "mpmb_migrate_send", "mpmb_migrate_recv",
     "mpmb_async_init", "mpmb_async_add", "mpmb_async_block_limits", "mpmb_async_advance", "mpmb_async_size", "mpmb_async_download",
+    "mpmb_async_schedule", "mpmb_async_advance_level", "mpmb_async_block_state",
     "mpmb_layer_counts", "mpmb_recut_pack", "mpmb_recut_apply",
     "mpmb_rigid_impulse_bytes", "mpmb_rigid_impulse_pack", "mpmb_rigid_impulse_apply", "mpmb_rigid_mailbox", "mpmb_rigid_mailbox_ipc_handle",
     "mpmb_rigid_connect", "mpmb_rigid_send", "mpmb_rigid_recv",
 ]
 ASYNC_SMALLER, ASYNC_EQUAL, ASYNC_LARGER, ASYNC_SWAP, ASYNC_CLEAR = 1, 2, 4, 8, 16   # per-block flags of mpmb_async_advance
+ERR_INVALID, ERR_LIMIT = -1, -5   # MPMB_ERR_INVALID; MPMB_ERR_LIMIT: a due block's time-step limit is below one unit
 RECORD_BYTES = 160   # one particle record of mpmb_recut_pack / mpmb_recut_apply (and of the migration messages)
 
 
@@ -402,6 +404,27 @@ class Engine:
         self._check(self.L.mpmb_async_download(self.h, C.c_int32(which), C.c_int64(n), C.byref(got), *[_ptr(out.get(k)) for k in (
             "id", "block", "x", "v", "F", "b", "mass", "vol", "ps", "group")]))
         return out
+
+    # --- AsyncMPM's block scheduler on the device: block state level / local_min / particle_t / backup_t
+    def async_schedule(self, t, strength_mul, cfl_mul, dx, inv_unit, max_units):
+        """update_dt_limits at clock t (the float32 scalars as the host scheduler rounds them).  Returns (min level, max level)."""
+        lo, hi = C.c_int32(0), C.c_int32(0)
+        self._check(self.L.mpmb_async_schedule(self.h, C.c_int64(int(t)), C.c_float(float(strength_mul)), C.c_float(float(cfl_mul)),
+                                               C.c_float(float(dx)), C.c_float(float(inv_unit)), C.c_int64(int(max_units)), C.byref(lo), C.byref(hi)))
+        return lo.value, hi.value
+
+    def async_advance_level(self, t, limit, dt):
+        """advance(limit) at clock t with the flags built on the device.  Returns the gathered count."""
+        n = C.c_int64(0)
+        self._check(self.L.mpmb_async_advance_level(self.h, C.c_int64(int(t)), C.c_int32(int(limit)), C.c_float(float(dt)), C.byref(n)))
+        return n.value
+
+    def async_block_state(self, fields=("level", "local_min", "particle_t", "backup_t")):
+        """The asked block state arrays, int64 of shape nb."""
+        nb = self._async_nb
+        out = {k: np.empty(nb, np.int32 if k == "level" else np.int64) for k in fields}
+        self._check(self.L.mpmb_async_block_state(self.h, *[_ptr(out.get(k)) for k in ("level", "local_min", "particle_t", "backup_t")]))
+        return {k: v.astype(np.int64) for k, v in out.items()}
 
     # --- hot path
     def substep(self, nsub=1):

@@ -2720,7 +2720,7 @@ __device__ __forceinline__ float async_allowed_dt(const Material &M, const float
 
 // One pass over the particle pool: per block an occupied bit (1), and with limits min(0.1, allowed_dt) and max |v|^2 as
 // the bits of non-negative floats read as signed integers (ordered like the floats), a NaN as a flag bit (2: the limit,
-// 4: |v|^2).  A type without a limit sets *bad.
+// 4: |v|^2).  A type without a limit counts in *bad; its block is still occupied.
 __global__ void __launch_bounds__(256) k_async_limits(ARec R, int n, Params P, int with_limits, uint32_t *bflag, int *bmin, int *bmax, int *bad) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -2733,8 +2733,12 @@ __global__ void __launch_bounds__(256) k_async_limits(ARec R, int n, Params P, i
   const float v2 = __fadd_rn(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy)), __fmul_rn(vz, vz));
   const int g = min(max(R.group[i], 0), MPMB_MAX_GROUPS - 1);
   float adt = async_allowed_dt(P.mats[g], R.F + 9 * (size_t)i, R.scalar[i], R.mass[i], R.vol[i], v2, P.dx);
-  if (adt == -1.0f) { atomicAdd(bad, 1); return; }
   unsigned f = 1u;
+  if (adt == -1.0f) {
+    atomicAdd(bad, 1);
+    atomicOr(&bflag[blk], f);
+    return;
+  }
   if (adt != adt) f |= 2u;
   else atomicMin(&bmin[blk], __float_as_int(fminf(0.1f, adt)));
   if (v2 != v2) f |= 4u;
@@ -2866,6 +2870,143 @@ __global__ void k_async_route(const int *rowk, int ng, const int *flags, const i
   const size_t o = (size_t)off + prefix[k];
   arec_copy(D, o, S, (size_t)rowk[k]);
   D.id[o] = gid[k];
+}
+
+// ---- the block scheduler on the device (mpmb_async_schedule / mpmb_async_advance_level): async_mpm.update_dt_limits and
+// the flag building of async_mpm.advance, per block instead of per numpy pass
+struct ASched {
+  int bad;      // pool particles of a type without a time-step limit (k_async_limits)
+  int due;      // some occupied block is due
+  int low;      // some due block's limit is below one unit
+  int ne_max;   // max level over the occupied blocks after their update, 1 if there are none
+  int lv_min, lv_max;   // over all blocks after the empty-block pass
+  int sc;       // MPMB_ASYNC_SWAP | MPMB_ASYNC_CLEAR bits of the last flag set built on the device
+};
+// the schedule fails, and no block state changes: a type without a limit while a block is due (the host raises wherever in
+// the pool that particle lies, async_mpm._pool_scan), or a due block's limit below one unit
+__device__ __forceinline__ bool async_sched_failed(const ASched *S) { return S->low || (S->bad && S->due); }
+
+__global__ void k_async_state_init(int nblk, int *level, long long *local_min, long long *particle_t, long long *backup_t) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nblk) return;
+  level[i] = 1;
+  local_min[i] = 1;
+  particle_t[i] = 0;
+  backup_t[i] = 0;
+}
+
+// the block reductions of k_async_limits start empty (0.1 / 1e-16 as in mpmb_async_block_limits), the counters from nothing
+__global__ void k_async_sched_reset(int nblk, uint32_t *bflag, int *bmin, int *bmax, ASched *S) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) *S = ASched{0, 0, 0, 1, 0x7fffffff, 0, 0};
+  if (i >= nblk) return;
+  bflag[i] = 0u;
+  bmin[i] = 0x3dcccccd;   // 0.1f
+  bmax[i] = 0x2539705f;   // 1e-16f
+}
+
+// float32 -> int64 as numpy's astype on x86 (cvttss2si): truncation, INT64_MIN for NaN and |x| >= 2^63
+__device__ __forceinline__ long long async_f2i64(float x) { return fabsf(x) < 9223372036854775808.0f ? (long long)x : INT64_MIN; }
+
+// occupied blocks (update_dt_limits, :95-131): a due block takes tmp = min(cdl, sdl, max_units) and moves its level toward it,
+// into lv_new; strength limit sdl = (s min_adt) inv_unit, CFL limit cdl = ((c dx) inv_unit) (1 / sqrt(max_v2)), every
+// operation rounded on its own as the host's fp32 numpy expressions
+__global__ void k_async_sched_due(const uint32_t *bflag, const int *bmin, const int *bmax, const int *level, int *lv_new, int nblk, long long t,
+                                  float smul, float cmul, float dx, float inv_unit, long long max_units, ASched *S) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nblk) return;
+  const uint32_t f = bflag[i];
+  if (!(f & 1u)) return;
+  long long lv = level[i];
+  if ((t & (lv - 1)) == 0) {
+    atomicOr(&S->due, 1);
+    const float min_adt = (f & 2u) ? __uint_as_float(0x7fc00000u) : __int_as_float(bmin[i]);
+    const float max_v2 = (f & 4u) ? __uint_as_float(0x7fc00000u) : __int_as_float(bmax[i]);
+    const long long sdl = async_f2i64(__fmul_rn(__fmul_rn(smul, min_adt), inv_unit));
+    const long long cdl = async_f2i64(__fmul_rn(__fmul_rn(__fmul_rn(cmul, dx), inv_unit), 1.0f / sqrtf(max_v2)));   // IEEE / and sqrt
+    const long long tmp = min(min(cdl, sdl), max_units);
+    if (tmp < 1) {
+      atomicOr(&S->low, 1);
+      return;
+    }
+    while (tmp < lv) lv >>= 1;
+    while (tmp >= 2 * lv && (t & (2 * lv - 1)) == 0) lv <<= 1;
+  }
+  lv_new[i] = (int)lv;
+  atomicMax(&S->ne_max, (int)lv);
+}
+
+// every block's level is committed: an occupied block's from lv_new, an aligned empty one moves toward the occupied blocks'
+// max (:138-152); then min / max over all blocks
+__global__ void k_async_sched_commit(const uint32_t *bflag, const int *lv_new, int *level, int nblk, long long t, ASched *S) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nblk || async_sched_failed(S)) return;
+  long long lv;
+  if (bflag[i] & 1u) {
+    lv = lv_new[i];
+  } else {
+    lv = level[i];
+    if ((t & (lv - 1)) == 0) {
+      const long long mx = S->ne_max;
+      while (mx < lv) lv >>= 1;
+      while (mx >= 2 * lv && (t & (2 * lv - 1)) == 0) lv <<= 1;
+    }
+  }
+  level[i] = (int)lv;
+  atomicMin(&S->lv_min, (int)lv);
+  atomicMax(&S->lv_max, (int)lv);
+}
+
+// fn(j) for the linear index j of every in-range neighbour of block i (the scheduler's cached_neighbours,
+// src/async/async_mpm.h:255-300)
+template <class Fn>
+__device__ __forceinline__ void async_neighbours(int i, int nb0, int nb1, int nb2, Fn fn) {
+  const int bz = i % nb2, by = (i / nb2) % nb1, bx = i / (nb1 * nb2);
+  for (int dx = -1; dx <= 1; dx++)
+    for (int dy = -1; dy <= 1; dy++)
+      for (int dz = -1; dz <= 1; dz++) {
+        const int x = bx + dx, y = by + dy, z = bz + dz;
+        if ((dx | dy | dz) == 0 || x < 0 || y < 0 || z < 0 || x >= nb0 || y >= nb1 || z >= nb2) continue;
+        fn((x * nb1 + y) * nb2 + z);
+      }
+}
+
+// local_min_dt_limit (:165-181): a block off the finest level takes the earliest time a neighbour is stepped next
+__global__ void k_async_local_min(const int *level, const long long *particle_t, long long *local_min, int nb0, int nb1, int nb2, const ASched *S) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nb0 * nb1 * nb2 || async_sched_failed(S) || level[i] == S->lv_min) return;
+  long long lm = 1ll << 31;
+  async_neighbours(i, nb0, nb1, nb2, [&](int j) { lm = min(lm, particle_t[j] + level[j]); });
+  local_min[i] = lm;
+}
+
+// the MPMB_ASYNC_* bits of every block for level `limit` at clock t (async_mpm.advance; the larger / smaller neighbour sets
+// of :183-250 reduce to: a neighbour is on that level)
+__global__ void k_async_level_flags(const int *level, const long long *particle_t, const long long *local_min, int nb0, int nb1, int nb2, long long t,
+                                    int limit, uint8_t *bfl, ASched *S) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nb0 * nb1 * nb2) return;
+  const int lv = level[i];
+  int f;
+  if (lv == limit) {
+    f = ASYNC_EQUAL | (particle_t[i] == t ? ASYNC_SWAP : 0);
+  } else {
+    bool touch = false;
+    async_neighbours(i, nb0, nb1, nb2, [&](int j) { touch |= level[j] == limit; });
+    f = !touch ? 0 : lv < limit ? ASYNC_SMALLER : ASYNC_LARGER | (local_min[i] == t + limit ? ASYNC_CLEAR : 0);
+  }
+  bfl[i] = (uint8_t)f;
+  if (f & (ASYNC_SWAP | ASYNC_CLEAR)) atomicOr(&S->sc, f & (ASYNC_SWAP | ASYNC_CLEAR));
+}
+
+// the blocks' clocks after an advance of level `limit` (:318-343), in the host's order
+__global__ void k_async_level_clocks(const uint8_t *bfl, int nblk, long long t, int limit, long long *particle_t, long long *backup_t) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nblk) return;
+  const int f = bfl[i];
+  if (f & ASYNC_SWAP) backup_t[i] = t;
+  if (f & ASYNC_EQUAL) particle_t[i] = t + limit;
+  if (f & ASYNC_CLEAR) backup_t[i] = t + limit;
 }
 
 }  // namespace mpmb
@@ -3055,6 +3196,9 @@ struct MpmbEngine {
   DevBuf<uint32_t> a_u[4];
   DevBuf<int> a_rowk;                                               // its size is the candidate capacity
   DevBuf<unsigned char> a_cub;
+  DevBuf<int> a_level, a_lvnew;                                     // [nblk] the device scheduler's block levels, their update
+  DevBuf<long long> a_local_min, a_particle_t, a_backup_t;          // [nblk] its block clocks
+  DevBuf<ASched> a_sched;                                           // its reductions and error word
 
   bool profiling = false;
   struct Ev { cudaEvent_t a, b; int stage; };
@@ -3718,7 +3862,7 @@ int mpmb_append_particles(MpmbHandle h, int64_t n, const float *x, const float *
 }
 
 static int scan_reserve(MpmbEngine *h, size_t n);
-static int scan_flags(MpmbEngine *h, size_t n, int *total);
+static int scan_flags(MpmbEngine *h, size_t n, int *total, const int *word = nullptr, int *word_out = nullptr);
 
 int mpmb_append_owned_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
                                 const float *mass, const float *vol, const float *scalar, const int32_t *group, int64_t first_id,
@@ -3813,13 +3957,18 @@ static int scan_reserve(MpmbEngine *h, size_t n) {
   CUDA_TRY(h, h->scan_tmp.reserve(need));
   return MPMB_OK;
 }
-// prefix = exclusive scan of flags over n (+1 so that prefix[n] is the total); returns the total
-static int scan_flags(MpmbEngine *h, size_t n, int *total) {
+// prefix = exclusive scan of flags over n (+1 so that prefix[n] is the total); returns the total.  With `word`, that device
+// int comes back in the same read-back (it is copied behind the total: scan_reserve(n + 1) leaves the room).
+static int scan_flags(MpmbEngine *h, size_t n, int *total, const int *word, int *word_out) {
   CUDA_TRY(h, cudaMemsetAsync(h->scan_a.get() + n, 0, sizeof(int), h->stream));
   size_t bytes = h->scan_tmp.size();
   cub::DeviceScan::ExclusiveSum(h->scan_tmp.get(), bytes, h->scan_a.get(), h->scan_b.get(), (int)(n + 1), h->stream);
-  CUDA_TRY(h, cudaMemcpyAsync(total, h->scan_b.get() + n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  int out[2] = {0, 0};
+  if (word) CUDA_TRY(h, cudaMemcpyAsync(h->scan_b.get() + n + 1, word, sizeof(int), cudaMemcpyDeviceToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(out, h->scan_b.get() + n, sizeof(int) * (word ? 2 : 1), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  *total = out[0];
+  if (word) *word_out = out[1];
   return MPMB_OK;
 }
 
@@ -5257,7 +5406,8 @@ int mpmb_recut_apply(MpmbHandle h, int32_t tile_z0, int32_t tile_z1, int64_t n_i
 }  // extern "C"
 
 // =====================================================================================
-// AsyncMPM pools (mpmb_async_*, SURVEY §8f row 3): the particle records live on the device, the scheduler on the host
+// AsyncMPM pools (mpmb_async_*, SURVEY §8f row 3): the particle records live on the device; the block scheduler's state and
+// decisions too with mpmb_async_schedule / mpmb_async_advance_level, the step loop on the host
 // =====================================================================================
 static int async_check(MpmbEngine *h, bool need_init) {
   if (need_init && !h->async_on) return fail(h, MPMB_ERR_STATE, "mpmb_async_init has not been called");
@@ -5341,6 +5491,15 @@ int mpmb_async_init(MpmbHandle h, const int32_t nb[3], float inv_dx) {
   CUDA_TRY(h, h->a_blk.alloc(nblk));
   CUDA_TRY(h, h->a_lim.alloc(2 * nblk));
   CUDA_TRY(h, h->a_bad.alloc(1));
+  CUDA_TRY(h, h->a_level.alloc(nblk));
+  CUDA_TRY(h, h->a_lvnew.alloc(nblk));
+  CUDA_TRY(h, h->a_local_min.alloc(nblk));
+  CUDA_TRY(h, h->a_particle_t.alloc(nblk));
+  CUDA_TRY(h, h->a_backup_t.alloc(nblk));
+  CUDA_TRY(h, h->a_sched.alloc(1));
+  k_async_state_init<<<nblocks(nblk), 256, 0, h->stream>>>((int)nblk, h->a_level.get(), h->a_local_min.get(), h->a_particle_t.get(), h->a_backup_t.get());
+  h->launches++;
+  CUDA_TRY(h, cudaGetLastError());
   for (auto &p : h->apool)
     if ((rc = apool_reserve(h, p, 1024)) != MPMB_OK) return rc;
   h->async_on = true;
@@ -5418,21 +5577,15 @@ int mpmb_async_block_limits(MpmbHandle h, int32_t with_limits, int64_t cap, int6
   return MPMB_OK;
 }
 
-int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_gathered) {
-  CHECK_HANDLE(h);
-  int rc = async_check(h, true);
-  if (rc != MPMB_OK) return rc;
-  if (!flags || !n_gathered) return fail(h, MPMB_ERR_INVALID, "null argument");
-  if (!(dt > 0.f) || !std::isfinite(dt)) return fail(h, MPMB_ERR_INVALID, "dt must be positive and finite");
+}  // extern "C"
+
+// The pool work of one advance on the block flags in a_bfl (mpmb_async_advance: steps 1-5).  sc holds the MPMB_ASYNC_SWAP /
+// MPMB_ASYNC_CLEAR bits present in some block, or is -1: flags built on the device, whose bits a_sched->sc holds; they are
+// read with the candidate count (no candidates: both pools are empty and their edits do nothing).
+static int async_advance_body(MpmbEngine *h, float dt, int sc, int64_t *n_gathered) {
+  int rc;
   *n_gathered = 0;
   MpmbEngine::APool &P0 = h->apool[0], &B0 = h->apool[1];
-  const int nblk = h->nblk;
-  bool any_swap = false, any_clear = false;
-  for (int i = 0; i < nblk; i++) {
-    any_swap |= (flags[i] & MPMB_ASYNC_SWAP) != 0;
-    any_clear |= (flags[i] & MPMB_ASYNC_CLEAR) != 0;
-  }
-  CUDA_TRY(h, cudaMemcpyAsync(h->a_bfl.get(), flags, (size_t)nblk, cudaMemcpyHostToDevice, h->stream));
 
   // 1. gather: flagged candidates -> sort by (part, page index) -> first copy of every id -> the set, in that order
   const int np = (int)P0.n, nbk = (int)B0.n;
@@ -5440,11 +5593,12 @@ int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_
   int nc = 0, ng = 0;
   ARec G{}, S{};   // the gathered set and its survivors
   if (nc_all > 0) {
-    if ((rc = scan_reserve(h, (size_t)nc_all)) != MPMB_OK) return rc;
+    if ((rc = scan_reserve(h, (size_t)nc_all + (sc < 0 ? 1 : 0))) != MPMB_OK) return rc;
     k_async_cand_flags<<<nblocks(nc_all), 256, 0, h->stream>>>(P0.rec(P0.cur).block, np, B0.rec(B0.cur).block, nbk, h->a_bfl.get(), h->scan_a.get());
     h->launches++;
-    if ((rc = scan_flags(h, (size_t)nc_all, &nc)) != MPMB_OK) return rc;
+    if ((rc = scan_flags(h, (size_t)nc_all, &nc, sc < 0 ? &h->a_sched.get()->sc : nullptr, &sc)) != MPMB_OK) return rc;
   }
+  const bool any_swap = sc > 0 && (sc & MPMB_ASYNC_SWAP), any_clear = sc > 0 && (sc & MPMB_ASYNC_CLEAR);
   if (nc > 0) {
     const int64_t ccap = (int64_t)h->a_rowk.size();   // the candidate capacity
     if (nc > ccap) {
@@ -5535,6 +5689,89 @@ int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
   *n_gathered = ng;
+  return MPMB_OK;
+}
+
+extern "C" {
+
+int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_gathered) {
+  CHECK_HANDLE(h);
+  int rc = async_check(h, true);
+  if (rc != MPMB_OK) return rc;
+  if (!flags || !n_gathered) return fail(h, MPMB_ERR_INVALID, "null argument");
+  if (!(dt > 0.f) || !std::isfinite(dt)) return fail(h, MPMB_ERR_INVALID, "dt must be positive and finite");
+  *n_gathered = 0;
+  int sc = 0;
+  for (int i = 0; i < h->nblk; i++) sc |= flags[i] & (MPMB_ASYNC_SWAP | MPMB_ASYNC_CLEAR);
+  CUDA_TRY(h, cudaMemcpyAsync(h->a_bfl.get(), flags, (size_t)h->nblk, cudaMemcpyHostToDevice, h->stream));
+  return async_advance_body(h, dt, sc, n_gathered);
+}
+
+int mpmb_async_schedule(MpmbHandle h, int64_t t, float strength_mul, float cfl_mul, float dx, float inv_unit, int64_t max_units, int32_t *min_level,
+                        int32_t *max_level) {
+  CHECK_HANDLE(h);
+  int rc = async_check(h, true);
+  if (rc != MPMB_OK) return rc;
+  if (!min_level || !max_level) return fail(h, MPMB_ERR_INVALID, "null argument");
+  if (t < 0) return fail(h, MPMB_ERR_INVALID, "t = %lld is negative", (long long)t);
+  if (max_units < 1 || max_units > (1ll << 30)) return fail(h, MPMB_ERR_INVALID, "max_units = %lld outside [1, 2^30]", (long long)max_units);
+  const int nblk = h->nblk;
+  const MpmbEngine::APool &p = h->apool[0];
+  ASched *S = h->a_sched.get();
+  k_async_sched_reset<<<nblocks(nblk), 256, 0, h->stream>>>(nblk, h->a_bflag.get(), h->a_bmin.get(), h->a_bmax.get(), S);
+  h->launches++;
+  if (p.n > 0) {
+    k_async_limits<<<nblocks(p.n), 256, 0, h->stream>>>(p.rec(p.cur), (int)p.n, h->P, 1, h->a_bflag.get(), h->a_bmin.get(), h->a_bmax.get(), &S->bad);
+    h->launches++;
+  }
+  k_async_sched_due<<<nblocks(nblk), 256, 0, h->stream>>>(h->a_bflag.get(), h->a_bmin.get(), h->a_bmax.get(), h->a_level.get(), h->a_lvnew.get(), nblk, (long long)t,
+                                                          strength_mul, cfl_mul, dx, inv_unit, (long long)max_units, S);
+  k_async_sched_commit<<<nblocks(nblk), 256, 0, h->stream>>>(h->a_bflag.get(), h->a_lvnew.get(), h->a_level.get(), nblk, (long long)t, S);
+  k_async_local_min<<<nblocks(nblk), 256, 0, h->stream>>>(h->a_level.get(), h->a_particle_t.get(), h->a_local_min.get(), h->anb[0], h->anb[1], h->anb[2], S);
+  h->launches += 3;
+  ASched s;
+  CUDA_TRY(h, cudaMemcpyAsync(&s, S, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  if (s.bad && s.due) return fail(h, MPMB_ERR_INVALID, "%d pool particles are of a type without a time-step limit (linear / jelly)", s.bad);
+  if (s.low) return fail(h, MPMB_ERR_LIMIT, "a due block's time-step limit is below unit_delta_t");
+  *min_level = s.lv_min;
+  *max_level = s.lv_max;
+  return MPMB_OK;
+}
+
+int mpmb_async_advance_level(MpmbHandle h, int64_t t, int32_t limit, float dt, int64_t *n_gathered) {
+  CHECK_HANDLE(h);
+  int rc = async_check(h, true);
+  if (rc != MPMB_OK) return rc;
+  if (!n_gathered) return fail(h, MPMB_ERR_INVALID, "null argument");
+  *n_gathered = 0;
+  if (t < 0) return fail(h, MPMB_ERR_INVALID, "t = %lld is negative", (long long)t);
+  if (limit < 1 || (limit & (limit - 1))) return fail(h, MPMB_ERR_INVALID, "limit = %d is not a positive power of two", limit);
+  if (!(dt > 0.f) || !std::isfinite(dt)) return fail(h, MPMB_ERR_INVALID, "dt must be positive and finite");
+  const int nblk = h->nblk;
+  CUDA_TRY(h, cudaMemsetAsync(&h->a_sched.get()->sc, 0, sizeof(int), h->stream));
+  k_async_level_flags<<<nblocks(nblk), 256, 0, h->stream>>>(h->a_level.get(), h->a_particle_t.get(), h->a_local_min.get(), h->anb[0], h->anb[1], h->anb[2],
+                                                            (long long)t, limit, h->a_bfl.get(), h->a_sched.get());
+  h->launches++;
+  if ((rc = async_advance_body(h, dt, -1, n_gathered)) != MPMB_OK) return rc;
+  // the clocks move only once the advance has succeeded
+  k_async_level_clocks<<<nblocks(nblk), 256, 0, h->stream>>>(h->a_bfl.get(), nblk, (long long)t, limit, h->a_particle_t.get(), h->a_backup_t.get());
+  h->launches++;
+  CUDA_TRY(h, cudaGetLastError());
+  return MPMB_OK;
+}
+
+int mpmb_async_block_state(MpmbHandle h, int32_t *level, int64_t *local_min, int64_t *particle_t, int64_t *backup_t) {
+  CHECK_HANDLE(h);
+  int rc = async_check(h, true);
+  if (rc != MPMB_OK) return rc;
+  const size_t n = (size_t)h->nblk;
+  const struct { void *d; const void *s; size_t w; } cp[] = {{level, h->a_level.get(), sizeof(int32_t)}, {local_min, h->a_local_min.get(), sizeof(int64_t)},
+                                                            {particle_t, h->a_particle_t.get(), sizeof(int64_t)}, {backup_t, h->a_backup_t.get(), sizeof(int64_t)}};
+  for (const auto &c : cp)
+    if (c.d) CUDA_TRY(h, cudaMemcpyAsync(c.d, c.s, c.w * n, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   return MPMB_OK;
 }
 
