@@ -91,7 +91,24 @@ typedef struct MpmbConfig {
   int32_t halo_capacity;     /* max active tiles in one boundary layer; 0 = the whole cross-section */
   int32_t no_graph;          /* 1: launch every kernel from the host; 0 (default): mpmb_substep replays pairs of
                               * substeps as a CUDA graph (same kernels, same order, same results)              */
-  int32_t reserved[6];       /* must be 0                                                         */
+  /* 0 or 3: MPM<3> (everything above and below).  2: MPM<2> (src/mpm.cpp:983-988): res[2] == 0, gravity[2] == 0,
+   * world == 1; particle arrays are dim-packed (x[n][2], v[n][2], F[n][4] and b[n][4] column-major), a dense node
+   * array is [res0+1][res1+1][4] with the z component 0, and only these entry points work on the handle:
+   *   mpmb_create, mpmb_destroy, mpmb_last_error, mpmb_set_stream, mpmb_synchronize, mpmb_set_material,
+   *   mpmb_set_delta_t, mpmb_set_planes / mpmb_set_levelset_shapes (planes, circles as MPMB_SHAPE_SPHERE, rectangles as
+   *   MPMB_SHAPE_CUBOID; every z part must be 0), mpmb_set_sdf, mpmb_upload_particles, mpmb_set_id_base,
+   *   mpmb_num_particles, mpmb_get_update_count, mpmb_download_particles, mpmb_download_bgeo_points (z = 0, as
+   *   MPM<2>::write_partio writes), mpmb_substep and its three stages, mpmb_download_grid, mpmb_set_profiling,
+   *   mpmb_get_profile, mpmb_get_counters.
+   * Every other entry point returns MPMB_ERR_STATE (the *_bytes calls included) with a message: AoS pools, lattice
+   * seeding, appends and deletions, rigid bodies, AsyncMPM, z-slabs and re-cuts are MPM<3> only.
+   * The deletion rule is the same as in 3-D with the 9-node stencil; in addition G2P clamps the position to
+   * [0, res - 1e-6] cells as MPM<2>::resample does, and a particle whose velocity is not finite is deleted too.      */
+  int32_t dim;
+  /* `apic_damping` / `rpic_damping` (src/mpm.cpp:33-34, src/mpm.h:465-469): apic_b = (1 - rpic) sym(b) + (1 - apic)
+   * skew(b).  dim == 2 only (0 otherwise: MPM<3>'s optimized resample passes them a block index).                  */
+  float apic_damping, rpic_damping;
+  int32_t reserved[3];       /* must be 0                                                         */
 } MpmbConfig;
 
 /* Byte offsets of the fields of one reference particle slot (ParticleContainer<3>, 320 B,

@@ -10,7 +10,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_PKG)
 SRC = [os.path.join(_PKG, "csrc", "mpmb_engine.cu")]
 # this file is a dependency too: a change of NVCC_FLAGS (e.g. the target architecture) rebuilds the library
-DEPS = SRC + [os.path.join(_PKG, "csrc", "mpmb_math.cuh"), os.path.join(_ROOT, "include", "mpmb.h"), os.path.abspath(__file__)]
+DEPS = SRC + [os.path.join(_PKG, "csrc", "mpmb_math.cuh"), os.path.join(_PKG, "csrc", "mpmb_math2d.cuh"), os.path.join(_ROOT, "include", "mpmb.h"), os.path.abspath(__file__)]
 LIB = os.path.join(_PKG, "lib", "libmpmb.so")
 # the bounds-checked variant (-DMPMB_CHECKED): an index that would leave its array is recorded and skipped
 CHECKED_LIB = os.path.join(_PKG, "lib", "libmpmb_checked.so")

@@ -60,7 +60,10 @@ class MpmbConfig(C.Structure):
         ("migrate_capacity", C.c_int64),
         ("halo_capacity", C.c_int32),
         ("no_graph", C.c_int32),
-        ("reserved", C.c_int32 * 6),
+        ("dim", C.c_int32),
+        ("apic_damping", C.c_float),
+        ("rpic_damping", C.c_float),
+        ("reserved", C.c_int32 * 3),
     ]
 
 
@@ -148,14 +151,17 @@ class Engine:
     """Thin object wrapper over one MpmbHandle."""
 
     def __init__(self, res, dx, dt, gravity=(0.0, -10.0, 0.0), particle_gravity=True, clean_boundary=True, device=0,
-                 capacity=0, rank=0, world=1, tile_z0=0, tile_z1=0, migrate_capacity=0, halo_capacity=0, no_graph=False):
+                 capacity=0, rank=0, world=1, tile_z0=0, tile_z1=0, migrate_capacity=0, halo_capacity=0, no_graph=False, dim=0,
+                 apic_damping=0.0, rpic_damping=0.0):
         self.L = lib()
         cfg = MpmbConfig()
         if np.isscalar(res):
             res = (res, res, res)
-        cfg.res[:] = [int(r) for r in res]
+        cfg.res[:] = [int(r) for r in res] + [0] * (3 - len(res))
+        cfg.dim = int(dim)
+        cfg.apic_damping, cfg.rpic_damping = float(apic_damping), float(rpic_damping)
         cfg.dx, cfg.dt = float(dx), float(dt)
-        cfg.gravity[:] = [float(g) for g in gravity]
+        cfg.gravity[:] = [float(g) for g in gravity] + [0.0] * (3 - len(gravity))
         cfg.particle_gravity = int(bool(particle_gravity))
         cfg.clean_boundary = int(bool(clean_boundary))
         cfg.device = int(device)
@@ -660,3 +666,44 @@ class Engine:
         a, b, c = C.c_int64(0), C.c_int64(0), C.c_int64(0)
         self._check(self.L.mpmb_get_counters(self.h, C.byref(a), C.byref(b), C.byref(c)))
         return dict(active_tiles=a.value, alive=b.value, kernel_launches=c.value)
+
+
+class Engine2D(Engine):
+    """A 2-D handle (MpmbConfig.dim = 2, MPM<2>): res = (r0, r1), gravity = (g_x, g_y); particle arrays are dim-packed
+    (x, v [n, 2]; F, b [n, 4] column-major) and dense node arrays are (r0 + 1, r1 + 1, 4) with the z component 0.  The
+    entry points include/mpmb.h lists for dim = 2 work; every other method returns the engine's error."""
+
+    def __init__(self, res, dx, dt, gravity=(0.0, -10.0), particle_gravity=True, clean_boundary=True, device=0, capacity=0,
+                 no_graph=False, apic_damping=0.0, rpic_damping=0.0):
+        res = tuple(int(r) for r in res)
+        if len(res) != 2 or len(gravity) != 2:
+            raise ValueError("a 2-D engine takes res = (r0, r1) and gravity = (g_x, g_y)")
+        super().__init__(res, dx, dt, gravity, particle_gravity, clean_boundary, device=device, capacity=capacity, no_graph=no_graph,
+                         dim=2, apic_damping=apic_damping, rpic_damping=rpic_damping)
+        self.res = res
+
+    def upload(self, x, v, mass, vol, F=None, b=None, scalar=None, group=None):
+        x = _f32(x).reshape(-1, 2)
+        n = len(x)
+        v, F, b = _f32(v, (n, 2)), _f32(F, (n, 4)), _f32(b, (n, 4))
+        mass, vol, scalar = _f32(mass, (n,)), _f32(vol, (n,)), _f32(scalar, (n,))
+        group = None if group is None else np.ascontiguousarray(group, np.int32).reshape(n)
+        self._check(self.L.mpmb_upload_particles(self.h, C.c_int64(n), _ptr(x), _ptr(v), _ptr(F), _ptr(b), _ptr(mass), _ptr(vol),
+                                                 _ptr(scalar), _ptr(group)))
+
+    def download(self, cap=None, sort_by_id=True):
+        """Returns dict(id,x,v,F,b,mass,vol,ps,group) of the live particles (x, v [n, 2]; F, b [n, 4])."""
+        if cap is None:
+            cap = max(self.num_particles(), 1)
+        out = dict(id=np.zeros(cap, np.uint32), x=np.zeros((cap, 2), np.float32), v=np.zeros((cap, 2), np.float32),
+                   F=np.zeros((cap, 4), np.float32), b=np.zeros((cap, 4), np.float32), mass=np.zeros(cap, np.float32),
+                   vol=np.zeros(cap, np.float32), ps=np.zeros(cap, np.float32), group=np.zeros(cap, np.int32))
+        n = C.c_int64(0)
+        self._check(self.L.mpmb_download_particles(self.h, C.c_int64(cap), C.byref(n), _ptr(out["id"]), _ptr(out["x"]), _ptr(out["v"]),
+                                                   _ptr(out["F"]), _ptr(out["b"]), _ptr(out["mass"]), _ptr(out["vol"]), _ptr(out["ps"]),
+                                                   _ptr(out["group"])))
+        out = {k: a[: n.value] for k, a in out.items()}
+        if sort_by_id:
+            o = np.argsort(out["id"], kind="stable")
+            out = {k: a[o] for k, a in out.items()}
+        return out

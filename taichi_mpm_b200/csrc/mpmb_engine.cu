@@ -36,6 +36,7 @@
 
 #include "../../include/mpmb.h"
 #include "mpmb_math.cuh"
+#include "mpmb_math2d.cuh"
 
 namespace mpmb {
 
@@ -3069,8 +3070,11 @@ static ARec arec_layout(float *w, int64_t cap) {
 static int64_t arec_cap(const DevBuf<float> &buf) { return (int64_t)(buf.size() / AREC_WORDS); }
 static ARec arec_of(const DevBuf<float> &buf) { return arec_layout(buf.get(), arec_cap(buf)); }
 
+struct Mpm2d;  // the 2-D engine (below, "The 2-D engine")
+
 struct MpmbEngine {
   MpmbConfig cfg{};
+  Mpm2d *m2 = nullptr;   // set on a 2-D handle (cfg.dim == 2): every entry point routes to it or refuses
   Params P{};
   cudaStream_t stream = nullptr;
   std::string err;
@@ -3437,6 +3441,740 @@ static int alloc_tile_arrays(MpmbEngine *h, int64_t cap_tiles) {
   return MPMB_OK;
 }
 
+// entry points that a 2-D handle does not have (include/mpmb.h lists what it has)
+#define NOT_2D(h) \
+  if ((h)->m2) return fail((h), MPMB_ERR_STATE, "%s is not available on a 2-D handle (dim = 2)", __func__)
+
+// =====================================================================================
+// The 2-D engine (MpmbConfig.dim == 2): MPM<2>::substep() of the reference (src/mpm.cpp:452-575) with the scalar
+// transfers MPM<2> runs (rasterize / resample, src/transfer.cpp:193-284, 585-701).  It sits after the handle type; the
+// C-ABI entry points route a 2-D handle here.  None of the 3-D tiles, arenas or orderings is used.
+//
+// Layout (DESIGN.md §10): particles are SoA, double buffered: x float2, v float2, F float4 and b float4
+// (column-major 2x2), aux float4 = (mass, vol, scalar, tag) with tag = group << 28 | id.  One substep is
+//   ordering  radix sort of the rows by the cell of their base node (dead rows last), a permutation into the other
+//             buffer and the [begin, end) row range of every cell;
+//   P2G       one thread per particle forms (X, m v, A = apic_b (4 m) - stress (4 dt / dx)); then one thread per node
+//             sums the particles of the 3x3 cells whose stencil covers it, in storage order, and finishes the node in
+//             place: normalise, gravity, level-set boundary.  No atomics: results are bit-reproducible;
+//   G2P       one thread per particle: gather, apic_b (damped), the 2x2 constitutive step, advection, the position
+//             clamp and the deletion rule, which writes the next ordering's key.
+// Nothing crosses the bus between substeps; mpmb_substep replays one captured substep per buffer parity.
+
+namespace mpmb {
+
+constexpr int M2_TILE = 16;  // node tile edge of the grid kernel (16 x 16 nodes = 256 threads)
+
+struct Params2 {
+  int res[2], nnode[2];
+  int ncells;  // res0 * res1; the key of a dead row
+  float dx, inv_dx, dt;
+  float gdt[2];  // gravity * dt
+  int particle_gravity, clean_boundary;
+  float friction;
+  int has_sdf;
+  float apic_damping, rpic_damping;
+  Material mats[MPMB_MAX_GROUPS];
+};
+
+struct Counters2 {
+  int n_alive;  // live rows after the last ordering
+  int n_live;   // scratch of mpmb_num_particles
+  int error;
+  int pad;
+  unsigned long long updates;
+};
+
+struct View2 {
+  float2 *x, *v;
+  float4 *F, *b, *aux;
+  float2 *xn, *vn;  // the other buffer (written by the ordering)
+  float4 *Fn, *bn, *auxn;
+  uint32_t *keys, *keys_sorted, *perm;
+  int *cell_begin, *cell_end;
+  float4 *pa, *pb;  // P2G records: (X, Y, m vx, m vy), affine (column-major)
+  float *pm;
+  float4 *graw;     // (p_x, p_y, 0, m) after P2G
+  float2 *gv;       // node velocity after normalise + boundary
+  const float4 *sdf4;
+  Counters2 *cnt;
+};
+
+__device__ __forceinline__ uint32_t cell_key2(const Params2 &P, float2 x) {
+  const float X = __fmul_rn(x.x, P.inv_dx), Y = __fmul_rn(x.y, P.inv_dx);
+  if (!isfinite(X) || !isfinite(Y)) return (uint32_t)P.ncells;
+  const int bx = (int)__fsub_rn(X, 0.5f), by = (int)__fsub_rn(Y, 0.5f);
+  // the 9-node stencil [base, base+2] must stay on the node grid
+  if (bx < 0 || by < 0 || bx + 2 > P.res[0] || by + 2 > P.res[1]) return (uint32_t)P.ncells;
+  return (uint32_t)(bx * P.res[1] + by);
+}
+
+__global__ void k2_pack(View2 V, Params2 P, int n, const float *x, const float *v, const float *F, const float *b, const float *mass,
+                        const float *vol, const float *scalar, const int *group, uint32_t id0) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int g = group ? group[i] : 0;
+  float m = mass[i];
+  if (g < 0 || g >= MPMB_MAX_GROUPS || !(m > 0.f)) {
+    atomicOr(&V.cnt->error, DEVERR_BAD_INPUT);
+    g = min(max(g, 0), MPMB_MAX_GROUPS - 1);
+    m = 1e-30f;
+  }
+  float ps;
+  if (scalar) ps = scalar[i];
+  else ps = (P.mats[g].kind == MAT_SNOW || P.mats[g].kind == MAT_WATER) ? 1.0f : 0.0f;  // Jp = 1, j = 1, logJp = 0
+  const float2 xx = make_float2(x[2 * (size_t)i], x[2 * (size_t)i + 1]);
+  V.x[i] = xx;
+  V.v[i] = make_float2(v[2 * (size_t)i], v[2 * (size_t)i + 1]);
+  V.F[i] = F ? make_float4(F[4 * (size_t)i], F[4 * (size_t)i + 1], F[4 * (size_t)i + 2], F[4 * (size_t)i + 3]) : make_float4(1.f, 0.f, 0.f, 1.f);
+  V.b[i] = b ? make_float4(b[4 * (size_t)i], b[4 * (size_t)i + 1], b[4 * (size_t)i + 2], b[4 * (size_t)i + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
+  V.aux[i] = make_float4(m, vol[i], ps, __uint_as_float(((uint32_t)g << TAG_ID_BITS) | (id0 + (uint32_t)i)));
+  V.keys[i] = cell_key2(P, xx);
+}
+
+// ---------------------------------------------------------------- ordering
+__global__ void k2_permute(View2 V, Params2 P, int n) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const uint32_t key = V.keys_sorted[j];
+  V.keys[j] = key;
+  if (key >= (uint32_t)P.ncells) return;
+  const uint32_t s = V.perm[j];
+  V.xn[j] = V.x[s];
+  V.vn[j] = V.v[s];
+  V.Fn[j] = V.F[s];
+  V.bn[j] = V.b[s];
+  V.auxn[j] = V.aux[s];
+}
+// [begin, end) of every cell from the sorted keys (cells without particles keep the memset 0, 0) and the live count
+__global__ void k2_cells(View2 V, Params2 P, int n) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const uint32_t dead = (uint32_t)P.ncells, k = V.keys_sorted[j];
+  const uint32_t prev = j > 0 ? V.keys_sorted[j - 1] : 0xffffffffu;
+  const uint32_t next = j + 1 < n ? V.keys_sorted[j + 1] : dead;
+  if (k < dead) {
+    if (k != prev) V.cell_begin[k] = j;
+    if (k != next) V.cell_end[k] = j + 1;
+    if (next >= dead) V.cnt->n_alive = j + 1;
+  } else if (j == 0) {
+    V.cnt->n_alive = 0;
+  }
+}
+
+// ---------------------------------------------------------------- P2G
+// MPM<2>::rasterize(dt, true) (src/transfer.cpp:193-278) without rigid bodies: the particle gravity kick, then per node
+// w (m v + apic_b (inv_D m) dpos - (dt force) dpos 4 inv_dx, m) with dpos = X - node in grid units
+__global__ void __launch_bounds__(256) k2_p2g_particles(View2 V, Params2 P, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) V.cnt->updates += (unsigned long long)V.cnt->n_alive;  // update_counter += particles.size() (src/mpm.cpp:436)
+  if (i >= n || V.keys[i] >= (uint32_t)P.ncells) return;
+  const float2 x = V.x[i];
+  float2 v = V.v[i];
+  const float4 f = V.F[i], b = V.b[i], aux = V.aux[i];
+  if (P.particle_gravity) v = make_float2(v.x + P.gdt[0], v.y + P.gdt[1]);
+  const int g = (int)(__float_as_uint(aux.w) >> TAG_ID_BITS);
+  const Mat2 F = {{f.x, f.y, f.z, f.w}};
+  const Mat2 force = calculate_force2(P.mats[g], F, aux.z, aux.y);
+  const float m = aux.x, bm = 4.0f * m, S = -4.0f * P.inv_dx * P.dt;  // Kernel::inv_D() = 4
+  V.pa[i] = make_float4(__fmul_rn(x.x, P.inv_dx), __fmul_rn(x.y, P.inv_dx), m * v.x, m * v.y);
+  V.pb[i] = make_float4(fmaf(force.m[0], S, b.x * bm), fmaf(force.m[1], S, b.y * bm), fmaf(force.m[2], S, b.z * bm), fmaf(force.m[3], S, b.w * bm));
+  V.pm[i] = m;
+}
+
+// One thread per node: the fixed-order sum over the particles of cells [i-2, i] x [j-2, j], then
+// normalize_grid_and_apply_external_force and apply_grid_boundary_conditions (src/mpm.cpp:277-372), static level set.
+__global__ void __launch_bounds__(256) k2_grid(View2 V, Params2 P, int tiles1) {
+  const int t = threadIdx.x;
+  const int i = (blockIdx.x / tiles1) * M2_TILE + (t >> 4), j = (blockIdx.x % tiles1) * M2_TILE + (t & 15);
+  if (i >= P.nnode[0] || j >= P.nnode[1]) return;
+  float px = 0.f, py = 0.f, m = 0.f;
+  for (int cx = max(i - 2, 0); cx <= min(i, P.res[0] - 1); cx++)
+    for (int cy = max(j - 2, 0); cy <= min(j, P.res[1] - 1); cy++) {
+      const int c = cx * P.res[1] + cy, e = V.cell_end[c];
+      for (int r = V.cell_begin[c]; r < e; r++) {
+        const float4 a = V.pa[r], A = V.pb[r];
+        int bx, by;
+        float wx[3], wy[3];
+        quadratic_weights2(a.x, bx, wx);
+        quadratic_weights2(a.y, by, wy);
+        const float w = wx[i - cx] * wy[j - cy];
+        const float dx = a.x - (float)i, dy = a.y - (float)j;
+        px += w * fmaf(A.z, dy, fmaf(A.x, dx, a.z));
+        py += w * fmaf(A.w, dy, fmaf(A.y, dx, a.w));
+        m += w * V.pm[r];
+      }
+    }
+  const size_t node = (size_t)i * P.nnode[1] + j;
+  V.graw[node] = make_float4(px, py, 0.f, m);
+  float2 vel = make_float2(px, py);
+  if (m > 0.f) {
+    const float inv = 1.0f / m;
+    const float ix = P.particle_gravity ? 0.f : P.gdt[0], iy = P.particle_gravity ? 0.f : P.gdt[1];
+    vel = make_float2(fmaf(px, inv, ix), fmaf(py, inv, iy));
+  }
+  if (P.has_sdf && m != 0.f) {
+    const float4 s = V.sdf4[node];
+    if (!(s.w < -3.f || 0.f < s.w)) vel = friction_project2(vel, make_float2(s.x, s.y), P.friction);
+  }
+  V.gv[node] = vel;
+}
+
+// ---------------------------------------------------------------- G2P
+// MPM<2>::resample() (src/transfer.cpp:585-687) without rigid bodies, then the deletion rule: clean_boundary = 1 deletes
+// in the 7-cell band (near_boundary, src/mpm.h:269-276) and non-finite particles (src/mpm.cpp:583-633); clean_boundary = 0
+// deletes a particle whose 9-node stencil leaves the node grid or whose position or velocity is not finite.
+__global__ void __launch_bounds__(256) k2_g2p(View2 V, Params2 P, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || V.keys[i] >= (uint32_t)P.ncells) return;
+  float2 x = V.x[i];
+  const float4 f = V.F[i];
+  float4 aux = V.aux[i];
+  const float X = __fmul_rn(x.x, P.inv_dx), Y = __fmul_rn(x.y, P.inv_dx);
+  int bx, by;
+  float wx[3], wy[3];
+  quadratic_weights2(X, bx, wx);
+  quadratic_weights2(Y, by, wy);
+  float vx = 0.f, vy = 0.f;
+  Mat2 B = {{0.f, 0.f, 0.f, 0.f}};
+#pragma unroll
+  for (int a = 0; a < 3; a++)
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+      const float2 gv = V.gv[(size_t)(bx + a) * P.nnode[1] + (by + c)];
+      const float w = wx[a] * wy[c];
+      const float dx = X - (float)(bx + a), dy = Y - (float)(by + c);
+      const float wgx = w * gv.x, wgy = w * gv.y;
+      vx += wgx;
+      vy += wgy;
+      B.m[0] = fmaf(wgx, dx, B.m[0]);
+      B.m[1] = fmaf(wgy, dx, B.m[1]);
+      B.m[2] = fmaf(wgx, dy, B.m[2]);
+      B.m[3] = fmaf(wgy, dy, B.m[3]);
+    }
+  // apic_b = damp_affine_momemtum(b) = (1 - rpic) sym(b) + (1 - apic) skew(b) (src/mpm.h:465-469)
+  const float sym_o = 0.5f * (B.m[1] + B.m[2]);
+  const float kr = 1.f - P.rpic_damping, ka = 1.f - P.apic_damping;
+  const float4 bd = make_float4(kr * B.m[0], kr * sym_o + ka * (B.m[1] - sym_o), kr * sym_o + ka * (B.m[2] - sym_o), kr * B.m[3]);
+  // cdg = I + dt (b (-4 inv_dx)) of the undamped b
+  const float S = -4.f * P.inv_dx;
+  Mat2 cdg;
+  cdg.m[0] = 1.f + P.dt * (B.m[0] * S);
+  cdg.m[1] = P.dt * (B.m[1] * S);
+  cdg.m[2] = P.dt * (B.m[2] * S);
+  cdg.m[3] = 1.f + P.dt * (B.m[3] * S);
+  const int g = (int)(__float_as_uint(aux.w) >> TAG_ID_BITS);
+  Mat2 F = {{f.x, f.y, f.z, f.w}};
+  plasticity2(P.mats[g], cdg, F, aux.z);
+  x = make_float2(x.x + P.dt * vx, x.y + P.dt * vy);
+  const bool finite = isfinite(x.x) && isfinite(x.y) && isfinite(vx) && isfinite(vy);
+  // position correction: (pos inv_dx).clamp(0, res - eps) dx, eps = 1e-6
+  x.x = fminf(fmaxf(x.x * P.inv_dx, 0.f), (float)P.res[0] - 1e-6f) * P.dx;
+  x.y = fminf(fmaxf(x.y * P.inv_dx, 0.f), (float)P.res[1] - 1e-6f) * P.dx;
+  bool dead = !finite;
+  if (P.clean_boundary) {
+    const float Xn = x.x * P.inv_dx, Yn = x.y * P.inv_dx;
+    dead |= fminf(Xn, Yn) < 7.0f || fmaxf(Xn - (float)P.res[0], Yn - (float)P.res[1]) > -7.0f;
+  }
+  V.x[i] = x;
+  V.v[i] = make_float2(vx, vy);
+  V.F[i] = make_float4(F.m[0], F.m[1], F.m[2], F.m[3]);
+  V.b[i] = bd;
+  V.aux[i] = aux;
+  V.keys[i] = dead ? (uint32_t)P.ncells : cell_key2(P, x);
+}
+
+__global__ void __launch_bounds__(256) k2_count_live(const uint32_t *keys, int n, uint32_t dead, Counters2 *cnt) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && keys[i] < dead) atomicAdd(&cnt->n_live, 1);
+}
+
+// the level set of 2-D solids: mpmb_set_planes / mpmb_set_levelset_shapes with zero z parts, node (n_x, n_y, 0, phi)
+__global__ void k2_shapes_to_sdf(Params2 P, int n_shapes, const MpmbShape *shapes, float4 *sdf4) {
+  const size_t n = (size_t)P.nnode[0] * P.nnode[1];
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int gx = (int)(i / P.nnode[1]), gy = (int)(i % P.nnode[1]);
+    float4 best = make_float4(1.f, 0.f, 0.f, 1e30f);
+    for (int k = 0; k < n_shapes; k++) {
+      const float4 c = shape_sdf(shapes[k], (float)gx, (float)gy, 0.f);
+      if (c.w < best.w) best = c;
+    }
+    sdf4[i] = best;
+  }
+}
+
+}  // namespace mpmb
+
+// ================================================================================================ host side
+struct Mpm2d {
+  Params2 P{};
+  int64_t cap = 0;   // rows allocated per buffer
+  int64_t rows = 0;  // rows of the current storage (the last upload's n); dead rows keep the dead key
+  int cur = 0;
+  int stage = 0;     // 0 idle / after G2P, 1 after the ordering, 2 after P2G
+  int key_bits = 32;
+  uint32_t id_base = 0;
+  DevBuf<float2> x[2], v[2];
+  DevBuf<float4> F[2], b[2], aux[2];
+  DevBuf<uint32_t> keys, keys_sorted, perm, iota;
+  DevBuf<unsigned char> cub_temp;
+  DevBuf<int> cell_begin, cell_end;
+  DevBuf<float4> pa, pb, graw, sdf4;
+  DevBuf<float> pm;
+  DevBuf<float2> gv;
+  DevBuf<Counters2> cnt;
+  DevBuf<float> stage_buf;
+  cudaGraphExec_t graph[2] = {nullptr, nullptr};
+  int graph_launches = 0;
+};
+
+static void m2_graph_reset(Mpm2d *m) {
+  for (int p = 0; p < 2; p++)
+    if (m->graph[p]) { cudaGraphExecDestroy(m->graph[p]); m->graph[p] = nullptr; }
+}
+
+static View2 m2_view(MpmbEngine *h) {
+  Mpm2d *m = h->m2;
+  View2 V{};
+  const int c = m->cur, o = c ^ 1;
+  V.x = m->x[c].get(); V.v = m->v[c].get(); V.F = m->F[c].get(); V.b = m->b[c].get(); V.aux = m->aux[c].get();
+  V.xn = m->x[o].get(); V.vn = m->v[o].get(); V.Fn = m->F[o].get(); V.bn = m->b[o].get(); V.auxn = m->aux[o].get();
+  V.keys = m->keys.get(); V.keys_sorted = m->keys_sorted.get(); V.perm = m->perm.get();
+  V.cell_begin = m->cell_begin.get(); V.cell_end = m->cell_end.get();
+  V.pa = m->pa.get(); V.pb = m->pb.get(); V.pm = m->pm.get();
+  V.graw = m->graw.get(); V.gv = m->gv.get();
+  V.sdf4 = m->sdf4.get();
+  V.cnt = m->cnt.get();
+  return V;
+}
+
+static unsigned m2_blocks(int64_t n, int t) { return (unsigned)std::max<int64_t>(1, (n + t - 1) / t); }
+
+static int m2_create(MpmbEngine *h, const MpmbConfig *cfg) {
+  Mpm2d *m = new Mpm2d();
+  h->m2 = m;
+  Params2 &P = m->P;
+  for (int d = 0; d < 2; d++) {
+    P.res[d] = cfg->res[d];
+    P.nnode[d] = cfg->res[d] + 1;
+    P.gdt[d] = cfg->gravity[d] * cfg->dt;
+  }
+  P.ncells = cfg->res[0] * cfg->res[1];
+  P.dx = cfg->dx;
+  P.inv_dx = 1.0f / cfg->dx;
+  P.dt = cfg->dt;
+  P.particle_gravity = cfg->particle_gravity;
+  P.clean_boundary = cfg->clean_boundary;
+  P.apic_damping = cfg->apic_damping;
+  P.rpic_damping = cfg->rpic_damping;
+  for (int g = 0; g < MPMB_MAX_GROUPS; g++) P.mats[g] = h->P.mats[g];  // the default material of mpmb_create
+  m->key_bits = 1;
+  while ((1ll << m->key_bits) <= (int64_t)P.ncells) m->key_bits++;
+  const size_t nodes = (size_t)P.nnode[0] * P.nnode[1];
+  if (m->cell_begin.alloc(P.ncells) != cudaSuccess || m->cell_end.alloc(P.ncells) != cudaSuccess || m->graw.alloc(nodes) != cudaSuccess ||
+      m->gv.alloc(nodes) != cudaSuccess || m->cnt.alloc(1) != cudaSuccess)
+    return fail(nullptr, MPMB_ERR_CUDA, "cudaMalloc of the 2-D grid (%lld nodes): %s", (long long)nodes, cudaGetErrorString(cudaGetLastError()));
+  cudaMemset(m->cnt.get(), 0, sizeof(Counters2));
+  return MPMB_OK;
+}
+
+static void m2_destroy(MpmbEngine *h) {
+  if (!h->m2) return;
+  m2_graph_reset(h->m2);
+  delete h->m2;
+  h->m2 = nullptr;
+}
+
+static int m2_alloc_rows(MpmbEngine *h, int64_t cap) {
+  Mpm2d *m = h->m2;
+  m2_graph_reset(m);
+  if (cap >= (1ll << 30)) return fail(h, MPMB_ERR_CAPACITY, "capacity %lld exceeds 2^30 particle rows per GPU", (long long)cap);
+  cap = std::max<int64_t>(cap, 1);
+  for (int b = 0; b < 2; b++) {
+    CUDA_TRY(h, m->x[b].alloc(cap)); CUDA_TRY(h, m->v[b].alloc(cap)); CUDA_TRY(h, m->F[b].alloc(cap));
+    CUDA_TRY(h, m->b[b].alloc(cap)); CUDA_TRY(h, m->aux[b].alloc(cap));
+  }
+  CUDA_TRY(h, m->keys.alloc(cap)); CUDA_TRY(h, m->keys_sorted.alloc(cap)); CUDA_TRY(h, m->perm.alloc(cap)); CUDA_TRY(h, m->iota.alloc(cap));
+  CUDA_TRY(h, m->pa.alloc(cap)); CUDA_TRY(h, m->pb.alloc(cap)); CUDA_TRY(h, m->pm.alloc(cap));
+  k_iota<<<m2_blocks(cap, 256), 256, 0, h->stream>>>(m->iota.get(), (int)cap);
+  h->launches++;
+  size_t bytes = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, bytes, m->keys.get(), m->keys_sorted.get(), m->iota.get(), m->perm.get(), (int)cap, 0, m->key_bits, h->stream);
+  CUDA_TRY(h, m->cub_temp.alloc(std::max<size_t>(bytes, 16)));
+  m->cap = cap;
+  return MPMB_OK;
+}
+
+static int m2_upload(MpmbEngine *h, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
+                     const float *vol, const float *scalar, const int32_t *group) {
+  Mpm2d *m = h->m2;
+  if (n < 0 || (n > 0 && (!x || !v || !mass || !vol))) return fail(h, MPMB_ERR_INVALID, "x, v, mass, vol are required");
+  if ((int64_t)m->id_base + n > (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_CAPACITY, "particle ids exceed 2^%d", TAG_ID_BITS);
+  if (m->stage != 0) return fail(h, MPMB_ERR_STATE, "upload between substeps, not inside one");
+  if (h->cfg.capacity > 0 && n > m->cap) return fail(h, MPMB_ERR_CAPACITY, "%lld particles exceed the configured capacity %lld", (long long)n, (long long)m->cap);
+  if (n > m->cap) { int rc = m2_alloc_rows(h, n); if (rc != MPMB_OK) return rc; }
+  m2_graph_reset(m);
+  const size_t words = (size_t)n * (2 + 2 + (F ? 4 : 0) + (b ? 4 : 0) + 1 + 1 + (scalar ? 1 : 0) + (group ? 1 : 0));
+  CUDA_TRY(h, m->stage_buf.reserve(std::max<size_t>(words, 1)));
+  float *p = m->stage_buf.get();
+  auto put = [&](const void *src, size_t count) -> float * {
+    if (!src) return nullptr;
+    float *dst = p;
+    cudaMemcpyAsync(dst, src, count * sizeof(float), cudaMemcpyHostToDevice, h->stream);
+    p += count;
+    return dst;
+  };
+  const float *dx = put(x, 2 * n), *dv = put(v, 2 * n), *dF = put(F, 4 * n), *db = put(b, 4 * n), *dm = put(mass, n), *dvol = put(vol, n);
+  const float *ds = put(scalar, n);
+  const int *dg = (const int *)put(group, n);
+  CUDA_TRY(h, cudaMemsetAsync(m->cnt.get(), 0, sizeof(int) * 4, h->stream));  // n_alive, n_live, error (updates are kept)
+  if (n > 0) {
+    k2_pack<<<m2_blocks(n, 128), 128, 0, h->stream>>>(m2_view(h), m->P, (int)n, dx, dv, dF, db, dm, dvol, ds, dg, m->id_base);
+    h->launches++;
+  }
+  m->rows = n;
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  return MPMB_OK;
+}
+
+// ---- the three stages
+static int m2_order(MpmbEngine *h) {
+  Mpm2d *m = h->m2;
+  if (m->stage != 0) return fail(h, MPMB_ERR_STATE, "stages run in the order sort, rasterize, resample");
+  const int n = (int)m->rows;
+  prof_begin(h, 0);
+  int nl = 0;
+  CUDA_TRY(h, cudaMemsetAsync(m->cell_begin.get(), 0, sizeof(int) * (size_t)m->P.ncells, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(m->cell_end.get(), 0, sizeof(int) * (size_t)m->P.ncells, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(m->cnt.get(), 0, sizeof(int), h->stream));  // n_alive
+  if (n > 0) {
+    size_t bytes = m->cub_temp.size();
+    CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(m->cub_temp.get(), bytes, m->keys.get(), m->keys_sorted.get(), m->iota.get(), m->perm.get(), n, 0,
+                                                 m->key_bits, h->stream));
+    const View2 V = m2_view(h);
+    k2_permute<<<m2_blocks(n, 256), 256, 0, h->stream>>>(V, m->P, n);
+    k2_cells<<<m2_blocks(n, 256), 256, 0, h->stream>>>(V, m->P, n);
+    nl += 3;
+  }
+  h->launches += nl;
+  prof_end(h, nl);
+  CUDA_TRY(h, cudaGetLastError());
+  m->cur ^= 1;
+  m->stage = 1;
+  return MPMB_OK;
+}
+
+static int m2_rasterize(MpmbEngine *h) {
+  Mpm2d *m = h->m2;
+  if (m->stage != 1) return fail(h, MPMB_ERR_STATE, "stages run in the order sort, rasterize, resample");
+  const int n = (int)m->rows;
+  const View2 V = m2_view(h);
+  const int t0 = (m->P.nnode[0] + M2_TILE - 1) / M2_TILE, t1 = (m->P.nnode[1] + M2_TILE - 1) / M2_TILE;
+  prof_begin(h, 1);
+  k2_p2g_particles<<<m2_blocks(n, 256), 256, 0, h->stream>>>(V, m->P, n);
+  k2_grid<<<(unsigned)(t0 * t1), 256, 0, h->stream>>>(V, m->P, t1);
+  h->launches += 2;
+  prof_end(h, 2);
+  CUDA_TRY(h, cudaGetLastError());
+  m->stage = 2;
+  return MPMB_OK;
+}
+
+static int m2_resample(MpmbEngine *h) {
+  Mpm2d *m = h->m2;
+  if (m->stage != 2) return fail(h, MPMB_ERR_STATE, "stages run in the order sort, rasterize, resample");
+  const int n = (int)m->rows;
+  prof_begin(h, 2);
+  if (n > 0) k2_g2p<<<m2_blocks(n, 256), 256, 0, h->stream>>>(m2_view(h), m->P, n);
+  h->launches += n > 0;
+  prof_end(h, n > 0);
+  CUDA_TRY(h, cudaGetLastError());
+  m->stage = 0;
+  return MPMB_OK;
+}
+
+static int m2_substep_once(MpmbEngine *h) {
+  int rc;
+  if ((rc = m2_order(h)) != MPMB_OK) return rc;
+  if ((rc = m2_rasterize(h)) != MPMB_OK) return rc;
+  return m2_resample(h);
+}
+
+// Captures one substep at the current buffer parity (graph[cur]) and leaves the host state as before; any failure turns
+// graphs off for this handle, and the substeps then run from the host with the same kernels.
+static void m2_capture(MpmbEngine *h) {
+  Mpm2d *m = h->m2;
+  if (!h->cap_stream && cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking) != cudaSuccess) { h->use_graph = false; cudaGetLastError(); return; }
+  const int cur0 = m->cur;
+  const int64_t l0 = h->launches;
+  cudaStream_t user = h->stream;
+  h->stream = h->cap_stream;
+  cudaGraph_t g = nullptr;
+  cudaError_t e = cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeThreadLocal);
+  int rc = MPMB_OK;
+  if (e == cudaSuccess) {
+    rc = m2_substep_once(h);
+    e = cudaStreamEndCapture(h->cap_stream, &g);
+  }
+  h->stream = user;
+  if (e == cudaSuccess && rc == MPMB_OK && g) e = cudaGraphInstantiate(&m->graph[cur0], g, 0);
+  if (g) cudaGraphDestroy(g);
+  if (e != cudaSuccess || rc != MPMB_OK || !m->graph[cur0]) {
+    cudaGetLastError();
+    m->graph[cur0] = nullptr;
+    h->use_graph = false;
+    h->sticky_cuda = false;
+  }
+  m->graph_launches = (int)(h->launches - l0);
+  m->cur = cur0;
+  m->stage = 0;
+  h->launches = l0;
+}
+
+static int m2_substep(MpmbEngine *h, int nsub) {
+  Mpm2d *m = h->m2;
+  if (m->stage != 0) return fail(h, MPMB_ERR_STATE, "mpmb_substep runs between substeps (the stage calls left one open)");
+  for (int s = 0; s < nsub; s++) {
+    if (h->use_graph && !h->profiling && m->rows > 0) {
+      if (!m->graph[m->cur]) m2_capture(h);
+      if (m->graph[m->cur]) {
+        CUDA_TRY(h, cudaGraphLaunch(m->graph[m->cur], h->stream));
+        h->launches += m->graph_launches;
+        m->cur ^= 1;
+        continue;
+      }
+    }
+    int rc = m2_substep_once(h);
+    if (rc != MPMB_OK) return rc;
+  }
+  return MPMB_OK;
+}
+
+static int m2_synchronize(MpmbEngine *h) {
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  Counters2 c;
+  CUDA_TRY(h, cudaMemcpy(&c, h->m2->cnt.get(), sizeof(c), cudaMemcpyDeviceToHost));
+  if (c.error & DEVERR_BAD_INPUT) return fail(h, MPMB_ERR_INVALID, "uploaded particles with group outside [0,%d) or mass <= 0", MPMB_MAX_GROUPS);
+  return MPMB_OK;
+}
+
+static int m2_num_particles(MpmbEngine *h, int64_t *n) {
+  Mpm2d *m = h->m2;
+  int rc = m2_synchronize(h);
+  if (rc != MPMB_OK) return rc;
+  CUDA_TRY(h, cudaMemsetAsync(&m->cnt.get()->n_live, 0, sizeof(int), h->stream));
+  if (m->rows > 0) {
+    k2_count_live<<<m2_blocks(m->rows, 256), 256, 0, h->stream>>>(m->keys.get(), (int)m->rows, (uint32_t)m->P.ncells, m->cnt.get());
+    h->launches++;
+  }
+  int live = 0;
+  CUDA_TRY(h, cudaMemcpyAsync(&live, &m->cnt.get()->n_live, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  *n = live;
+  return MPMB_OK;
+}
+
+// The live rows of the current storage on the host, in storage order: keys, x, v, F, b, aux (staging for the downloads;
+// a download is not on the substep's path).
+struct M2Rows {
+  std::vector<uint32_t> keys;
+  std::vector<float2> x, v;
+  std::vector<float4> F, b, aux;
+  std::vector<int64_t> live;  // row indices
+};
+static int m2_read_rows(MpmbEngine *h, M2Rows *r) {
+  Mpm2d *m = h->m2;
+  int rc = m2_synchronize(h);
+  if (rc != MPMB_OK) return rc;
+  const size_t n = (size_t)m->rows;
+  r->keys.resize(n); r->x.resize(n); r->v.resize(n); r->F.resize(n); r->b.resize(n); r->aux.resize(n);
+  r->live.clear();
+  if (n == 0) return MPMB_OK;
+  const int c = m->cur;
+  CUDA_TRY(h, cudaMemcpy(r->keys.data(), m->keys.get(), sizeof(uint32_t) * n, cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(r->x.data(), m->x[c].get(), sizeof(float2) * n, cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(r->v.data(), m->v[c].get(), sizeof(float2) * n, cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(r->F.data(), m->F[c].get(), sizeof(float4) * n, cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(r->b.data(), m->b[c].get(), sizeof(float4) * n, cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(r->aux.data(), m->aux[c].get(), sizeof(float4) * n, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < n; i++)
+    if (r->keys[i] < (uint32_t)m->P.ncells) r->live.push_back((int64_t)i);
+  return MPMB_OK;
+}
+
+static uint32_t m2_bits(float f) {
+  uint32_t u;
+  memcpy(&u, &f, 4);
+  return u;
+}
+
+static int m2_download(MpmbEngine *h, int64_t cap, int64_t *n_out, uint32_t *id, float *x, float *v, float *F, float *b, float *mass, float *vol,
+                       float *scalar, int32_t *group) {
+  if (!n_out) return fail(h, MPMB_ERR_INVALID, "null n_out");
+  M2Rows r;
+  int rc = m2_read_rows(h, &r);
+  if (rc != MPMB_OK) return rc;
+  const int64_t n = (int64_t)r.live.size();
+  if (n > cap) return fail(h, MPMB_ERR_CAPACITY, "%lld live particles do not fit in %lld rows", (long long)n, (long long)cap);
+  for (int64_t k = 0; k < n; k++) {
+    const int64_t i = r.live[k];
+    const uint32_t tag = m2_bits(r.aux[i].w);
+    if (id) id[k] = tag & TAG_ID_MASK;
+    if (x) { x[2 * k] = r.x[i].x; x[2 * k + 1] = r.x[i].y; }
+    if (v) { v[2 * k] = r.v[i].x; v[2 * k + 1] = r.v[i].y; }
+    if (F) { F[4 * k] = r.F[i].x; F[4 * k + 1] = r.F[i].y; F[4 * k + 2] = r.F[i].z; F[4 * k + 3] = r.F[i].w; }
+    if (b) { b[4 * k] = r.b[i].x; b[4 * k + 1] = r.b[i].y; b[4 * k + 2] = r.b[i].z; b[4 * k + 3] = r.b[i].w; }
+    if (mass) mass[k] = r.aux[i].x;
+    if (vol) vol[k] = r.aux[i].y;
+    if (scalar) scalar[k] = r.aux[i].z;
+    if (group) group[k] = (int32_t)(tag >> TAG_ID_BITS);
+  }
+  *n_out = n;
+  return MPMB_OK;
+}
+
+// The 48-byte point records of write_partio (src/visualize.cpp:16-100) for MPM<2>: the dim loops fill x, y and v_x, v_y
+// and leave the third components 0.  In id order.
+static int m2_bgeo_points(MpmbEngine *h, int64_t id_range, void *records, int64_t cap_records, int64_t *n_out) {
+  Mpm2d *m = h->m2;
+  M2Rows r;
+  int rc = m2_read_rows(h, &r);
+  if (rc != MPMB_OK) return rc;
+  std::vector<std::pair<uint32_t, int64_t>> order;
+  order.reserve(r.live.size());
+  for (int64_t i : r.live) {
+    const uint32_t gid = m2_bits(r.aux[i].w) & TAG_ID_MASK;
+    if ((int64_t)(gid - m->id_base) >= id_range || gid < m->id_base) return fail(h, MPMB_ERR_INVALID, "particle id %u outside [id_base, id_base + id_range)", gid);
+    order.push_back({gid, i});
+  }
+  std::sort(order.begin(), order.end());
+  if ((int64_t)order.size() > cap_records) return fail(h, MPMB_ERR_CAPACITY, "%lld live particles do not fit in the %lld records provided", (long long)order.size(), (long long)cap_records);
+  auto be = [](uint32_t v) { return (v >> 24) | ((v >> 8) & 0xff00u) | ((v << 8) & 0xff0000u) | (v << 24); };
+  uint32_t *out = (uint32_t *)records;
+  for (size_t k = 0; k < order.size(); k++) {
+    const int64_t i = order[k].second;
+    uint32_t *w = out + 12 * k;
+    w[0] = be(m2_bits(r.x[i].x)); w[1] = be(m2_bits(r.x[i].y)); w[2] = 0u; w[3] = be(m2_bits(1.0f));
+    w[4] = 0u; w[5] = be(order[k].first); w[6] = be(1u); w[7] = be(1u);
+    w[8] = be(1u); w[9] = be(m2_bits(r.v[i].x)); w[10] = be(m2_bits(r.v[i].y)); w[11] = 0u;
+  }
+  *n_out = (int64_t)order.size();
+  return MPMB_OK;
+}
+
+static int m2_download_grid(MpmbEngine *h, int which, float *dense4) {
+  Mpm2d *m = h->m2;
+  if (m->stage != 2) return fail(h, MPMB_ERR_STATE, "the grid exists between rasterize and resample");
+  if (!dense4 || which < 0 || which > 1) return fail(h, MPMB_ERR_INVALID, "bad argument");
+  const size_t n = (size_t)m->P.nnode[0] * m->P.nnode[1];
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaMemcpy(dense4, m->graw.get(), sizeof(float4) * n, cudaMemcpyDeviceToHost));
+  if (which == 1) {
+    std::vector<float2> gv(n);
+    CUDA_TRY(h, cudaMemcpy(gv.data(), m->gv.get(), sizeof(float2) * n, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < n; i++) { dense4[4 * i] = gv[i].x; dense4[4 * i + 1] = gv[i].y; }
+  }
+  return MPMB_OK;
+}
+
+static int m2_set_material(MpmbEngine *h, int group, int kind, const float *params, int n_params) {
+  Mpm2d *m = h->m2;
+  m->P.mats[group].kind = kind;
+  for (int k = 0; k < 8; k++) m->P.mats[group].p[k] = k < n_params ? params[k] : 0.f;
+  m2_graph_reset(m);
+  return MPMB_OK;
+}
+
+static int m2_set_delta_t(MpmbEngine *h, float dt) {
+  Mpm2d *m = h->m2;
+  if (m->stage != 0) return fail(h, MPMB_ERR_STATE, "delta_t changes between substeps, not inside one");
+  h->cfg.dt = dt;
+  m->P.dt = dt;
+  for (int d = 0; d < 2; d++) m->P.gdt[d] = h->cfg.gravity[d] * dt;
+  m2_graph_reset(m);
+  return MPMB_OK;
+}
+
+// shapes with zero z parts only (a 2-D solid): planes n_z = 0, circles c_z = 0, rectangles lo_z = hi_z = 0
+static int m2_set_shapes(MpmbEngine *h, int n_shapes, const MpmbShape *shapes, float friction) {
+  Mpm2d *m = h->m2;
+  for (int k = 0; k < n_shapes; k++) {
+    const MpmbShape &s = shapes[k];
+    const bool flat = s.kind == MPMB_SHAPE_CUBOID ? (s.p[2] == 0.f && s.p[5] == 0.f) : s.p[2] == 0.f;
+    if (!flat) return fail(h, MPMB_ERR_INVALID, "shape %d of a 2-D level set has a z part (must be 0)", k);
+  }
+  std::vector<MpmbShape> flat(shapes, shapes + n_shapes);
+  for (auto &s : flat)  // a rectangle is the cuboid unbounded along z
+    if (s.kind == MPMB_SHAPE_CUBOID) { s.p[2] = -1e30f; s.p[5] = 1e30f; }
+  const size_t n = (size_t)m->P.nnode[0] * m->P.nnode[1];
+  CUDA_TRY(h, m->sdf4.reserve(n));
+  DevBuf<MpmbShape> d;
+  CUDA_TRY(h, d.alloc(n_shapes));
+  CUDA_TRY(h, cudaMemcpyAsync(d.get(), flat.data(), sizeof(MpmbShape) * n_shapes, cudaMemcpyHostToDevice, h->stream));
+  k2_shapes_to_sdf<<<h->num_sms * 8, 256, 0, h->stream>>>(m->P, n_shapes, d.get(), m->sdf4.get());
+  h->launches++;
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  m->P.has_sdf = 1;
+  m->P.friction = friction;
+  m2_graph_reset(m);
+  return MPMB_OK;
+}
+
+static int m2_set_planes(MpmbEngine *h, int n_planes, const float *planes4, float friction) {
+  std::vector<MpmbShape> s(n_planes);
+  for (int k = 0; k < n_planes; k++) {
+    s[k] = MpmbShape{};
+    s[k].kind = MPMB_SHAPE_PLANE;
+    for (int c = 0; c < 4; c++) s[k].p[c] = planes4[4 * k + c];
+  }
+  return m2_set_shapes(h, n_planes, s.data(), friction);
+}
+
+static int m2_set_sdf(MpmbEngine *h, const float *sdf4, float friction) {
+  Mpm2d *m = h->m2;
+  m2_graph_reset(m);
+  if (!sdf4) {
+    m->P.has_sdf = 0;
+    return MPMB_OK;
+  }
+  const size_t n = (size_t)m->P.nnode[0] * m->P.nnode[1];
+  CUDA_TRY(h, m->sdf4.reserve(n));
+  CUDA_TRY(h, cudaMemcpyAsync(m->sdf4.get(), sdf4, sizeof(float4) * n, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  m->P.has_sdf = 1;
+  m->P.friction = friction;
+  return MPMB_OK;
+}
+// ===================================================================================== end of the 2-D engine
+
+// mpmb_create of a 2-D handle (cfg->dim == 2, validated): the 2-D engine and the handle's shared parts (stream, profiling,
+// default materials, CUDA-graph switch)
+static int create_2d(MpmbEngine *h, const MpmbConfig *cfg, MpmbHandle *out) {
+  for (int g = 0; g < MPMB_MAX_GROUPS; g++) {
+    h->P.mats[g].kind = MAT_JELLY;  // JellyParticle defaults E=1e5, nu=0.3 (src/particles.cpp:383-389)
+    for (int k = 0; k < 8; k++) h->P.mats[g].p[k] = 0.f;
+    h->P.mats[g].p[0] = 1e5f / (2.f * 1.3f);
+    h->P.mats[g].p[1] = 1e5f * 0.3f / (1.3f * 0.4f);
+  }
+  h->use_graph = cfg->no_graph == 0;
+  if (cudaSetDevice(cfg->device) != cudaSuccess) { delete h; return fail(nullptr, MPMB_ERR_CUDA, "cudaSetDevice failed"); }
+  cudaDeviceProp prop;
+  cudaGetDeviceProperties(&prop, cfg->device);
+  h->num_sms = prop.multiProcessorCount;
+  int rc = m2_create(h, cfg);
+  if (rc == MPMB_OK && cfg->capacity > 0) {
+    rc = m2_alloc_rows(h, cfg->capacity);
+    if (rc != MPMB_OK) g_create_error = h->err;
+  }
+  if (rc != MPMB_OK) {
+    mpmb_destroy(h);
+    return rc;
+  }
+  *out = h;
+  return MPMB_OK;
+}
+
 extern "C" {
 
 static int read_n_store(MpmbEngine *h, int *n_store);
@@ -3448,8 +4186,16 @@ const char *mpmb_last_error(MpmbHandle h) { return h ? h->err.c_str() : g_create
 int mpmb_create(const MpmbConfig *cfg, MpmbHandle *out) {
   if (!cfg || !out) return fail(nullptr, MPMB_ERR_INVALID, "null argument");
   *out = nullptr;
-  for (int d = 0; d < 3; d++)
+  if (cfg->dim != 0 && cfg->dim != 2 && cfg->dim != 3) return fail(nullptr, MPMB_ERR_INVALID, "dim=%d: 0 or 3 (MPM<3>) or 2 (MPM<2>)", cfg->dim);
+  const bool two_d = cfg->dim == 2;
+  for (int d = 0; d < (two_d ? 2 : 3); d++)
     if (cfg->res[d] < 16 || cfg->res[d] > 4096) return fail(nullptr, MPMB_ERR_INVALID, "res[%d]=%d out of range [16,4096]", d, cfg->res[d]);
+  if (two_d && (cfg->res[2] != 0 || cfg->gravity[2] != 0.f || cfg->world > 1))
+    return fail(nullptr, MPMB_ERR_INVALID, "dim=2 needs res[2] == 0, gravity[2] == 0 and world == 1");
+  if (!two_d && (cfg->apic_damping != 0.f || cfg->rpic_damping != 0.f))
+    return fail(nullptr, MPMB_ERR_INVALID, "apic_damping / rpic_damping are supported with dim=2 only");
+  if (two_d && (!std::isfinite(cfg->apic_damping) || !std::isfinite(cfg->rpic_damping)))
+    return fail(nullptr, MPMB_ERR_INVALID, "apic_damping / rpic_damping must be finite");
   if (!(cfg->dx > 0.f) || !(cfg->dt > 0.f)) return fail(nullptr, MPMB_ERR_INVALID, "dx and dt must be positive");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -3458,6 +4204,7 @@ int mpmb_create(const MpmbConfig *cfg, MpmbHandle *out) {
   MpmbEngine *h = new MpmbEngine();
   h->cfg = *cfg;
   if (h->cfg.world <= 0) h->cfg.world = 1;
+  if (two_d) return create_2d(h, cfg, out);
   Params &P = h->P;
   for (int d = 0; d < 3; d++) {
     P.res[d] = cfg->res[d];
@@ -3545,6 +4292,7 @@ int mpmb_destroy(MpmbHandle h) {
   if (!h) return MPMB_OK;
   cudaSetDevice(h->cfg.device);
   cudaDeviceSynchronize();
+  m2_destroy(h);
   // memory is freed by the buffers' destructors (with this device current); here go the handles that are not memory
   for (int k = 0; k < 2; k++)
     for (int f = 0; f < 2; f++)
@@ -3566,6 +4314,7 @@ int mpmb_set_stream(MpmbHandle h, void *s) {
 
 int mpmb_synchronize(MpmbHandle h) {
   CHECK_HANDLE(h);
+  if (h->m2) return m2_synchronize(h);
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   Counters c;
   CUDA_TRY(h, cudaMemcpy(&c, h->cnt.get(), sizeof(c), cudaMemcpyDeviceToHost));
@@ -3582,6 +4331,7 @@ int mpmb_set_material(MpmbHandle h, int32_t group, int32_t kind, const float *pa
   if (group < 0 || group >= MPMB_MAX_GROUPS) return fail(h, MPMB_ERR_INVALID, "group %d out of range", group);
   if (kind < MPMB_MAT_LINEAR || kind > MPMB_MAT_VISCO) return fail(h, MPMB_ERR_INVALID, "unknown material kind %d", kind);
   if (n_params < 0 || n_params > MPMB_MAT_PARAMS || (n_params > 0 && !params)) return fail(h, MPMB_ERR_INVALID, "bad parameter vector");
+  if (h->m2) return m2_set_material(h, group, kind, params, n_params);
   h->P.mats[group].kind = kind;
   for (int k = 0; k < 8; k++) h->P.mats[group].p[k] = k < n_params ? params[k] : 0.f;
   graph_reset(h);
@@ -3613,6 +4363,7 @@ static bool apply_delta_t(MpmbEngine *h, float dt) {
 int mpmb_set_delta_t(MpmbHandle h, float dt) {
   CHECK_HANDLE(h);
   if (!(dt > 0.f) || !std::isfinite(dt)) return fail(h, MPMB_ERR_INVALID, "delta_t must be positive and finite");
+  if (h->m2) return m2_set_delta_t(h, dt);
   if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "delta_t changes between substeps, not inside one");
   if (!apply_delta_t(h, dt)) return MPMB_OK;
   // resident particles: the affine matrix cached for the next rasterize carries the old dt (stress * (-4 dt / dx))
@@ -3635,6 +4386,7 @@ int mpmb_set_delta_t(MpmbHandle h, float dt) {
 int mpmb_set_id_base(MpmbHandle h, int64_t base) {
   CHECK_HANDLE(h);
   if (base < 0 || base >= (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_INVALID, "id base %lld outside [0, 2^%d)", (long long)base, TAG_ID_BITS);
+  if (h->m2) { h->m2->id_base = (uint32_t)base; return MPMB_OK; }
   if ((uint32_t)base != h->id_base) graph_reset(h);   // the captured rigid kernels take id_base by value
   h->id_base = (uint32_t)base;
   return MPMB_OK;
@@ -3642,6 +4394,7 @@ int mpmb_set_id_base(MpmbHandle h, int64_t base) {
 
 int mpmb_set_sdf(MpmbHandle h, const float *sdf4, float friction) {
   CHECK_HANDLE(h);
+  if (h->m2) return m2_set_sdf(h, sdf4, friction);
   size_t n = (size_t)h->P.nnode[0] * h->P.nnode[1] * h->P.nnode[2];
   if (!sdf4) {
     h->P.has_sdf = 0;
@@ -3660,6 +4413,7 @@ int mpmb_set_sdf(MpmbHandle h, const float *sdf4, float friction) {
 int mpmb_set_planes(MpmbHandle h, int32_t n_planes, const float *planes4, float friction) {
   CHECK_HANDLE(h);
   if (n_planes <= 0 || n_planes > 64 || !planes4) return fail(h, MPMB_ERR_INVALID, "need 1..64 planes");
+  if (h->m2) return m2_set_planes(h, n_planes, planes4, friction);
   size_t n = (size_t)h->P.nnode[0] * h->P.nnode[1] * h->P.nnode[2];
   CUDA_TRY(h, h->sdf4.reserve(n));
   DevBuf<float4> d_planes;
@@ -3679,6 +4433,7 @@ int mpmb_set_levelset_shapes(MpmbHandle h, int32_t n_shapes, const MpmbShape *sh
   if (n_shapes <= 0 || n_shapes > 64 || !shapes) return fail(h, MPMB_ERR_INVALID, "need 1..64 shapes");
   for (int k = 0; k < n_shapes; k++)
     if (shapes[k].kind < MPMB_SHAPE_PLANE || shapes[k].kind > MPMB_SHAPE_CUBOID) return fail(h, MPMB_ERR_INVALID, "unknown shape kind %d", shapes[k].kind);
+  if (h->m2) return m2_set_shapes(h, n_shapes, shapes, friction);
   size_t n = (size_t)h->P.nnode[0] * h->P.nnode[1] * h->P.nnode[2];
   CUDA_TRY(h, h->sdf4.reserve(n));
   DevBuf<MpmbShape> d_shapes;
@@ -3822,6 +4577,7 @@ static int pack_fields(MpmbEngine *h, int64_t n, const float *x, const float *v,
 int mpmb_upload_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
                           const float *mass, const float *vol, const float *scalar, const int32_t *group) {
   CHECK_HANDLE(h);
+  if (h->m2) return m2_upload(h, n, x, v, F, b, mass, vol, scalar, group);
   if (n < 0 || (n > 0 && (!x || !v || !mass || !vol))) return fail(h, MPMB_ERR_INVALID, "x, v, mass, vol are required");
   if ((int64_t)h->id_base + n > (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_CAPACITY, "particle ids exceed 2^%d", TAG_ID_BITS);
   h->aos_host_pool = nullptr;
@@ -3842,6 +4598,7 @@ static int edit_allowed(MpmbEngine *h, const char *what) {
 int mpmb_append_particles(MpmbHandle h, int64_t n, const float *x, const float *v, const float *F, const float *b,
                           const float *mass, const float *vol, const float *scalar, const int32_t *group, int64_t *first_id) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (n < 0 || (n > 0 && (!x || !v || !mass || !vol))) return fail(h, MPMB_ERR_INVALID, "x, v, mass, vol are required");
   int rc = edit_allowed(h, "append");
   if (rc != MPMB_OK) return rc;
@@ -3868,6 +4625,7 @@ int mpmb_append_owned_particles(MpmbHandle h, int64_t n, const float *x, const f
                                 const float *mass, const float *vol, const float *scalar, const int32_t *group, int64_t first_id,
                                 int64_t *n_kept) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!n_kept) return fail(h, MPMB_ERR_INVALID, "null argument");
   *n_kept = 0;
   if (n < 0 || (n > 0 && (!x || !v || !mass || !vol))) return fail(h, MPMB_ERR_INVALID, "x, v, mass, vol are required");
@@ -3904,6 +4662,7 @@ int mpmb_append_owned_particles(MpmbHandle h, int64_t n, const float *x, const f
 
 int mpmb_id_end(MpmbHandle h, int64_t *id_end) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!id_end) return fail(h, MPMB_ERR_INVALID, "null argument");
   *id_end = std::max<int64_t>(h->id_end, h->id_base);
   return MPMB_OK;
@@ -3933,6 +4692,7 @@ static int delete_inside(MpmbEngine *h, int64_t *n_deleted) {
 
 int mpmb_delete_inside_levelset(MpmbHandle h, int64_t *n_deleted) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!n_deleted) return fail(h, MPMB_ERR_INVALID, "null argument");
   *n_deleted = 0;
   int rc = edit_allowed(h, "delete_inside_levelset");
@@ -3942,6 +4702,7 @@ int mpmb_delete_inside_levelset(MpmbHandle h, int64_t *n_deleted) {
 
 int mpmb_delete_owned_inside_levelset(MpmbHandle h, int64_t *n_deleted) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!n_deleted) return fail(h, MPMB_ERR_INVALID, "null argument");
   *n_deleted = 0;
   if (h->stage != 0 || h->rigid_pending) return fail(h, MPMB_ERR_STATE, "delete_owned_inside_levelset runs between substeps, not inside one");
@@ -3994,6 +4755,7 @@ static int aos_reserve(MpmbEngine *h, size_t pool_bytes, size_t n_idx) {
 int mpmb_upload_aos(MpmbHandle h, int64_t n, const void *pool, int64_t pool_slots, const uint32_t *indices,
                     const MpmbAosLayout *L, const int32_t *group) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (n < 0 || !pool || !indices || !L || L->stride <= 0) return fail(h, MPMB_ERR_INVALID, "pool, indices and layout are required");
   if ((int64_t)h->id_base + n > (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_CAPACITY, "particle ids exceed 2^%d", TAG_ID_BITS);
   int rc = ensure_capacity(h, n);
@@ -4031,6 +4793,7 @@ int mpmb_upload_aos(MpmbHandle h, int64_t n, const void *pool, int64_t pool_slot
 int mpmb_seed_lattice(MpmbHandle h, const int32_t lo_cell[3], const int32_t hi_cell[3], float vol, float mass, float jitter, uint32_t seed,
                       int32_t group, const float v0[3], int64_t *n_seeded) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!lo_cell || !hi_cell) return fail(h, MPMB_ERR_INVALID, "null argument");
   if (group < 0 || group >= MPMB_MAX_GROUPS || !(mass > 0.f) || !(vol > 0.f)) return fail(h, MPMB_ERR_INVALID, "bad group, mass or volume");
   SeedBox B{};
@@ -4089,6 +4852,7 @@ int mpmb_num_particles(MpmbHandle h, int64_t *n) {
   CHECK_HANDLE(h);
   if (!n) return fail(h, MPMB_ERR_INVALID, "null argument");
   *n = 0;
+  if (h->m2) return m2_num_particles(h, n);
   if (h->cap == 0) return MPMB_OK;
   CUDA_TRY(h, cudaMemsetAsync(&h->cnt.get()->n_live, 0, sizeof(int), h->stream));
   k_count_live<<<h->num_sms * 4, 256, 0, h->stream>>>(h->keys[h->cur].get(), h->special_min, h->cnt.get());
@@ -4106,6 +4870,12 @@ int mpmb_get_update_count(MpmbHandle h, int64_t *updates) {
   if (!updates) return fail(h, MPMB_ERR_INVALID, "null argument");
   int rc = mpmb_synchronize(h);
   if (rc != MPMB_OK) return rc;
+  if (h->m2) {
+    unsigned long long u = 0;
+    CUDA_TRY(h, cudaMemcpy(&u, &h->m2->cnt.get()->updates, sizeof(u), cudaMemcpyDeviceToHost));
+    *updates = (int64_t)u;
+    return MPMB_OK;
+  }
   unsigned long long u = 0;
   CUDA_TRY(h, cudaMemcpy(&u, &h->cnt.get()->updates, sizeof(u), cudaMemcpyDeviceToHost));
   *updates = (int64_t)u;
@@ -4133,6 +4903,7 @@ static void unpack_live(MpmbEngine *h, int n, uint32_t *id, float *x, float *v, 
 int mpmb_download_particles(MpmbHandle h, int64_t cap, int64_t *n_out, uint32_t *id, float *x, float *v, float *F, float *b,
                             float *mass, float *vol, float *scalar, int32_t *group) {
   CHECK_HANDLE(h);
+  if (h->m2) return m2_download(h, cap, n_out, id, x, v, F, b, mass, vol, scalar, group);
   if (!n_out) return fail(h, MPMB_ERR_INVALID, "n_out is required");
   int rc = mpmb_synchronize(h);
   if (rc != MPMB_OK) return rc;
@@ -4172,6 +4943,7 @@ int mpmb_download_particles(MpmbHandle h, int64_t cap, int64_t *n_out, uint32_t 
 int mpmb_download_aos(MpmbHandle h, void *pool, int64_t pool_slots, uint32_t *indices, int64_t n_indices, const MpmbAosLayout *L,
                       int64_t *n_alive) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!pool || !indices || !L || !n_alive || L->stride <= 0 || n_indices < 0) return fail(h, MPMB_ERR_INVALID, "null argument");
   int ns = 0, rc;
   if ((rc = mpmb_synchronize(h)) != MPMB_OK) return rc;
@@ -4219,6 +4991,7 @@ int mpmb_download_aos(MpmbHandle h, void *pool, int64_t pool_slots, uint32_t *in
 int mpmb_download_bgeo_points(MpmbHandle h, int64_t id_range, void *records, int64_t cap_records, int64_t *n_out) {
   CHECK_HANDLE(h);
   if (!records || !n_out || id_range <= 0) return fail(h, MPMB_ERR_INVALID, "bad argument");
+  if (h->m2) return m2_bgeo_points(h, id_range, records, cap_records, n_out);
   int ns = 0, rc;
   if ((rc = mpmb_synchronize(h)) != MPMB_OK) return rc;
   if ((rc = read_n_store(h, &ns)) != MPMB_OK) return rc;
@@ -4278,6 +5051,7 @@ static int rigid_prepare(MpmbEngine *h, const View &V, int *nl) {
 
 int mpmb_set_rigid_samples(MpmbHandle h, int32_t n_bodies, int64_t n_samples, const float *offset3, const float *tri9, const int32_t *rigid_id) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "rigid samples change between substeps, not inside one");
   if (n_samples == 0) { h->rigid_on = false; h->motion_on = false; graph_reset(h); return MPMB_OK; }
   if (n_bodies < 2 || n_bodies > RIGID_MAX || n_samples < 0 || n_samples > (1 << 24) || !offset3 || !tri9 || !rigid_id)
@@ -4341,6 +5115,7 @@ int mpmb_set_rigid_samples(MpmbHandle h, int32_t n_bodies, int64_t n_samples, co
 
 int mpmb_set_rigid_coupling(MpmbHandle h, float penalty, float pushing_force) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   h->penalty = penalty;
   h->pushing_force = pushing_force;
   graph_reset(h);   // both are kernel arguments
@@ -4349,6 +5124,7 @@ int mpmb_set_rigid_coupling(MpmbHandle h, float penalty, float pushing_force) {
 
 int mpmb_set_rigid_state(MpmbHandle h, int32_t n_bodies, const MpmbRigidBody *bodies) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies: call mpmb_set_rigid_samples first");
   if (n_bodies != h->rigid_bodies || !bodies) return fail(h, MPMB_ERR_INVALID, "expected %d bodies", h->rigid_bodies);
   if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "z-slab rank: the bodies change after the impulse reduction, not before it");
@@ -4377,6 +5153,7 @@ int mpmb_set_rigid_state(MpmbHandle h, int32_t n_bodies, const MpmbRigidBody *bo
 
 int mpmb_get_rigid_state(MpmbHandle h, int32_t n_bodies, MpmbRigidBody *bodies) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies");
   if (n_bodies != h->rigid_bodies || !bodies) return fail(h, MPMB_ERR_INVALID, "expected %d bodies", h->rigid_bodies);
   RigidDev dev[RIGID_MAX];
@@ -4396,6 +5173,7 @@ int mpmb_get_rigid_state(MpmbHandle h, int32_t n_bodies, MpmbRigidBody *bodies) 
 
 int mpmb_set_rigid_motion(MpmbHandle h, int32_t n_bodies, const MpmbRigidMotion *motion, int32_t levelset_collision) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (n_bodies == 0) { h->motion_on = false; graph_reset(h); return MPMB_OK; }
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies: call mpmb_set_rigid_samples first");
   if (h->stage != 0 || h->rigid_pending) return fail(h, MPMB_ERR_STATE, "rigid motion changes between substeps, not inside one");
@@ -4439,6 +5217,7 @@ int mpmb_set_rigid_motion(MpmbHandle h, int32_t n_bodies, const MpmbRigidMotion 
 
 int mpmb_set_rigid_script(MpmbHandle h, int32_t n_substeps, const double *poses) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!h->rigid_on || !h->motion_on) return fail(h, MPMB_ERR_STATE, "no device-advanced bodies: call mpmb_set_rigid_motion first");
   if (h->stage != 0 || h->rigid_pending) return fail(h, MPMB_ERR_STATE, "the script changes between substeps, not inside one");
   if (n_substeps < 0 || (n_substeps > 0 && !poses)) return fail(h, MPMB_ERR_INVALID, "need n_substeps >= 0 and a table");
@@ -4479,6 +5258,7 @@ static void launch_rigid_motion(MpmbEngine *h) {
 
 int mpmb_set_particle_states(MpmbHandle h, int64_t n, const uint32_t *states) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies");
   if (n < 0 || (n > 0 && !states)) return fail(h, MPMB_ERR_INVALID, "bad argument");
   int rc = rigid_reserve_ids(h, std::max<int64_t>(n, h->cap));
@@ -4490,6 +5270,7 @@ int mpmb_set_particle_states(MpmbHandle h, int64_t n, const uint32_t *states) {
 
 int mpmb_get_particle_cdf(MpmbHandle h, int64_t n, uint32_t *states, float *normal3, float *distance, uint8_t *near_boundary) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!h->rigid_on || !h->p_states.get()) return fail(h, MPMB_ERR_STATE, "no rigid bodies / no substep yet");
   if (n < 0 || n > (int64_t)h->p_states.size()) return fail(h, MPMB_ERR_INVALID, "n exceeds the %d particle ids tracked", (int)h->p_states.size());
   std::vector<float4> cdf((size_t)n);
@@ -4511,6 +5292,7 @@ int mpmb_get_particle_cdf(MpmbHandle h, int64_t n, uint32_t *states, float *norm
 
 int mpmb_download_cdf(MpmbHandle h, uint32_t *node_states, float *node_distance) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (!h->rigid_on) return fail(h, MPMB_ERR_STATE, "no rigid bodies");
   const size_t nn = h->node_key.size();
   std::vector<unsigned long long> key(nn);
@@ -4534,6 +5316,7 @@ int mpmb_download_cdf(MpmbHandle h, uint32_t *node_states, float *node_distance)
 // ------------------------------------------------------------------------------ stages
 int mpmb_sort_particles_and_populate_grid(MpmbHandle h) {
   CHECK_HANDLE(h);
+  if (h->m2) return m2_order(h);
   if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "sort must follow resample/upload");
   if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "z-slab rank: the G2P rigid impulses of the last substep have not been reduced");
   prof_begin(h, 0);
@@ -4566,6 +5349,7 @@ int mpmb_sort_particles_and_populate_grid(MpmbHandle h) {
 
 int mpmb_rasterize(MpmbHandle h) {
   CHECK_HANDLE(h);
+  if (h->m2) return m2_rasterize(h);
   if (h->stage != 1) return fail(h, MPMB_ERR_STATE, "rasterize must follow sort_particles_and_populate_grid");
   prof_begin(h, 1);
   View V = make_view(h);
@@ -4601,6 +5385,7 @@ static void launch_g2p(MpmbEngine *h, const View &V, int part, int commit, bool 
 
 int mpmb_resample(MpmbHandle h) {
   CHECK_HANDLE(h);
+  if (h->m2) return m2_resample(h);
   if (h->stage != 2) return fail(h, MPMB_ERR_STATE, "resample must follow rasterize");
   if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "z-slab rank: reduce the P2G rigid impulses over the ranks before the resample");
   const bool motion = h->rigid_on && h->motion_on;
@@ -4647,6 +5432,7 @@ int mpmb_migrate_recv(MpmbHandle h, int32_t face);
 // rest (part 2), so that the host can put the halo exchange between them (include/mpmb.h).
 int mpmb_rasterize_part(MpmbHandle h, int32_t part) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (part != 1 && part != 2) return fail(h, MPMB_ERR_INVALID, "part must be 1 (boundary) or 2 (interior)");
   if (!((part == 1 && h->stage == 1) || (part == 2 && h->stage == 11))) return fail(h, MPMB_ERR_STATE, "rasterize_part: boundary first, then interior, after sort");
   prof_begin(h, 1);
@@ -4667,6 +5453,7 @@ int mpmb_rasterize_part(MpmbHandle h, int32_t part) {
 
 int mpmb_resample_part(MpmbHandle h, int32_t part) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (part != 1 && part != 2) return fail(h, MPMB_ERR_INVALID, "part must be 1 (boundary) or 2 (interior)");
   if (!((part == 2 && h->stage == 2) || (part == 1 && h->stage == 22))) return fail(h, MPMB_ERR_STATE, "resample_part: interior first, then boundary, after rasterize");
   if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "z-slab rank: reduce the P2G rigid impulses over the ranks before the resample");
@@ -4758,6 +5545,7 @@ static int graph_capture_pair(MpmbEngine *h, bool peers) {
 
 int mpmb_substep(MpmbHandle h, int32_t nsub) {
   CHECK_HANDLE(h);
+  if (h->m2) return m2_substep(h, nsub);
   const bool peers = peers_connected(h);
   if (h->cfg.world > 1 && !peers) return fail(h, MPMB_ERR_STATE, "z-slab run: connect the peers (mpmb_xchg_connect) or drive the stages and move the buffers yourself");
   if (h->cfg.world > 1 && h->rigid_on && !rigid_connected(h))
@@ -4795,6 +5583,7 @@ int mpmb_substep(MpmbHandle h, int32_t nsub) {
 
 int mpmb_download_grid(MpmbHandle h, int32_t which, float *dense4) {
   CHECK_HANDLE(h);
+  if (h->m2) return m2_download_grid(h, which, dense4);
   if (h->stage != 2) return fail(h, MPMB_ERR_STATE, "the grid exists between rasterize and resample");
   if (!dense4 || which < 0 || which > 1) return fail(h, MPMB_ERR_INVALID, "bad argument");
   size_t n = (size_t)h->P.nnode[0] * h->P.nnode[1] * h->P.nnode[2];
@@ -4880,6 +5669,15 @@ int mpmb_get_counters(MpmbHandle h, int64_t *active_tiles, int64_t *alive, int64
   CHECK_HANDLE(h);
   int rc = mpmb_synchronize(h);
   if (rc != MPMB_OK) return rc;
+  if (h->m2) {   // 2-D: the node tiles of the grid kernel, the live particles of the last ordering
+    Counters2 c2;
+    CUDA_TRY(h, cudaMemcpy(&c2, h->m2->cnt.get(), sizeof(c2), cudaMemcpyDeviceToHost));
+    const Params2 &P2 = h->m2->P;
+    if (active_tiles) *active_tiles = (int64_t)((P2.nnode[0] + M2_TILE - 1) / M2_TILE) * ((P2.nnode[1] + M2_TILE - 1) / M2_TILE);
+    if (alive) *alive = c2.n_alive;
+    if (kernel_launches) *kernel_launches = h->launches;
+    return MPMB_OK;
+  }
   Counters c;
   CUDA_TRY(h, cudaMemcpy(&c, h->cnt.get(), sizeof(c), cudaMemcpyDeviceToHost));
   if (active_tiles) *active_tiles = c.n_tiles;
@@ -4891,6 +5689,7 @@ int mpmb_get_counters(MpmbHandle h, int64_t *active_tiles, int64_t *alive, int64
 // rows of the current storage, movers waiting for the next ordering (= holes of their old runs), ghost tiles
 int mpmb_get_ordering_stats(MpmbHandle h, int64_t *rows, int64_t *movers, int64_t *ghost_tiles) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = mpmb_synchronize(h);
   if (rc != MPMB_OK) return rc;
   Counters c;
@@ -4909,12 +5708,14 @@ static int64_t halo_cap_xy(MpmbEngine *h) {
 static int64_t halo_idx_bytes(MpmbEngine *h) { return (halo_cap_xy(h) * 4 + 15) / 16 * 16; }
 
 int64_t mpmb_halo_bytes(MpmbHandle h) {
+  if (h && h->m2) return fail(h, MPMB_ERR_STATE, "%s is not available on a 2-D handle (dim = 2)", __func__);
   if (!h || h->cfg.world <= 1) return 0;
   return 16 + halo_idx_bytes(h) + halo_cap_xy(h) * ARENA * (int64_t)sizeof(float4);
 }
 
 int mpmb_halo_pack(MpmbHandle h, int32_t face, void *dev_buf) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1) return fail(h, MPMB_ERR_STATE, "halo exchange needs world > 1");
   if (h->stage != 2 && h->stage != 11) return fail(h, MPMB_ERR_STATE, "halo_pack must follow rasterize (or its boundary part)");
   if (!dev_buf || face < 0 || face > 1) return fail(h, MPMB_ERR_INVALID, "bad argument");
@@ -4933,6 +5734,7 @@ int mpmb_halo_pack(MpmbHandle h, int32_t face, void *dev_buf) {
 
 int mpmb_halo_unpack(MpmbHandle h, int32_t face, const void *dev_buf) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1) return fail(h, MPMB_ERR_STATE, "halo exchange needs world > 1");
   if (h->stage != 2 && h->stage != 22) return fail(h, MPMB_ERR_STATE, "halo_unpack must follow rasterize (and may follow the interior resample)");
   if (!dev_buf || face < 0 || face > 1) return fail(h, MPMB_ERR_INVALID, "bad argument");
@@ -4951,12 +5753,14 @@ int mpmb_halo_unpack(MpmbHandle h, int32_t face, const void *dev_buf) {
 }
 
 int64_t mpmb_migrate_bytes(MpmbHandle h) {
+  if (h && h->m2) return fail(h, MPMB_ERR_STATE, "%s is not available on a 2-D handle (dim = 2)", __func__);
   if (!h || h->cfg.world <= 1) return 0;
   return 16 + h->mig_cap * N_Q * (int64_t)sizeof(float4);
 }
 
 int mpmb_migrate_pack(MpmbHandle h, int32_t face, void *dev_buf) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1) return fail(h, MPMB_ERR_STATE, "migration needs world > 1");
   if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "migrate_pack must follow resample");
   if (!dev_buf || face < 0 || face > 1) return fail(h, MPMB_ERR_INVALID, "bad argument");
@@ -4974,6 +5778,7 @@ int mpmb_migrate_pack(MpmbHandle h, int32_t face, void *dev_buf) {
 
 int mpmb_migrate_unpack(MpmbHandle h, int32_t face, const void *dev_buf) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1) return fail(h, MPMB_ERR_STATE, "migration needs world > 1");
   if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "migrate_unpack must follow resample");
   if (!dev_buf || face < 0 || face > 1) return fail(h, MPMB_ERR_INVALID, "bad argument");
@@ -4992,6 +5797,7 @@ int mpmb_migrate_unpack(MpmbHandle h, int32_t face, const void *dev_buf) {
 // ------------------------------------------------------------------------------ peer-memory exchange
 int mpmb_xchg_buffer(MpmbHandle h, int32_t kind, int32_t face, void **dev_ptr) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1 || kind < 0 || kind > 1 || face < 0 || face > 1 || !dev_ptr) return fail(h, MPMB_ERR_INVALID, "bad argument");
   *dev_ptr = h->rx[kind][face].get();
   return MPMB_OK;
@@ -4999,6 +5805,7 @@ int mpmb_xchg_buffer(MpmbHandle h, int32_t kind, int32_t face, void **dev_ptr) {
 
 int mpmb_xchg_ipc_handle(MpmbHandle h, int32_t kind, int32_t face, void *out64) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1 || kind < 0 || kind > 1 || face < 0 || face > 1 || !out64) return fail(h, MPMB_ERR_INVALID, "bad argument");
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
   cudaIpcMemHandle_t hd;
@@ -5011,6 +5818,7 @@ int mpmb_xchg_ipc_handle(MpmbHandle h, int32_t kind, int32_t face, void *out64) 
 // either that buffer's IPC handle (another process) or its device pointer (same process).
 int mpmb_xchg_connect(MpmbHandle h, int32_t kind, int32_t face, const void *handle64, void *same_process_ptr) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1 || kind < 0 || kind > 1 || face < 0 || face > 1) return fail(h, MPMB_ERR_INVALID, "bad argument");
   if (same_process_ptr) {
     h->tx[kind][face] = (char *)same_process_ptr;
@@ -5116,6 +5924,7 @@ static int xchg_migrate_fused(MpmbEngine *h) {
 // the same steps one face at a time, for hosts that drive the stages themselves (same kernels, one-face masks)
 int mpmb_halo_send(MpmbHandle h, int32_t face) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1 || face < 0 || face > 1 || !h->tx[0][face]) return fail(h, MPMB_ERR_STATE, "no connected peer through face %d", face);
   if (h->stage != 2) return fail(h, MPMB_ERR_STATE, "halo_send must follow rasterize");
   return xchg_halo_launch(h, 1 << face, 0);
@@ -5123,6 +5932,7 @@ int mpmb_halo_send(MpmbHandle h, int32_t face) {
 
 int mpmb_halo_recv(MpmbHandle h, int32_t face) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1 || face < 0 || face > 1 || !h->tx[0][face]) return fail(h, MPMB_ERR_STATE, "no connected peer through face %d", face);
   if (h->stage != 2) return fail(h, MPMB_ERR_STATE, "halo_recv must follow rasterize");
   return xchg_halo_launch(h, 0, 1 << face);
@@ -5130,6 +5940,7 @@ int mpmb_halo_recv(MpmbHandle h, int32_t face) {
 
 int mpmb_migrate_send(MpmbHandle h, int32_t face) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1 || face < 0 || face > 1 || !h->tx[1][face]) return fail(h, MPMB_ERR_STATE, "no connected peer through face %d", face);
   if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "migrate_send must follow resample");
   return xchg_migrate_launch(h, 1 << face, 0);
@@ -5137,6 +5948,7 @@ int mpmb_migrate_send(MpmbHandle h, int32_t face) {
 
 int mpmb_migrate_recv(MpmbHandle h, int32_t face) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1 || face < 0 || face > 1 || !h->tx[1][face]) return fail(h, MPMB_ERR_STATE, "no connected peer through face %d", face);
   if (h->stage != 0) return fail(h, MPMB_ERR_STATE, "migrate_recv must follow resample");
   return xchg_migrate_launch(h, 0, 1 << face);
@@ -5173,12 +5985,14 @@ static int rigid_mail_recv(MpmbEngine *h) {
 }
 
 int64_t mpmb_rigid_impulse_bytes(MpmbHandle h) {
+  if (h && h->m2) return fail(h, MPMB_ERR_STATE, "%s is not available on a 2-D handle (dim = 2)", __func__);
   if (!h || h->cfg.world <= 1) return 0;
   return (int64_t)sizeof(float) * RIGID_IMPULSE_FLOATS;
 }
 
 int mpmb_rigid_impulse_pack(MpmbHandle h, void *dev_buf) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = rigid_reduce_allowed(h, "rigid_impulse_pack");
   if (rc != MPMB_OK) return rc;
   if (!dev_buf) return fail(h, MPMB_ERR_INVALID, "null buffer");
@@ -5190,6 +6004,7 @@ int mpmb_rigid_impulse_pack(MpmbHandle h, void *dev_buf) {
 
 int mpmb_rigid_impulse_apply(MpmbHandle h, const void *dev_all) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = rigid_reduce_allowed(h, "rigid_impulse_apply");
   if (rc != MPMB_OK) return rc;
   if (!dev_all) return fail(h, MPMB_ERR_INVALID, "null buffer");
@@ -5200,6 +6015,7 @@ int mpmb_rigid_impulse_apply(MpmbHandle h, const void *dev_all) {
 
 int mpmb_rigid_mailbox(MpmbHandle h, void **dev_ptr) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1 || !dev_ptr) return fail(h, MPMB_ERR_INVALID, "bad argument");
   *dev_ptr = h->rmail.get();
   return MPMB_OK;
@@ -5207,6 +6023,7 @@ int mpmb_rigid_mailbox(MpmbHandle h, void **dev_ptr) {
 
 int mpmb_rigid_mailbox_ipc_handle(MpmbHandle h, void *out64) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1 || !out64) return fail(h, MPMB_ERR_INVALID, "bad argument");
   cudaIpcMemHandle_t hd;
   CUDA_TRY(h, cudaIpcGetMemHandle(&hd, h->rmail.get()));
@@ -5216,6 +6033,7 @@ int mpmb_rigid_mailbox_ipc_handle(MpmbHandle h, void *out64) {
 
 int mpmb_rigid_connect(MpmbHandle h, int32_t rank, const void *handle64, void *same_process_ptr) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   if (h->cfg.world <= 1 || rank < 0 || rank >= h->cfg.world || rank == h->cfg.rank) return fail(h, MPMB_ERR_INVALID, "bad rank %d", rank);
   if (h->rigid_pending) return fail(h, MPMB_ERR_STATE, "rigid mailboxes connect between substeps");
   if (h->rmail_ipc[rank] && h->rmail_tx[rank]) cudaIpcCloseMemHandle(h->rmail_tx[rank]);
@@ -5239,6 +6057,7 @@ int mpmb_rigid_connect(MpmbHandle h, int32_t rank, const void *handle64, void *s
 
 int mpmb_rigid_send(MpmbHandle h) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = rigid_reduce_allowed(h, "rigid_send");
   if (rc != MPMB_OK) return rc;
   if (!rigid_connected(h)) return fail(h, MPMB_ERR_STATE, "rigid_send: connect every rank's mailbox first (mpmb_rigid_connect)");
@@ -5250,6 +6069,7 @@ int mpmb_rigid_send(MpmbHandle h) {
 
 int mpmb_rigid_recv(MpmbHandle h) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = rigid_reduce_allowed(h, "rigid_recv");
   if (rc != MPMB_OK) return rc;
   if (!h->rigid_sent) return fail(h, MPMB_ERR_STATE, "rigid_recv follows rigid_send");
@@ -5289,6 +6109,7 @@ static int layer_hist(MpmbEngine *h, int64_t *counts) {
 
 int mpmb_layer_counts(MpmbHandle h, int32_t n_layers, int64_t *counts) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = recut_allowed(h, "layer_counts");
   if (rc != MPMB_OK) return rc;
   if (!counts) return fail(h, MPMB_ERR_INVALID, "null argument");
@@ -5298,6 +6119,7 @@ int mpmb_layer_counts(MpmbHandle h, int32_t n_layers, int64_t *counts) {
 
 int mpmb_recut_pack(MpmbHandle h, const int32_t *cuts, void *dev_buf, int64_t cap_rows, int64_t *counts) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = recut_allowed(h, "recut_pack");
   if (rc != MPMB_OK) return rc;
   const int world = h->cfg.world, nl = h->nt2_global;
@@ -5338,6 +6160,7 @@ int mpmb_recut_pack(MpmbHandle h, const int32_t *cuts, void *dev_buf, int64_t ca
 
 int mpmb_recut_apply(MpmbHandle h, int32_t tile_z0, int32_t tile_z1, int64_t n_in, const void *dev_records) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = recut_allowed(h, "recut_apply");
   if (rc != MPMB_OK) return rc;
   if (tile_z0 < 0 || tile_z1 > h->nt2_global || tile_z0 >= tile_z1)
@@ -5466,6 +6289,7 @@ extern "C" {
 
 int mpmb_async_init(MpmbHandle h, const int32_t nb[3], float inv_dx) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = async_check(h, false);
   if (rc != MPMB_OK) return rc;
   if (!nb) return fail(h, MPMB_ERR_INVALID, "null argument");
@@ -5509,6 +6333,7 @@ int mpmb_async_init(MpmbHandle h, const int32_t nb[3], float inv_dx) {
 int mpmb_async_add(MpmbHandle h, int32_t which, int64_t n, const float *x, const float *v, const float *F, const float *b, const float *mass,
                    const float *vol, const float *scalar, const int32_t *group, const uint32_t *id) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = async_check(h, true);
   if (rc != MPMB_OK) return rc;
   if (which < 0 || which > 1) return fail(h, MPMB_ERR_INVALID, "which = %d: 0 (particle pool) or 1 (backup pool)", which);
@@ -5537,6 +6362,7 @@ int mpmb_async_add(MpmbHandle h, int32_t which, int64_t n, const float *x, const
 
 int mpmb_async_block_limits(MpmbHandle h, int32_t with_limits, int64_t cap, int64_t *n_blocks, int32_t *block, float *min_dt, float *max_v2) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = async_check(h, true);
   if (rc != MPMB_OK) return rc;
   if (!n_blocks || (cap > 0 && !block) || (with_limits && cap > 0 && (!min_dt || !max_v2))) return fail(h, MPMB_ERR_INVALID, "null argument");
@@ -5696,6 +6522,7 @@ extern "C" {
 
 int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_gathered) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = async_check(h, true);
   if (rc != MPMB_OK) return rc;
   if (!flags || !n_gathered) return fail(h, MPMB_ERR_INVALID, "null argument");
@@ -5710,6 +6537,7 @@ int mpmb_async_advance(MpmbHandle h, const uint8_t *flags, float dt, int64_t *n_
 int mpmb_async_schedule(MpmbHandle h, int64_t t, float strength_mul, float cfl_mul, float dx, float inv_unit, int64_t max_units, int32_t *min_level,
                         int32_t *max_level) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = async_check(h, true);
   if (rc != MPMB_OK) return rc;
   if (!min_level || !max_level) return fail(h, MPMB_ERR_INVALID, "null argument");
@@ -5742,6 +6570,7 @@ int mpmb_async_schedule(MpmbHandle h, int64_t t, float strength_mul, float cfl_m
 
 int mpmb_async_advance_level(MpmbHandle h, int64_t t, int32_t limit, float dt, int64_t *n_gathered) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = async_check(h, true);
   if (rc != MPMB_OK) return rc;
   if (!n_gathered) return fail(h, MPMB_ERR_INVALID, "null argument");
@@ -5764,6 +6593,7 @@ int mpmb_async_advance_level(MpmbHandle h, int64_t t, int32_t limit, float dt, i
 
 int mpmb_async_block_state(MpmbHandle h, int32_t *level, int64_t *local_min, int64_t *particle_t, int64_t *backup_t) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = async_check(h, true);
   if (rc != MPMB_OK) return rc;
   const size_t n = (size_t)h->nblk;
@@ -5777,6 +6607,7 @@ int mpmb_async_block_state(MpmbHandle h, int32_t *level, int64_t *local_min, int
 
 int mpmb_async_size(MpmbHandle h, int64_t *n_pool, int64_t *n_backup) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = async_check(h, true);
   if (rc != MPMB_OK) return rc;
   if (n_pool) *n_pool = h->apool[0].n;
@@ -5787,6 +6618,7 @@ int mpmb_async_size(MpmbHandle h, int64_t *n_pool, int64_t *n_backup) {
 int mpmb_async_download(MpmbHandle h, int32_t which, int64_t cap, int64_t *n_out, uint32_t *id, int32_t *block, float *x, float *v, float *F,
                         float *b, float *mass, float *vol, float *scalar, int32_t *group) {
   CHECK_HANDLE(h);
+  NOT_2D(h);
   int rc = async_check(h, true);
   if (rc != MPMB_OK) return rc;
   if (which < 0 || which > 1) return fail(h, MPMB_ERR_INVALID, "which = %d: 0 (particle pool) or 1 (backup pool)", which);

@@ -15,6 +15,12 @@ reference tree by scripts/async/async_mpm.py:17-300) and the `MPM<3>` plugin beh
 Everything numerical happens in libmpmb.so (capi.Engine); this file is glue: kwargs -> MpmbConfig,
 registered particle type names -> material groups, level-set planes -> the engine's dense SDF.
 Only the fast path of the reference is mirrored (optimized=True, static level set); rigid bodies are advanced on the device.
+
+MPM2D(res=(r0, r1), ...) is the same surface on the MPM<2> engine (capi.Engine2D; MPM itself keeps refusing a 2-D res): positions and velocities are 2-vectors, gravity defaults to
+(0, -10), add_particles(benchmark_block=...) seeds 4 particles per cell, apic_damping / rpic_damping are honoured, and level
+sets take planes, circles (add_sphere) and rectangles (add_cuboid) with 2-vectors.  Rigid bodies, AsyncMPM, z-slabs, dynamic
+level sets and delete_particles_inside_level_set are MPM<3> only and raise ValueError.  Particles added between steps take a
+host round trip; their ids are kept.
 """
 import os
 
@@ -43,6 +49,20 @@ def frame_attributes(p, group_kinds, verbose=False):
     return bgeo.reference_attributes(p, verbose=verbose, debug_code=debug)
 
 
+def _pad3(a):
+    """[n, 2] -> [n, 3] with a zero third column."""
+    a = np.asarray(a, np.float32)
+    return np.concatenate([a, np.zeros((len(a), 1), np.float32)], 1)
+
+
+def _pad3x3(b):
+    """[n, 4] column-major 2x2 -> [n, 9] column-major 3x3, zero third row and column."""
+    b = np.asarray(b, np.float32).reshape(-1, 2, 2)
+    out = np.zeros((len(b), 3, 3), np.float32)
+    out[:, :2, :2] = b
+    return out.reshape(-1, 9)
+
+
 class LevelSet:
     """Static level set made of half-spaces (tc.core LevelSet3D.add_plane / set_friction as used by
     scripts/mls-cpic/sand_sweep.py:13-19).  World units: phi(x) = n.x + d, inside is phi>0."""
@@ -55,18 +75,25 @@ class LevelSet:
         self.friction = 0.0
         self.dense = None
 
+    def _vec(self, v):
+        """A point or direction of this level set's dimension, as the 3-vector the engine takes (z = 0 in 2-D)."""
+        v = [float(c) for c in v]
+        if len(v) != len(self.res):
+            raise ValueError("a %d-D level set takes %d-vectors, got %r" % (len(self.res), len(self.res), v))
+        return v + [0.0] * (3 - len(v))
+
     def add_plane(self, normal, d):
-        n = np.asarray(normal, np.float64)
+        n = np.asarray(self._vec(normal), np.float64)
         n = n / np.linalg.norm(n)
         self.planes.append((n[0], n[1], n[2], float(d)))
 
     def add_sphere(self, center, radius, inside_out=False):
-        """tc LevelSet3D.add_sphere (scripts/mls-cpic/sand_stir.py:9)."""
-        self.shapes.append((capi.SHAPE_SPHERE, bool(inside_out), [float(c) for c in center] + [float(radius)]))
+        """tc LevelSet3D.add_sphere (scripts/mls-cpic/sand_stir.py:9); a circle in 2-D."""
+        self.shapes.append((capi.SHAPE_SPHERE, bool(inside_out), self._vec(center) + [float(radius)]))
 
     def add_cuboid(self, lower, upper, inside_out=False):
-        """tc LevelSet3D.add_cuboid (scripts/async/sand.py:35)."""
-        self.shapes.append((capi.SHAPE_CUBOID, bool(inside_out), [float(c) for c in lower] + [float(c) for c in upper]))
+        """tc LevelSet3D.add_cuboid (scripts/async/sand.py:35); a rectangle in 2-D."""
+        self.shapes.append((capi.SHAPE_CUBOID, bool(inside_out), self._vec(lower) + self._vec(upper)))
 
     def set_friction(self, f):
         self.friction = float(f)
@@ -92,7 +119,7 @@ class LevelSet:
         sh = self.shapes_grid_units()
         if not sh:
             return np.full(tuple(r + 1 for r in self.res), 1e30, np.float32)
-        return scenes.shapes_sdf(self.res, sh)[..., 3]
+        return (scenes.shapes_sdf2d if len(self.res) == 2 else scenes.shapes_sdf)(self.res, sh)[..., 3]
 
     def sample(self, X):
         """phi at positions X (grid units), trilinear in the node values — LevelSet::sample as
@@ -113,29 +140,38 @@ class LevelSet:
 
 
 class MPM:
-    """Mirror of `tc.dynamics.MPM(**kwargs)` for 3D scenes on the accelerated path."""
+    """Mirror of `tc.dynamics.MPM(**kwargs)` for 3D scenes (MPM<3>) on the accelerated path; MPM2D is the same surface for 2D
+    scenes (MPM<2>)."""
+
+    DIM = 3
 
     PARTICLE_TYPES = capi.MATERIAL_BY_NAME  # registered names, src/particles.cpp:845-856
 
     def __init__(self, **kwargs):
         res = kwargs["res"]
-        if len(res) != 3:
-            raise ValueError("the accelerated path is MPM<3>; 2D scenes run on the CPU reference")
+        if len(res) != self.DIM:
+            raise ValueError("%s takes a %d-D res; %s" % (type(self).__name__, self.DIM, "2-D scenes run with MPM2D(res=(r0, r1), ...)"
+                                                                  if len(res) == 2 else "3-D scenes run with MPM(res=(r0, r1, r2), ...)"))
         self.res = tuple(int(r) for r in res)
+        self.dim = len(self.res)
         self.delta_x = float(kwargs.get("delta_x", 1.0 / self.res[0]))          # async_mpm.py:40-41
         # the reference's clocks are `real` = float (src/mpm.h:100, src/mpm.cpp:42-43,428-450,573): carried as float32 so
         # that a frame runs exactly the reference's number of substeps
         self.base_delta_t = float(np.float32(np.float32(kwargs.get("base_delta_t", 1e-4)) * np.float32(kwargs.get("dt_multiplier", 1.0))))
-        g = kwargs.get("gravity", (0.0, -10.0, 0.0))                            # mpm.cpp:38
+        g = kwargs.get("gravity", (0.0, -10.0, 0.0)[: self.dim])               # mpm.cpp:38: Vector::axis(1) * -10
         if np.isscalar(g):
-            g = (0.0, float(g), 0.0)
+            g = (0.0, float(g), 0.0)[: self.dim]
         self.gravity = tuple(float(x) for x in g)
+        if len(self.gravity) != self.dim:
+            raise ValueError("gravity must have %d components" % self.dim)
         self.frame_dt = float(kwargs.get("frame_dt", 0.01))
         self.particle_gravity = bool(kwargs.get("particle_gravity", True))      # mpm.cpp:47
         self.clean_boundary = bool(kwargs.get("clean_boundary", True))          # mpm.cpp:563
         if not kwargs.get("optimized", True):
             raise ValueError("optimized=False (the scalar transfers) is not accelerated")
-        for key in ("apic_damping", "rpic_damping", "affine_damping"):
+        # MPM<2>'s resample damps apic_b with apic_damping / rpic_damping (src/mpm.h:465-469); MPM<3>'s optimized resample
+        # does not damp the matrix (it passes a block index), and affine_damping is not read by either transfer
+        for key in (("apic_damping", "rpic_damping", "affine_damping") if self.dim == 3 else ("affine_damping",)):
             if float(kwargs.get(key, 0.0)) != 0.0:
                 raise ValueError("%s != 0 is outside the accelerated fast path" % key)
         self.penalty = float(kwargs.get("penalty", 0.0))                        # mpm.cpp:35: rigid-coupled scenes only
@@ -144,8 +180,13 @@ class MPM:
         self.rigids = []          # HostRigidBody per add_particles(type='rigid'); engine body id = index + 1 (rigids[0] of the
         self._rigid_dirty = False  # reference is the background body, mpm.cpp:72-74)
         self._rigid_seen = None   # body states at the last read-back (a difference is a user edit, pushed before the next step)
-        self.engine = capi.Engine(self.res, self.delta_x, self.base_delta_t, self.gravity, self.particle_gravity,
-                                  self.clean_boundary, device=int(kwargs.get("device", 0)), capacity=int(kwargs.get("capacity", 0)))
+        if self.dim == 2:
+            self.engine = capi.Engine2D(self.res, self.delta_x, self.base_delta_t, self.gravity, self.particle_gravity, self.clean_boundary,
+                                        device=int(kwargs.get("device", 0)), capacity=int(kwargs.get("capacity", 0)),
+                                        apic_damping=float(kwargs.get("apic_damping", 0.0)), rpic_damping=float(kwargs.get("rpic_damping", 0.0)))
+        else:
+            self.engine = capi.Engine(self.res, self.delta_x, self.base_delta_t, self.gravity, self.particle_gravity,
+                                      self.clean_boundary, device=int(kwargs.get("device", 0)), capacity=int(kwargs.get("capacity", 0)))
         self.current_t = np.float32(0.0)
         self.request_t = np.float32(0.0)
         self._update_counter = 0   # "Times of particle updating" (mpm.cpp:436,449): summed on the device, read lazily
@@ -160,6 +201,10 @@ class MPM:
         self._n_uploaded = 0
         self._id_base = 0         # the engine's id base (set by 'load')
         self._id_span = 0         # ids handed out since the last upload: [id_base, id_base + _id_span)
+        # 2-D: the engine numbers an upload 0..n-1, so the ids a user sees are kept here: _ids[engine id], increasing
+        self._ids = np.zeros(0, np.int64)
+        self._host_ids = None     # ids of the pending host set
+        self._next_id = 0
 
     # ---- level set
     def create_levelset(self):
@@ -196,6 +241,8 @@ class MPM:
         reference type (E, nu, youngs_modulus, friction_angle, ...) are honoured."""
         name = kwargs["type"]
         if name == "rigid":
+            if self.dim == 2:
+                raise ValueError("2-D rigid bodies (segment meshes, CPIC) are not accelerated")
             return self.add_rigid_particle(**kwargs)
         if name not in self.PARTICLE_TYPES:
             raise ValueError("unknown particle type %r" % name)
@@ -205,19 +252,35 @@ class MPM:
         density = float(kwargs.get("density", 400.0))                           # mpm.cpp:135
         if "benchmark_block" in kwargs:
             lo, hi = kwargs["benchmark_block"]
-            x, mass, vol = scenes.lattice_block(self.res[0], lo, hi, density, kwargs.get("jitter", 0.0), dx=self.delta_x)
+            if self.dim == 2:   # this project's 2-D lattice: the reference's benchmark branch is 3-D only (mpm.cpp:152)
+                x, mass, vol = scenes.lattice_block2d(self.res, lo, hi, density, kwargs.get("jitter", 0.0), dx=self.delta_x,
+                                                      maximum=float(kwargs.get("maximum", 4.0)))
+            else:
+                x, mass, vol = scenes.lattice_block(self.res[0], lo, hi, density, kwargs.get("jitter", 0.0), dx=self.delta_x)
         else:
-            x = np.ascontiguousarray(kwargs["positions"], np.float32).reshape(-1, 3)
-            ppc = float(kwargs.get("maximum", 8.0))
-            vol = np.full(len(x), self.delta_x ** 3 / ppc, np.float32)          # mpm.cpp:134
+            x = np.ascontiguousarray(kwargs["positions"], np.float32).reshape(-1, self.dim)
+            ppc = float(kwargs.get("maximum", 8.0 if self.dim == 3 else 4.0))
+            vol = np.full(len(x), self.delta_x ** self.dim / ppc, np.float32)   # mpm.cpp:134
             mass = (vol * density).astype(np.float32)
         # near_boundary particles are ignored (mpm.cpp:129-132)
         X = x / np.float32(self.delta_x)
         keep = (X.min(1) >= 7.0) & ((X - np.asarray(self.res, np.float32)).max(1) <= -7.0)
         x, mass, vol = x[keep], mass[keep], vol[keep]
-        st = scenes.make_state(x, mass, vol, kind, group, kwargs.get("initial_velocity", (0.0, 0.0, 0.0)))
+        if self.dim == 2:
+            st = scenes.make_state2d(x, mass, vol, kind, group, kwargs.get("initial_velocity", (0.0, 0.0)))
+        else:
+            st = scenes.make_state(x, mass, vol, kind, group, kwargs.get("initial_velocity", (0.0, 0.0, 0.0)))
         if kind == scenes.MAT_VISCO and "tau" in kwargs:                         # visco_tau, src/particles.cpp:62
             st["ps"][:] = np.float32(kwargs["tau"])
+        if self.dim == 2:   # a host round trip that keeps every id: the new particles are numbered after all ids so far
+            cur = self._pull_host()
+            new_ids = np.arange(self._next_id, self._next_id + len(x), dtype=np.int64)
+            self._next_id += len(x)
+            st.pop("alive")
+            self._host = st if cur is None else {k: np.concatenate([cur[k], st[k]]) for k in st}
+            self._host_ids = new_ids if cur is None else np.concatenate([self._host_ids, new_ids])
+            self._dirty = True
+            return ""
         if self._host is None and self._n_uploaded > 0 and hasattr(self.engine, "append"):
             # particles are resident and no host copy is pending: append on the device (mpm.cpp:147), the resident
             # particles keep their ids and state, the new ones are numbered after every id handed out so far
@@ -322,12 +385,17 @@ class MPM:
             return None
         d = self.engine.download()
         self._host = dict(x=d["x"], v=d["v"], F=d["F"], b=d["b"], mass=d["mass"], vol=d["vol"], ps=d["ps"], group=d["group"])
+        if self.dim == 2:
+            self._host_ids = self._ids[d["id"].astype(np.int64)]
         return self._host
 
     def _push(self):
         if self._dirty and self._host is not None:
             h = self._host
             self.engine.upload(h["x"], h["v"], h["mass"], h["vol"], h["F"], h["b"], h["ps"], h["group"])
+            if self.dim == 2:
+                self._ids = self._host_ids
+                self._host_ids = None
             self._n_uploaded = len(h["x"])
             self._id_span = len(h["x"])     # an upload numbers its particles id_base + 0..n-1
             self._dirty = False
@@ -389,7 +457,10 @@ class MPM:
     def get_particles(self):
         """Live particles as numpy arrays (the data visualize() writes: src/visualize.cpp:16-100)."""
         self._push()
-        return self.engine.download()
+        p = self.engine.download()
+        if self.dim == 2:
+            p["id"] = self._ids[p["id"].astype(np.int64)].astype(np.uint32)
+        return p
 
     def num_particles(self):
         self._push()
@@ -421,15 +492,24 @@ class MPM:
             # instead of the full state, and no host pass over the particles)
             self._push()
             n, block = self.engine.download_bgeo_points(self._id_range())
+            if self.dim == 2 and n:   # the index word carries the engine id: the kept ids are increasing in it, the order holds
+                w = block.view(">u4").reshape(n, 12)
+                w[:, 5] = self._ids[w[:, 5].astype(np.int64)]
             bgeo.write_bgeo_packed(fn, n, block)
             return fn
         p = self.get_particles()
+        if self.dim == 2:   # write_partio leaves the third components 0 (src/visualize.cpp:62,78,90)
+            p = dict(p, x=_pad3(p["x"]), v=_pad3(p["v"]), b=_pad3x3(p["b"]))
         bgeo.write_bgeo(fn, p["x"], frame_attributes(p, [k for k, _ in self._groups], self.verbose_bgeo))
         return fn
 
     def _id_range(self):
         # ids lie in [id_base, id_base + id span): the last upload plus every device append since
         return max(int(self._id_span), 1)
+
+    def _refuse_2d(self, what):
+        if self.dim == 2:
+            raise ValueError("%s is MPM<3> only" % what)
 
     def general_action(self, **kwargs):
         """The actions of MPM<dim>::general_action (src/mpm.cpp:920-976) that concern the accelerated
@@ -467,6 +547,7 @@ class MPM:
             self._push_with_ids(ids)
             return ""
         if action == "delete_particles_inside_level_set":                      # mpm.cpp:958-972
+            self._refuse_2d("delete_particles_inside_level_set")
             ls = getattr(self, "_levelset", None)
             if ls is not None and self._host is None and self._n_uploaded > 0 and hasattr(self.engine, "delete_inside_levelset"):
                 self.engine.delete_inside_levelset()     # on the device: the survivors keep their ids and state
@@ -522,8 +603,22 @@ class MPM:
         order = np.argsort(ids, kind="stable")
         h = {k: v[order] for k, v in h.items()}
         ids = ids[order]
+        if self.dim == 2:   # the snapshot's ids are kept as they are
+            self._host = h
+            self._host_ids = ids.astype(np.int64)
+            self._next_id = int(ids[-1]) + 1 if len(ids) else 0
+            self._push()
+            return
         base = int(ids[0]) if len(ids) and np.array_equal(ids - ids[0], np.arange(len(ids), dtype=ids.dtype)) else 0
         self.engine.set_id_base(base)
         self._id_base = base
         self._host = h
         self._push()
+
+
+class MPM2D(MPM):
+    """Mirror of `tc.dynamics.MPM(res=(r0, r1), ...)`: the same surface as MPM on the 2-D engine (capi.Engine2D, MPM<2>).
+    Positions and velocities are 2-vectors, gravity defaults to (0, -10), add_particles(benchmark_block=...) seeds 4 particles per
+    cell, apic_damping / rpic_damping are honoured and level sets take 2-vectors (planes, circles, rectangles)."""
+
+    DIM = 2

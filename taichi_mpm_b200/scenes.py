@@ -211,6 +211,57 @@ def shapes_sdf(res, shapes, dtype=np.float32):
     return out.astype(dtype)
 
 
+# ---------------------------------------------------------------------------------------------------- 2-D (MPM<2>)
+def lattice_block2d(res, lo_cell, hi_cell, density=400.0, jitter=0.0, seed=20260922, dx=None, maximum=4):
+    """The 2-D lattice of this project (the reference's `benchmark` branch is 3-D only, src/mpm.cpp:152): 4 particles
+    per cell over cells [lo_cell, hi_cell) at (cell + 0.5 +- 0.25) * dx, vol = dx^2 / maximum (the texture-seeding
+    convention vol = dx^dim / maximum, src/mpm.cpp:134-135), mass = vol * density."""
+    dx = 1.0 / res[0] if dx is None else float(dx)
+    lo, hi = np.asarray(lo_cell, np.int64), np.asarray(hi_cell, np.int64)
+    ii, jj = np.meshgrid(np.arange(lo[0], hi[0]), np.arange(lo[1], hi[1]), indexing="ij")
+    centre = np.stack([ii, jj], -1).reshape(-1, 1, 2) + 0.5
+    sign = np.array([[-1, -1], [-1, 1], [1, -1], [1, 1]], np.float64)
+    X = (centre + 0.25 * sign[None]).reshape(-1, 2)
+    if jitter > 0:
+        X = X + np.random.default_rng(seed).uniform(-jitter, jitter, X.shape)
+    x = (X * dx).astype(np.float32)
+    vol = np.full(len(x), dx * dx / maximum, np.float32)
+    return x, (vol * density).astype(np.float32), vol
+
+
+def make_state2d(x, mass, vol, kind, group=0, v0=(0.0, 0.0)):
+    n = len(x)
+    F = np.zeros((n, 4), np.float32)
+    F[:, 0] = F[:, 3] = 1.0
+    return dict(x=np.asarray(x, np.float32), v=np.tile(np.asarray(v0, np.float32), (n, 1)), F=F, b=np.zeros((n, 4), np.float32),
+                mass=np.asarray(mass, np.float32), vol=np.asarray(vol, np.float32), ps=np.full(n, default_scalar(kind), np.float32),
+                group=np.full(n, group, np.int32), alive=np.ones(n, np.uint8))
+
+
+def flat_shapes2d(shapes):
+    """2-D solids as the engine rasterises them (include/mpmb.h, dim = 2): plane (n_x, n_y, 0, d), circle (c_x, c_y, 0, r)
+    and rectangle (lo_x, lo_y, 0, hi_x, hi_y, 0); a rectangle is the cuboid that is unbounded along z."""
+    out = []
+    for kind, io, prm in shapes:
+        p = [float(v) for v in prm] + [0.0] * (6 - len(prm))
+        if (p[2] != 0.0) or (kind == 2 and p[5] != 0.0):
+            raise ValueError("a 2-D shape has no z part: %r" % (prm,))
+        if kind == 2:
+            p[2], p[5] = -1e30, 1e30
+        out.append((kind, io, p))
+    return out
+
+
+def shapes_sdf2d(res, shapes, dtype=np.float32):
+    """Numpy twin of mpmb_set_levelset_shapes on a 2-D handle: (r0+1, r1+1, 4) = (n_x, n_y, 0, phi), grid units."""
+    return shapes_sdf((int(res[0]), int(res[1]), 0), flat_shapes2d(shapes), dtype)[:, :, 0].copy()
+
+
+def planes_sdf2d(res, planes, dtype=np.float32):
+    """Numpy twin of mpmb_set_planes on a 2-D handle: planes (n_x, n_y, 0, d)."""
+    return shapes_sdf2d(res, [(0, 0, p) for p in np.asarray(planes, np.float32).reshape(-1, 4)], dtype)
+
+
 def config(name, scale=1.0, state=True):
     """The BASELINE.json configs as dict(scene=..., state=..., meta=...).
 

@@ -59,10 +59,17 @@ def slab_partition(tile_z, n_layers, world):
     return partition_counts(layer_histogram(tile_z, n_layers), world)
 
 
+def _refuse_2d(engine):
+    """z-slabs split the z axis of an MPM<3> engine; a 2-D engine (capi.Engine2D) has none."""
+    if getattr(getattr(engine, "cfg", None), "dim", 0) == 2:
+        raise ValueError("z-slab runs are MPM<3> only: a 2-D engine runs on one GPU")
+
+
 class EngineAdapter:
     """Binds torch buffers to the pointer-based exchange calls of capi.Engine."""
 
     def __init__(self, engine):
+        _refuse_2d(engine)
         self.e = engine
 
     def halo_bytes(self):
@@ -264,6 +271,7 @@ def _on_all_ranks(call, dist, op):
 
 def global_id_end(engine, dist=None):
     """The next free particle id of the run: the maximum of engine.id_end() over the ranks."""
+    _refuse_2d(engine)
     return _on_all_ranks(engine.id_end, dist, "MAX")
 
 
@@ -271,6 +279,7 @@ def share_id_end(engine, dist=None):
     """Raises this rank's id end to the run's (global_id_end) and returns it.  A z-slab rank with rigid coupling keeps the
     particles' colour states by absolute id below its id end, and an immigrant may carry any id of the run: after per-rank
     uploads (set_id_base + upload, seed_lattice) every rank must know the run's id end.  connect_peers and SlabRunner call it."""
+    _refuse_2d(engine)
     end = global_id_end(engine, dist)
     z3, z1 = np.zeros((0, 3), np.float32), np.zeros(0, np.float32)
     engine.append_owned(z3, z3, z1, z1, first_id=end)   # no particle: only the id end moves
@@ -285,6 +294,7 @@ def append_particles(engine, batch, first_id, dist=None):
     If a rank fails, every rank raises.  A rank whose configured capacity is too small raises MPMB_ERR_CAPACITY and is left
     unchanged, but the other ranks have made their part of the edit: the run is then inconsistent.  Engines created with
     capacity 0 (the default) grow instead and never fail this way."""
+    _refuse_2d(engine)
     return _on_all_ranks(lambda: engine.append_owned(batch["x"], batch["v"], batch["mass"], batch["vol"], batch.get("F"), batch.get("b"),
                                                      batch.get("ps"), batch.get("group"), first_id=first_id),
                          dist, "SUM")
@@ -292,6 +302,7 @@ def append_particles(engine, batch, first_id, dist=None):
 
 def delete_inside_levelset(engine, dist=None):
     """Removes the particles inside the level set (phi < 0) on every rank; returns the number removed over all ranks."""
+    _refuse_2d(engine)
     return _on_all_ranks(engine.delete_owned_inside_levelset, dist, "SUM")
 
 
@@ -299,6 +310,7 @@ def connect_peers(engine, rank, world, dist):
     """Maps the ring neighbours' receive buffers and every rank's rigid impulse mailbox into `engine` with CUDA IPC (one
     process per GPU): afterwards engine.substep(n) runs whole z-slab substeps, halo, migration and the rigid impulse
     reductions included, with no host transport.  Handles travel through torch.distributed once."""
+    _refuse_2d(engine)
     share_id_end(engine, dist)
     mine = {(k, f): engine.xchg_ipc_handle(k, f) for k in (0, 1) for f in (0, 1)}
     mine["rigid"] = engine.rigid_mailbox_ipc_handle()
@@ -324,6 +336,7 @@ def rebalance(engine, rank, world, dist, cuts=None):
     The bytes go through dist.all_to_all_single on device buffers (NCCL) rather than the ring neighbours' peer mappings: a
     re-cut is rare and may send particles to any rank.  Configured capacities are checked on every rank before any rank
     changes; if one is too small, every rank raises SlabEditError and nothing changes."""
+    _refuse_2d(engine)
     import torch
     from .capi import RECORD_BYTES
     dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend() == "nccl" else torch.device("cpu")
