@@ -113,7 +113,19 @@ typedef struct MpmbConfig {
 
 /* Byte offsets of the fields of one reference particle slot (ParticleContainer<3>, 320 B,
  * src/mpm_fwd.h:59-67; fields src/particles.h:24-45).  Obtained with offsetof() on the reference
- * side (INTEGRATION.md); never hard-coded here.  Offset < 0 = field absent.                       */
+ * side (INTEGRATION.md); never hard-coded here.  Offset < 0 = field absent.
+ *
+ * The plastic scalar has two modes.
+ *  - Single offset (off_scalar_by_kind all 0, the zero-initialised struct): every row's scalar is at
+ *    off_scalar.  With off_scalar = -1 the upload packs 0 for every row, snow and water included (not
+ *    the Jp = 1 / j = 1 of mpmb_upload_particles; kept as it always was), and the download writes none.
+ *  - Per kind (any off_scalar_by_kind entry != 0): the pool mixes particle types, each of which keeps
+ *    its scalar at its own offset.  off_scalar must be -1, and each entry is -1 (no scalar in the slot)
+ *    or a 4-aligned offset in (0, stride - 4]; otherwise both AoS calls return MPMB_ERR_INVALID and
+ *    change nothing.  A row's offset follows the material KIND of its group (mpmb_set_material), not
+ *    the group number: snow reads Jp, water j, sand logJp, visco visco_tau.  Rows of a kind without an
+ *    offset (linear, jelly, elastic, von Mises, or an entry of -1) get mpmb_upload_particles' defaults
+ *    (Jp = 1, j = 1, otherwise 0) and have no scalar written back.                                    */
 typedef struct MpmbAosLayout {
   int32_t stride;      /* bytes per slot (320)                                       */
   int32_t off_pos;     /* float[3]   `pos`                                           */
@@ -123,7 +135,9 @@ typedef struct MpmbAosLayout {
   int32_t col_pitch;   /* bytes between matrix columns (16)                          */
   int32_t off_vol;     /* float      `vol`                                           */
   int32_t off_scalar;  /* float      Jp / j / logJp of the subclass, or -1           */
-  int32_t reserved[4];
+  /* float  per-kind scalar: [0] SnowParticle::Jp, [1] WaterParticle::j, [2] SandParticle::logJp,
+   * [3] ViscoParticle::visco_tau; -1 = not in the slot; all 0 = single-offset mode (above)          */
+  int32_t off_scalar_by_kind[4];
 } MpmbAosLayout;
 
 /* ------------------------------------------------------------------------------ lifetime */
@@ -187,7 +201,10 @@ int mpmb_upload_particles(MpmbHandle h, int64_t n, const float *x, const float *
  * that ids stay unique after migration.  Ids must stay below 2^28.                                 */
 int mpmb_set_id_base(MpmbHandle h, int64_t base);
 /* Same, reading the reference's own AoS pool: slot indices[k] of `pool` (ParticleAllocator::pool,
- * src/particle_allocator.h:39; MPM::particles index vector, src/mpm.h:116).  group[k] may be NULL. */
+ * src/particle_allocator.h:39; MPM::particles index vector, src/mpm.h:116).  group[k] may be NULL.
+ * With per-kind scalar offsets (MpmbAosLayout) the call takes a snapshot of the 16 groups' kinds: set
+ * every group's material BEFORE the upload.  The snapshot picks each row's scalar offset here and in the
+ * next mpmb_download_aos, whatever mpmb_set_material does in between.                              */
 int mpmb_upload_aos(MpmbHandle h, int64_t n, const void *pool, int64_t pool_slots, const uint32_t *indices,
                     const MpmbAosLayout *layout, const int32_t *group);
 /* Replaces the `benchmark` branch of MPM<3>::add_particles (src/mpm.cpp:149-186: 8 particles per cell of the
@@ -263,7 +280,11 @@ int mpmb_download_particles(MpmbHandle h, int64_t cap, int64_t *n_out, uint32_t 
  * reference's 320 bytes), so bytes outside it (vptr, flags, ...) are never touched on the host.  Fields
  * inside the window that the engine does not own (e.g. boundary_normal) return as uploaded: do not
  * modify the pool between the two calls (the device owns the particles during step(), SURVEY §8b).
- * Without a preceding mpmb_upload_aos of the same pool the image is read first.                      */
+ * Without a preceding mpmb_upload_aos of the same pool the image is read first.  With per-kind scalar
+ * offsets each row's scalar goes to the offset of its group's kind as of the last mpmb_upload_aos (its
+ * snapshot), and only for kinds that have one; no other byte of any slot is written.  That mode needs an
+ * mpmb_upload_aos on the handle since the last mpmb_upload_particles / mpmb_seed_lattice (else
+ * MPMB_ERR_STATE).                                                                                  */
 int mpmb_download_aos(MpmbHandle h, void *pool, int64_t pool_slots, uint32_t *indices, int64_t n_indices,
                       const MpmbAosLayout *layout, int64_t *n_alive);
 

@@ -71,8 +71,22 @@ class MpmbAosLayout(C.Structure):
     _fields_ = [
         ("stride", C.c_int32), ("off_pos", C.c_int32), ("off_v_and_m", C.c_int32), ("off_dg_e", C.c_int32),
         ("off_apic_b", C.c_int32), ("col_pitch", C.c_int32), ("off_vol", C.c_int32), ("off_scalar", C.c_int32),
-        ("reserved", C.c_int32 * 4),
+        ("off_scalar_by_kind", C.c_int32 * 4),
     ]
+
+    # the material kinds that keep a plastic scalar, in the order of off_scalar_by_kind (snow Jp, water j, sand logJp, visco_tau)
+    SCALAR_KINDS = (2, 3, 4, 7)
+
+    def set_scalar_offsets(self, by_kind):
+        """Per-kind plastic-scalar offsets for a pool that mixes particle types: `by_kind` maps a material kind (scenes.MAT_*) to
+        the byte offset of its scalar in the slot.  Kinds left out get -1 (no scalar in the slot: the upload's default);
+        off_scalar becomes -1.  A kind without a plastic scalar is an error."""
+        bad = set(by_kind) - set(self.SCALAR_KINDS)
+        if bad:
+            raise ValueError("kinds without a plastic scalar: %s" % sorted(bad))
+        self.off_scalar = -1
+        self.off_scalar_by_kind[:] = [int(by_kind.get(k, -1)) for k in self.SCALAR_KINDS]
+        return self
 
 
 class MpmbShape(C.Structure):

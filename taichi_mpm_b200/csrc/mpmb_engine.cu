@@ -377,8 +377,17 @@ __global__ void k_owned_flags(Params P, int n, const float *x, int *flags) {
   if (i < n) flags[i] = make_key(P, x[3 * (size_t)i], x[3 * (size_t)i + 1], x[3 * (size_t)i + 2]) < (uint32_t)P.ntiles_total ? 1 : 0;
 }
 
+// Per-kind plastic scalars of a mixed AoS pool (MpmbAosLayout.off_scalar_by_kind), resolved per group on the host from the
+// group -> kind snapshot of mpmb_upload_aos: the slot offset of the group's scalar (-1: none in the slot) and the value a row
+// without one starts with.  on == 0: the single off_scalar of the layout applies.
+struct AosScalars {
+  int on;
+  int32_t off[MPMB_MAX_GROUPS];
+  float dflt[MPMB_MAX_GROUPS];
+};
+
 // Reference AoS slots (staged on the device) -> q streams.
-__global__ void k_pack_aos(View V, Params P, int n, const unsigned char *pool, const uint32_t *indices, MpmbAosLayout L,
+__global__ void k_pack_aos(View V, Params P, int n, const unsigned char *pool, const uint32_t *indices, MpmbAosLayout L, AosScalars S,
                            const int *group, uint32_t *keys, uint32_t id_base) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -396,7 +405,13 @@ __global__ void k_pack_aos(View V, Params P, int n, const unsigned char *pool, c
   }
   int g = group ? group[i] : 0;
   float vol = *(const float *)(s + L.off_vol);
-  float ps = L.off_scalar >= 0 ? *(const float *)(s + L.off_scalar) : 0.f;
+  float ps;
+  if (S.on) {
+    const int gs = min(max(g, 0), MPMB_MAX_GROUPS - 1);   // a group out of range is flagged by pack_one
+    ps = S.off[gs] >= 0 ? *(const float *)(s + S.off[gs]) : S.dflt[gs];
+  } else {
+    ps = L.off_scalar >= 0 ? *(const float *)(s + L.off_scalar) : 0.f;
+  }
   pack_one(V, P, i, id_base + (uint32_t)i, make_float3(pos[0], pos[1], pos[2]), make_float3(vm[0], vm[1], vm[2]), f, bb, vm[3], vol, ps, g, keys);
 }
 
@@ -606,7 +621,8 @@ __global__ void k_bgeo_points(View V, const uint32_t *keys, int n, uint32_t spec
 // mpmb_download_aos on the device: every live row goes back into its slot of the (device image of the) reference's
 // pool and raises the alive flag of its id; the survivors' slots, in id order, are then one stream compaction away.
 __global__ void k_aos_scatter(View V, const uint32_t *keys, int n, uint32_t special_min, unsigned char *pool, const uint32_t *indices,
-                              int64_t n_indices, int64_t pool_slots, MpmbAosLayout L, uint32_t id_base, int *alive_flag, Counters *cnt) {
+                              int64_t n_indices, int64_t pool_slots, MpmbAosLayout L, AosScalars S, uint32_t id_base, int *alive_flag,
+                              Counters *cnt) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   if (keys[i] >= special_min) return;
@@ -627,7 +643,12 @@ __global__ void k_aos_scatter(View V, const uint32_t *keys, int n, uint32_t spec
 #pragma unroll
     for (int r = 0; r < 3; r++) { fc[r] = Fm[c * 3 + r]; bc[r] = bm[c * 3 + r]; }
   }
-  if (L.off_scalar >= 0) *(float *)(sl + L.off_scalar) = q6.y;
+  if (S.on) {
+    const int32_t off = S.off[__float_as_uint(q6.w) >> TAG_ID_BITS];
+    if (off >= 0) *(float *)(sl + off) = q6.y;
+  } else if (L.off_scalar >= 0) {
+    *(float *)(sl + L.off_scalar) = q6.y;
+  }
 }
 __global__ void k_compact_survivors(const uint32_t *indices, const int *alive_flag, const int *prefix, int64_t n, uint32_t *out) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -3121,6 +3142,9 @@ struct MpmbEngine {
   DevBuf<uint32_t> aos_idx;
   const void *aos_host_pool = nullptr;  // not owned: the host pool, kept only to identify the image (with slots and particle count)
   int64_t aos_slots = 0, aos_n = 0;
+  // group -> material kind at the last mpmb_upload_aos: where per-kind scalars are read at upload and written at download
+  int32_t aos_kinds[MPMB_MAX_GROUPS] = {};
+  bool aos_kinds_valid = false;
   DevBuf<int> scan_a, scan_b;  // flags / prefix scratch (downloads, seeding)
   DevBuf<unsigned char> scan_tmp;
   uint32_t id_base = 0;
@@ -4514,6 +4538,7 @@ static int reorder_from_scratch(MpmbEngine *h, int64_t n_rows) {
 static int rigid_reserve_ids(MpmbEngine *h, int64_t n_ids);
 // A new resident set of n rows (upload, seeding): its id span, fresh rigid colours, then the ordering.
 static int finish_upload(MpmbEngine *h, int64_t n) {
+  h->aos_kinds_valid = false;   // mpmb_upload_aos takes its snapshot after this
   h->id_span = std::max<int64_t>(h->id_span_pending, n);
   h->id_span_pending = 0;
   h->id_end = (int64_t)h->id_base + h->id_span;
@@ -4742,8 +4767,37 @@ static void aos_window(const MpmbAosLayout *L, int *lo, int *hi) {
   a = std::min(a, L->off_vol);
   b = std::max(b, L->off_vol + 4);
   if (L->off_scalar >= 0) { a = std::min(a, L->off_scalar); b = std::max(b, L->off_scalar + 4); }
+  for (int k = 0; k < 4; k++)
+    if (L->off_scalar_by_kind[k] > 0) { a = std::min(a, L->off_scalar_by_kind[k]); b = std::max(b, L->off_scalar_by_kind[k] + 4); }
   *lo = std::max(0, a & ~15);
   *hi = std::min(L->stride, (b + 15) & ~15);
+}
+
+// the layout's scalar mode: per kind when any off_scalar_by_kind entry is set, checked (MpmbAosLayout in mpmb.h)
+static int aos_scalar_mode(MpmbEngine *h, const MpmbAosLayout *L, bool *per_kind) {
+  *per_kind = false;
+  for (int k = 0; k < 4; k++) *per_kind |= L->off_scalar_by_kind[k] != 0;
+  if (!*per_kind) return MPMB_OK;
+  if (L->off_scalar != -1) return fail(h, MPMB_ERR_INVALID, "per-kind scalar offsets need off_scalar = -1");
+  for (int k = 0; k < 4; k++) {
+    const int32_t o = L->off_scalar_by_kind[k];
+    if (o != -1 && (o <= 0 || o > L->stride - 4 || (o & 3)))
+      return fail(h, MPMB_ERR_INVALID, "off_scalar_by_kind[%d] = %d is not -1 or a 4-aligned offset in (0, stride - 4]", k, o);
+  }
+  return MPMB_OK;
+}
+
+// per-group scalar offsets and defaults from a group -> kind table (the snapshot of mpmb_upload_aos)
+static AosScalars aos_scalars(const MpmbAosLayout *L, const int32_t *kinds, bool per_kind) {
+  AosScalars S{};
+  S.on = per_kind ? 1 : 0;
+  for (int g = 0; g < MPMB_MAX_GROUPS; g++) {
+    const int kind = kinds[g];
+    const int k = kind == MAT_SNOW ? 0 : kind == MAT_WATER ? 1 : kind == MAT_SAND ? 2 : kind == MAT_VISCO ? 3 : -1;
+    S.off[g] = k >= 0 ? L->off_scalar_by_kind[k] : -1;
+    S.dflt[g] = (kind == MAT_SNOW || kind == MAT_WATER) ? 1.0f : 0.0f;   // as mpmb_upload_particles with scalar = NULL
+  }
+  return S;
 }
 
 static int aos_reserve(MpmbEngine *h, size_t pool_bytes, size_t n_idx) {
@@ -4758,10 +4812,19 @@ int mpmb_upload_aos(MpmbHandle h, int64_t n, const void *pool, int64_t pool_slot
   NOT_2D(h);
   if (n < 0 || !pool || !indices || !L || L->stride <= 0) return fail(h, MPMB_ERR_INVALID, "pool, indices and layout are required");
   if ((int64_t)h->id_base + n > (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_CAPACITY, "particle ids exceed 2^%d", TAG_ID_BITS);
-  int rc = ensure_capacity(h, n);
+  bool per_kind;
+  int rc = aos_scalar_mode(h, L, &per_kind);
   if (rc != MPMB_OK) return rc;
+  if ((rc = ensure_capacity(h, n)) != MPMB_OK) return rc;
   h->aos_host_pool = nullptr;
-  if (n == 0) return finish_upload(h, 0);
+  int32_t kinds[MPMB_MAX_GROUPS];
+  for (int g = 0; g < MPMB_MAX_GROUPS; g++) kinds[g] = h->P.mats[g].kind;
+  if (n == 0) {
+    if ((rc = finish_upload(h, 0)) != MPMB_OK) return rc;
+    std::copy(kinds, kinds + MPMB_MAX_GROUPS, h->aos_kinds);
+    h->aos_kinds_valid = true;
+    return MPMB_OK;
+  }
   // the pool's device image and the index vector stay resident (grow-only buffers): mpmb_download_aos scatters the
   // results into the image and returns it with one contiguous copy
   const size_t pool_bytes = (size_t)pool_slots * L->stride;
@@ -4780,14 +4843,18 @@ int mpmb_upload_aos(MpmbHandle h, int64_t n, const void *pool, int64_t pool_slot
                                   cudaMemcpyHostToDevice, h->stream));
   }
   View V = make_view(h);
-  k_pack_aos<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, h->aos_pool.get(), h->aos_idx.get(), *L, d_grp, h->keys[h->cur].get(), h->id_base);
+  k_pack_aos<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(V, h->P, (int)n, h->aos_pool.get(), h->aos_idx.get(), *L, aos_scalars(L, kinds, per_kind),
+                                                                  d_grp, h->keys[h->cur].get(), h->id_base);
   h->launches++;
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
   h->aos_host_pool = pool;
   h->aos_slots = pool_slots;
   h->aos_n = n;
-  return finish_upload(h, n);
+  if ((rc = finish_upload(h, n)) != MPMB_OK) return rc;
+  std::copy(kinds, kinds + MPMB_MAX_GROUPS, h->aos_kinds);
+  h->aos_kinds_valid = true;
+  return MPMB_OK;
 }
 
 int mpmb_seed_lattice(MpmbHandle h, const int32_t lo_cell[3], const int32_t hi_cell[3], float vol, float mass, float jitter, uint32_t seed,
@@ -4945,7 +5012,11 @@ int mpmb_download_aos(MpmbHandle h, void *pool, int64_t pool_slots, uint32_t *in
   CHECK_HANDLE(h);
   NOT_2D(h);
   if (!pool || !indices || !L || !n_alive || L->stride <= 0 || n_indices < 0) return fail(h, MPMB_ERR_INVALID, "null argument");
-  int ns = 0, rc;
+  bool per_kind;
+  int ns = 0, rc = aos_scalar_mode(h, L, &per_kind);
+  if (rc != MPMB_OK) return rc;
+  if (per_kind && !h->aos_kinds_valid)
+    return fail(h, MPMB_ERR_STATE, "per-kind scalar offsets need the group kinds of an mpmb_upload_aos of the resident set");
   if ((rc = mpmb_synchronize(h)) != MPMB_OK) return rc;
   if ((rc = read_n_store(h, &ns)) != MPMB_OK) return rc;
   *n_alive = 0;
@@ -4964,7 +5035,7 @@ int mpmb_download_aos(MpmbHandle h, void *pool, int64_t pool_slots, uint32_t *in
   if (ns > 0 && h->cap > 0) {
     View V = make_view(h);
     k_aos_scatter<<<(ns + 127) / 128, 128, 0, h->stream>>>(V, h->keys[h->cur].get(), ns, h->special_min, h->aos_pool.get(), h->aos_idx.get(), n_indices, pool_slots, *L,
-                                                           h->id_base, h->scan_a.get(), h->cnt.get());
+                                                           aos_scalars(L, h->aos_kinds, per_kind), h->id_base, h->scan_a.get(), h->cnt.get());
     h->launches++;
   }
   int alive = 0;
