@@ -99,9 +99,10 @@ typedef struct MpmbConfig {
    *   MPMB_SHAPE_CUBOID; every z part must be 0), mpmb_set_sdf, mpmb_upload_particles, mpmb_set_id_base,
    *   mpmb_num_particles, mpmb_get_update_count, mpmb_download_particles, mpmb_download_bgeo_points (z = 0, as
    *   MPM<2>::write_partio writes), mpmb_substep and its three stages, mpmb_download_grid, mpmb_set_profiling,
-   *   mpmb_get_profile, mpmb_get_counters.
-   * Every other entry point returns MPMB_ERR_STATE (the *_bytes calls included) with a message: AoS pools, lattice
-   * seeding, appends and deletions, rigid bodies, AsyncMPM, z-slabs and re-cuts are MPM<3> only.
+   *   mpmb_get_profile, mpmb_get_counters, mpmb_upload_aos and mpmb_download_aos (MPM<2>'s own pool; the 2-D meaning of
+   *   MpmbAosLayout is given there).
+   * Every other entry point returns MPMB_ERR_STATE (the *_bytes calls included) with a message: lattice seeding,
+   * appends and deletions, rigid bodies, AsyncMPM, z-slabs and re-cuts are MPM<3> only.
    * The deletion rule is the same as in 3-D with the 9-node stencil; in addition G2P clamps the position to
    * [0, res - 1e-6] cells as MPM<2>::resample does, and a particle whose velocity is not finite is deleted too.      */
   int32_t dim;
@@ -114,6 +115,13 @@ typedef struct MpmbConfig {
 /* Byte offsets of the fields of one reference particle slot (ParticleContainer<3>, 320 B,
  * src/mpm_fwd.h:59-67; fields src/particles.h:24-45).  Obtained with offsetof() on the reference
  * side (INTEGRATION.md); never hard-coded here.  Offset < 0 = field absent.
+ *
+ * On a 2-D handle (MpmbConfig.dim = 2) the same struct describes a ParticleContainer<2> slot of MPM<2>
+ * (192 B in the reference's build): pos is float[2], v_and_m float[3] = (vx, vy, mass) (v_and_m[dim]
+ * is the mass, src/particles.h:66-72), dg_e and apic_b are 2 columns of 2 floats col_pitch apart
+ * (column-major, as MatrixND<2> stores them), and vol and the scalar modes are as in 3-D.  Every field
+ * must lie inside `stride` at a 4-aligned offset, stride must be a multiple of 4 and col_pitch a multiple
+ * of 4 that is at least 8; otherwise both AoS calls return MPMB_ERR_INVALID and change nothing.
  *
  * The plastic scalar has two modes.
  *  - Single offset (off_scalar_by_kind all 0, the zero-initialised struct): every row's scalar is at
@@ -128,11 +136,12 @@ typedef struct MpmbConfig {
  *    (Jp = 1, j = 1, otherwise 0) and have no scalar written back.                                    */
 typedef struct MpmbAosLayout {
   int32_t stride;      /* bytes per slot (320)                                       */
-  int32_t off_pos;     /* float[3]   `pos`                                           */
-  int32_t off_v_and_m; /* float[4]   `v_and_m` = (vx,vy,vz,mass)                     */
-  int32_t off_dg_e;    /* 3 x float[4] padded columns of `dg_e` (column pitch below) */
-  int32_t off_apic_b;  /* 3 x float[4] padded columns of `apic_b`                    */
-  int32_t col_pitch;   /* bytes between matrix columns (16)                          */
+  int32_t off_pos;     /* float[3]   `pos`                         (2-D: float[2])     */
+  int32_t off_v_and_m; /* float[4]   `v_and_m` = (vx,vy,vz,mass)   (2-D: (vx,vy,mass)) */
+  int32_t off_dg_e;    /* 3 x float[4] padded columns of `dg_e` (column pitch below)
+                        *                                          (2-D: 2 x float[2]) */
+  int32_t off_apic_b;  /* 3 x float[4] padded columns of `apic_b`  (2-D: 2 x float[2]) */
+  int32_t col_pitch;   /* bytes between matrix columns (16)          (2-D: >= 8)         */
   int32_t off_vol;     /* float      `vol`                                           */
   int32_t off_scalar;  /* float      Jp / j / logJp of the subclass, or -1           */
   /* float  per-kind scalar: [0] SnowParticle::Jp, [1] WaterParticle::j, [2] SandParticle::logJp,
@@ -205,6 +214,8 @@ int mpmb_set_id_base(MpmbHandle h, int64_t base);
  * With per-kind scalar offsets (MpmbAosLayout) the call takes a snapshot of the 16 groups' kinds: set
  * every group's material BEFORE the upload.  The snapshot picks each row's scalar offset here and in the
  * next mpmb_download_aos, whatever mpmb_set_material does in between.                              */
+/* On a 2-D handle the rows are those mpmb_upload_particles makes of the same particles.  A slot index
+ * outside the pool returns MPMB_ERR_INVALID and leaves the resident set as it was.                  */
 int mpmb_upload_aos(MpmbHandle h, int64_t n, const void *pool, int64_t pool_slots, const uint32_t *indices,
                     const MpmbAosLayout *layout, const int32_t *group);
 /* Replaces the `benchmark` branch of MPM<3>::add_particles (src/mpm.cpp:149-186: 8 particles per cell of the
@@ -285,6 +296,8 @@ int mpmb_download_particles(MpmbHandle h, int64_t cap, int64_t *n_out, uint32_t 
  * snapshot), and only for kinds that have one; no other byte of any slot is written.  That mode needs an
  * mpmb_upload_aos on the handle since the last mpmb_upload_particles / mpmb_seed_lattice (else
  * MPMB_ERR_STATE).                                                                                  */
+/* On a 2-D handle a particle id or slot index outside the vectors returns MPMB_ERR_INVALID before any
+ * byte of the host pool or of `indices` is written.                                                   */
 int mpmb_download_aos(MpmbHandle h, void *pool, int64_t pool_slots, uint32_t *indices, int64_t n_indices,
                       const MpmbAosLayout *layout, int64_t *n_alive);
 

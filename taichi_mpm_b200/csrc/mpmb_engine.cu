@@ -93,7 +93,8 @@ struct Counters {  // device-resident
 #else
 #define MPMB_CHK(cnt, cond, site, a, b, c) true
 #endif
-enum { DEVERR_TILE_CAPACITY = 1, DEVERR_MIGRATE_CAPACITY = 2, DEVERR_PARTICLE_CAPACITY = 4, DEVERR_PEER_TIMEOUT = 8, DEVERR_BAD_INPUT = 16 };
+enum { DEVERR_TILE_CAPACITY = 1, DEVERR_MIGRATE_CAPACITY = 2, DEVERR_PARTICLE_CAPACITY = 4, DEVERR_PEER_TIMEOUT = 8, DEVERR_BAD_INPUT = 16,
+       DEVERR_BAD_SLOT = 32 };   // BAD_SLOT: a 2-D AoS call met an id or slot index outside its vectors (Counters2::aos_error)
 
 // Tile-scheduling trace (-DMPMB_TILE_TRACE, read by bench_tail.py through mpmb_debug_tile_trace): every CTA of k_p2g
 // and k_g2p records when it started and ended (%globaltimer, ns), its SM and the tiles and particle rows it
@@ -3505,7 +3506,7 @@ struct Counters2 {
   int n_alive;  // live rows after the last ordering
   int n_live;   // scratch of mpmb_num_particles
   int error;
-  int pad;
+  int aos_error;  // error bits of the running mpmb_upload_aos / mpmb_download_aos: that call reports them and changes nothing
   unsigned long long updates;
 };
 
@@ -3554,6 +3555,71 @@ __global__ void k2_pack(View2 V, Params2 P, int n, const float *x, const float *
   V.b[i] = b ? make_float4(b[4 * (size_t)i], b[4 * (size_t)i + 1], b[4 * (size_t)i + 2], b[4 * (size_t)i + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
   V.aux[i] = make_float4(m, vol[i], ps, __uint_as_float(((uint32_t)g << TAG_ID_BITS) | (id0 + (uint32_t)i)));
   V.keys[i] = cell_key2(P, xx);
+}
+
+// ---------------------------------------------------------------- AoS pools
+// mpmb_upload_aos: slot indices[k] of the device image of the reference's pool (MPMParticle<2>: pos float[2], v_and_m
+// float[3] = (vx, vy, mass), dg_e and apic_b as two columns of two floats col_pitch apart) -> row k, the row k2_pack makes
+// of the same particle given field-wise.  The rows go to the spare buffers and the keys to keys_sorted; the host keeps them
+// only when no slot lies outside the pool.  Every error bit goes to cnt->aos_error.
+__global__ void k2_pack_aos(View2 V, Params2 P, int n, const unsigned char *pool, int64_t pool_slots, const uint32_t *indices, MpmbAosLayout L,
+                            AosScalars S, const int *group, uint32_t id0) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t slot = indices[i];
+  if ((int64_t)slot >= pool_slots) { atomicOr(&V.cnt->aos_error, DEVERR_BAD_SLOT); return; }
+  const unsigned char *s = pool + (size_t)slot * L.stride;
+  const float *pos = (const float *)(s + L.off_pos), *vm = (const float *)(s + L.off_v_and_m);
+  const float *f0 = (const float *)(s + L.off_dg_e), *f1 = (const float *)(s + L.off_dg_e + L.col_pitch);
+  const float *b0 = (const float *)(s + L.off_apic_b), *b1 = (const float *)(s + L.off_apic_b + L.col_pitch);
+  int g = group ? group[i] : 0;
+  float m = vm[2];
+  if (g < 0 || g >= MPMB_MAX_GROUPS || !(m > 0.f)) {
+    atomicOr(&V.cnt->aos_error, DEVERR_BAD_INPUT);
+    g = min(max(g, 0), MPMB_MAX_GROUPS - 1);
+    m = 1e-30f;
+  }
+  float ps;
+  if (S.on) ps = S.off[g] >= 0 ? *(const float *)(s + S.off[g]) : S.dflt[g];
+  else ps = L.off_scalar >= 0 ? *(const float *)(s + L.off_scalar) : 0.f;
+  const float2 xx = make_float2(pos[0], pos[1]);
+  V.xn[i] = xx;
+  V.vn[i] = make_float2(vm[0], vm[1]);
+  V.Fn[i] = make_float4(f0[0], f0[1], f1[0], f1[1]);
+  V.bn[i] = make_float4(b0[0], b0[1], b1[0], b1[1]);
+  V.auxn[i] = make_float4(m, *(const float *)(s + L.off_vol), ps, __uint_as_float(((uint32_t)g << TAG_ID_BITS) | (id0 + (uint32_t)i)));
+  V.keys_sorted[i] = cell_key2(P, xx);
+}
+
+// mpmb_download_aos: every live row back into its slot of the device image (slot = indices[id - id_base]) and the alive
+// flag of its id; the survivors' slots in id order are then one stream compaction away (k_compact_survivors).  Dead rows
+// write nothing.  An id or slot outside the vectors sets DEVERR_BAD_SLOT in cnt->aos_error and writes nothing.
+__global__ void k2_aos_scatter(View2 V, Params2 P, int n, unsigned char *pool, const uint32_t *indices, int64_t n_indices, int64_t pool_slots,
+                               MpmbAosLayout L, AosScalars S, uint32_t id_base, int *alive_flag) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || V.keys[i] >= (uint32_t)P.ncells) return;
+  const float4 aux = V.aux[i];
+  const uint32_t tag = __float_as_uint(aux.w), id = (tag & TAG_ID_MASK) - id_base;
+  if ((int64_t)id >= n_indices) { atomicOr(&V.cnt->aos_error, DEVERR_BAD_SLOT); return; }
+  const uint32_t slot = indices[id];
+  if ((int64_t)slot >= pool_slots) { atomicOr(&V.cnt->aos_error, DEVERR_BAD_SLOT); return; }
+  alive_flag[id] = 1;
+  const float2 x = V.x[i], v = V.v[i];
+  const float4 F = V.F[i], b = V.b[i];
+  unsigned char *sl = pool + (size_t)slot * L.stride;
+  float *pos = (float *)(sl + L.off_pos), *vm = (float *)(sl + L.off_v_and_m);
+  float *f0 = (float *)(sl + L.off_dg_e), *f1 = (float *)(sl + L.off_dg_e + L.col_pitch);
+  float *b0 = (float *)(sl + L.off_apic_b), *b1 = (float *)(sl + L.off_apic_b + L.col_pitch);
+  pos[0] = x.x; pos[1] = x.y;
+  vm[0] = v.x; vm[1] = v.y; vm[2] = aux.x;
+  f0[0] = F.x; f0[1] = F.y; f1[0] = F.z; f1[1] = F.w;
+  b0[0] = b.x; b0[1] = b.y; b1[0] = b.z; b1[1] = b.w;
+  if (S.on) {
+    const int32_t off = S.off[tag >> TAG_ID_BITS];
+    if (off >= 0) *(float *)(sl + off) = aux.z;
+  } else if (L.off_scalar >= 0) {
+    *(float *)(sl + L.off_scalar) = aux.z;
+  }
 }
 
 // ---------------------------------------------------------------- ordering
@@ -3838,6 +3904,8 @@ static int m2_upload(MpmbEngine *h, int64_t n, const float *x, const float *v, c
   if (h->cfg.capacity > 0 && n > m->cap) return fail(h, MPMB_ERR_CAPACITY, "%lld particles exceed the configured capacity %lld", (long long)n, (long long)m->cap);
   if (n > m->cap) { int rc = m2_alloc_rows(h, n); if (rc != MPMB_OK) return rc; }
   m2_graph_reset(m);
+  h->aos_host_pool = nullptr;   // the resident set is no longer the AoS pool's (mpmb_download_aos needs a new upload)
+  h->aos_kinds_valid = false;
   const size_t words = (size_t)n * (2 + 2 + (F ? 4 : 0) + (b ? 4 : 0) + 1 + 1 + (scalar ? 1 : 0) + (group ? 1 : 0));
   CUDA_TRY(h, m->stage_buf.reserve(std::max<size_t>(words, 1)));
   float *p = m->stage_buf.get();
@@ -4759,11 +4827,12 @@ static int scan_flags(MpmbEngine *h, size_t n, int *total, const int *word, int 
 }
 
 // byte range [lo, hi) of a slot that the layout's fields occupy: only that window of every slot crosses the bus (a 2-D
-// copy with the slot stride as pitch) — 204 of the reference's 320 bytes
-static void aos_window(const MpmbAosLayout *L, int *lo, int *hi) {
-  const int mat = 2 * L->col_pitch + 12;  // three padded columns, the last one 3 floats long
+// copy with the slot stride as pitch) — 204 of the reference's 320 bytes.  dim 3: pos float[3], v_and_m float[4], three
+// columns of three floats; dim 2: pos float[2], v_and_m float[3], two columns of two floats.
+static void aos_window(const MpmbAosLayout *L, int dim, int *lo, int *hi) {
+  const int mat = (dim - 1) * L->col_pitch + 4 * dim;  // padded columns, the last one dim floats long
   int a = std::min(std::min(L->off_pos, L->off_v_and_m), std::min(L->off_dg_e, L->off_apic_b));
-  int b = std::max(std::max(L->off_pos + 12, L->off_v_and_m + 16), std::max(L->off_dg_e + mat, L->off_apic_b + mat));
+  int b = std::max(std::max(L->off_pos + 4 * dim, L->off_v_and_m + 4 * (dim + 1)), std::max(L->off_dg_e + mat, L->off_apic_b + mat));
   a = std::min(a, L->off_vol);
   b = std::max(b, L->off_vol + 4);
   if (L->off_scalar >= 0) { a = std::min(a, L->off_scalar); b = std::max(b, L->off_scalar + 4); }
@@ -4806,10 +4875,142 @@ static int aos_reserve(MpmbEngine *h, size_t pool_bytes, size_t n_idx) {
   return MPMB_OK;
 }
 
+// ---- the AoS calls of a 2-D handle (kernels k2_pack_aos / k2_aos_scatter in the 2-D engine's section)
+// MpmbAosLayout against MPMParticle<2>'s extents: every field inside the slot, 4-aligned (the kernels read floats)
+static int m2_aos_layout_check(MpmbEngine *h, const MpmbAosLayout *L, bool *per_kind) {
+  const int32_t st = L->stride, cp = L->col_pitch;
+  if (st <= 0 || (st & 3)) return fail(h, MPMB_ERR_INVALID, "2-D handle: layout stride %d is not a positive multiple of 4", st);
+  if (cp < 8 || (cp & 3)) return fail(h, MPMB_ERR_INVALID, "2-D handle: col_pitch %d is not a multiple of 4 >= 8", cp);
+  const int32_t off[5] = {L->off_pos, L->off_v_and_m, L->off_dg_e, L->off_apic_b, L->off_vol};
+  const int32_t len[5] = {8, 12, cp + 8, cp + 8, 4};
+  static const char *name[5] = {"off_pos", "off_v_and_m", "off_dg_e", "off_apic_b", "off_vol"};
+  for (int k = 0; k < 5; k++)
+    if (off[k] < 0 || (off[k] & 3) || off[k] > st - len[k])
+      return fail(h, MPMB_ERR_INVALID, "2-D handle: %s = %d with %d bytes is not a 4-aligned field inside the %d-byte slot", name[k], off[k], len[k], st);
+  if (L->off_scalar != -1 && (L->off_scalar < 0 || (L->off_scalar & 3) || L->off_scalar > st - 4))
+    return fail(h, MPMB_ERR_INVALID, "2-D handle: off_scalar = %d is not -1 or a 4-aligned offset inside the slot", L->off_scalar);
+  return aos_scalar_mode(h, L, per_kind);
+}
+
+static int m2_upload_aos(MpmbEngine *h, int64_t n, const void *pool, int64_t pool_slots, const uint32_t *indices, const MpmbAosLayout *L,
+                         const int32_t *group) {
+  Mpm2d *m = h->m2;
+  if (n < 0 || !pool || !indices || !L || pool_slots < 0) return fail(h, MPMB_ERR_INVALID, "2-D handle: pool, indices and layout are required");
+  bool per_kind;
+  int rc = m2_aos_layout_check(h, L, &per_kind);
+  if (rc != MPMB_OK) return rc;
+  if ((int64_t)m->id_base + n > (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_CAPACITY, "particle ids exceed 2^%d", TAG_ID_BITS);
+  if (m->stage != 0) return fail(h, MPMB_ERR_STATE, "upload between substeps, not inside one");
+  if (h->cfg.capacity > 0 && n > m->cap) return fail(h, MPMB_ERR_CAPACITY, "%lld particles exceed the configured capacity %lld", (long long)n, (long long)m->cap);
+  if (n > m->cap) {
+    if ((rc = m2_alloc_rows(h, n)) != MPMB_OK) return rc;
+    m->rows = 0;   // the new storage holds nothing yet
+  }
+  h->aos_host_pool = nullptr;   // the device image is rewritten below
+  int32_t kinds[MPMB_MAX_GROUPS];
+  for (int g = 0; g < MPMB_MAX_GROUPS; g++) kinds[g] = m->P.mats[g].kind;
+  const size_t pool_bytes = (size_t)pool_slots * L->stride;
+  if (n > 0 && (rc = aos_reserve(h, pool_bytes, (size_t)n)) != MPMB_OK) return rc;
+  CUDA_TRY(h, cudaMemsetAsync(&m->cnt.get()->aos_error, 0, sizeof(int), h->stream));
+  if (n > 0) {
+    const int *d_grp = nullptr;
+    if (group) {
+      CUDA_TRY(h, m->stage_buf.reserve((size_t)n));
+      d_grp = (const int *)m->stage_buf.get();
+      CUDA_TRY(h, cudaMemcpyAsync(m->stage_buf.get(), group, sizeof(int32_t) * n, cudaMemcpyHostToDevice, h->stream));
+    }
+    CUDA_TRY(h, cudaMemcpyAsync(h->aos_idx.get(), indices, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, h->stream));
+    if (pool_slots > 0) {
+      int lo, hi;
+      aos_window(L, 2, &lo, &hi);
+      CUDA_TRY(h, cudaMemcpy2DAsync(h->aos_pool.get() + lo, (size_t)L->stride, (const char *)pool + lo, (size_t)L->stride, (size_t)(hi - lo),
+                                    (size_t)pool_slots, cudaMemcpyHostToDevice, h->stream));
+    }
+    k2_pack_aos<<<m2_blocks(n, 128), 128, 0, h->stream>>>(m2_view(h), m->P, (int)n, h->aos_pool.get(), pool_slots, h->aos_idx.get(), *L,
+                                                           aos_scalars(L, kinds, per_kind), d_grp, m->id_base);
+    h->launches++;
+  }
+  int err = 0;
+  CUDA_TRY(h, cudaMemcpyAsync(&err, &m->cnt.get()->aos_error, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  if (err & DEVERR_BAD_SLOT)   // the packed rows are in the spare buffers: the resident set stays as it was
+    return fail(h, MPMB_ERR_INVALID, "2-D handle: a slot index is outside the pool of %lld slots", (long long)pool_slots);
+  // keep the new rows: the spare buffers become the current ones and keys_sorted the keys; the counters restart as after
+  // mpmb_upload_particles, with a bad group or mass reported by the next synchronize
+  m2_graph_reset(m);
+  m->cur ^= 1;
+  std::swap(m->keys, m->keys_sorted);
+  m->rows = n;
+  const int c3[3] = {0, 0, err & DEVERR_BAD_INPUT};   // n_alive, n_live, error
+  CUDA_TRY(h, cudaMemcpy(m->cnt.get(), c3, sizeof(c3), cudaMemcpyHostToDevice));
+  if (n > 0) {
+    h->aos_host_pool = pool;
+    h->aos_slots = pool_slots;
+    h->aos_n = n;
+  }
+  std::copy(kinds, kinds + MPMB_MAX_GROUPS, h->aos_kinds);
+  h->aos_kinds_valid = true;
+  return MPMB_OK;
+}
+
+static int m2_download_aos(MpmbEngine *h, void *pool, int64_t pool_slots, uint32_t *indices, int64_t n_indices, const MpmbAosLayout *L,
+                           int64_t *n_alive) {
+  Mpm2d *m = h->m2;
+  if (!pool || !indices || !L || !n_alive || n_indices < 0 || pool_slots < 0)
+    return fail(h, MPMB_ERR_INVALID, "2-D handle: pool, indices, layout and n_alive are required");
+  bool per_kind;
+  int rc = m2_aos_layout_check(h, L, &per_kind);
+  if (rc != MPMB_OK) return rc;
+  if (per_kind && !h->aos_kinds_valid)
+    return fail(h, MPMB_ERR_STATE, "per-kind scalar offsets need the group kinds of an mpmb_upload_aos of the resident set");
+  if ((rc = m2_synchronize(h)) != MPMB_OK) return rc;
+  *n_alive = 0;
+  if (n_indices == 0) return MPMB_OK;
+  if (m->cap < n_indices) return fail(h, MPMB_ERR_CAPACITY, "index vector longer than the particle capacity");
+  // the device image of the pool: still resident from mpmb_upload_aos of the same pool, else brought in now
+  const bool resident = h->aos_host_pool == pool && h->aos_slots == pool_slots && h->aos_n == n_indices && h->aos_pool.get();
+  h->aos_host_pool = nullptr;   // the image is written below: the next download reads the host pool again
+  if (!resident) {
+    if ((rc = aos_reserve(h, (size_t)pool_slots * L->stride, (size_t)n_indices)) != MPMB_OK) return rc;
+    CUDA_TRY(h, cudaMemcpyAsync(h->aos_idx.get(), indices, sizeof(uint32_t) * n_indices, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->aos_pool.get(), pool, (size_t)pool_slots * L->stride, cudaMemcpyHostToDevice, h->stream));
+  }
+  if ((rc = scan_reserve(h, (size_t)n_indices + 1)) != MPMB_OK) return rc;   // + 1: the room for aos_error behind the total
+  CUDA_TRY(h, cudaMemsetAsync(h->scan_a.get(), 0, sizeof(int) * (size_t)n_indices, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(&m->cnt.get()->aos_error, 0, sizeof(int), h->stream));
+  if (m->rows > 0) {
+    k2_aos_scatter<<<m2_blocks(m->rows, 128), 128, 0, h->stream>>>(m2_view(h), m->P, (int)m->rows, h->aos_pool.get(), h->aos_idx.get(), n_indices,
+                                                                    pool_slots, *L, aos_scalars(L, h->aos_kinds, per_kind), m->id_base, h->scan_a.get());
+    h->launches++;
+  }
+  int alive = 0, err = 0;
+  if ((rc = scan_flags(h, (size_t)n_indices, &alive, &m->cnt.get()->aos_error, &err)) != MPMB_OK) return rc;
+  if (err & DEVERR_BAD_SLOT)   // nothing has reached the host pool or the index vector yet
+    return fail(h, MPMB_ERR_INVALID, "2-D handle: a particle id or slot index is outside the index vector of %lld or the pool of %lld slots",
+                (long long)n_indices, (long long)pool_slots);
+  // survivors' slots in id order == what clear_boundary_particles leaves in MPM::particles (src/mpm.cpp:618-622); the
+  // scratch is keys_sorted, which the next ordering rewrites
+  uint32_t *d_surv = m->keys_sorted.get();
+  k_compact_survivors<<<(unsigned)((n_indices + 255) / 256), 256, 0, h->stream>>>(h->aos_idx.get(), h->scan_a.get(), h->scan_b.get(), n_indices, d_surv);
+  h->launches++;
+  if (pool_slots > 0) {  // only the window of every slot that holds the layout's fields comes back
+    int lo, hi;
+    aos_window(L, 2, &lo, &hi);
+    CUDA_TRY(h, cudaMemcpy2DAsync((char *)pool + lo, (size_t)L->stride, h->aos_pool.get() + lo, (size_t)L->stride, (size_t)(hi - lo), (size_t)pool_slots,
+                                  cudaMemcpyDeviceToHost, h->stream));
+  }
+  if (alive > 0) CUDA_TRY(h, cudaMemcpyAsync(indices, d_surv, sizeof(uint32_t) * (size_t)alive, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  *n_alive = alive;
+  return MPMB_OK;
+}
+
 int mpmb_upload_aos(MpmbHandle h, int64_t n, const void *pool, int64_t pool_slots, const uint32_t *indices,
                     const MpmbAosLayout *L, const int32_t *group) {
   CHECK_HANDLE(h);
-  NOT_2D(h);
+  if (h->m2) return m2_upload_aos(h, n, pool, pool_slots, indices, L, group);
   if (n < 0 || !pool || !indices || !L || L->stride <= 0) return fail(h, MPMB_ERR_INVALID, "pool, indices and layout are required");
   if ((int64_t)h->id_base + n > (1ll << TAG_ID_BITS)) return fail(h, MPMB_ERR_CAPACITY, "particle ids exceed 2^%d", TAG_ID_BITS);
   bool per_kind;
@@ -4838,7 +5039,7 @@ int mpmb_upload_aos(MpmbHandle h, int64_t n, const void *pool, int64_t pool_slot
   CUDA_TRY(h, cudaMemcpyAsync(h->aos_idx.get(), indices, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, h->stream));
   {
     int lo, hi;
-    aos_window(L, &lo, &hi);
+    aos_window(L, 3, &lo, &hi);
     CUDA_TRY(h, cudaMemcpy2DAsync(h->aos_pool.get() + lo, (size_t)L->stride, (const char *)pool + lo, (size_t)L->stride, (size_t)(hi - lo), (size_t)pool_slots,
                                   cudaMemcpyHostToDevice, h->stream));
   }
@@ -5010,7 +5211,7 @@ int mpmb_download_particles(MpmbHandle h, int64_t cap, int64_t *n_out, uint32_t 
 int mpmb_download_aos(MpmbHandle h, void *pool, int64_t pool_slots, uint32_t *indices, int64_t n_indices, const MpmbAosLayout *L,
                       int64_t *n_alive) {
   CHECK_HANDLE(h);
-  NOT_2D(h);
+  if (h->m2) return m2_download_aos(h, pool, pool_slots, indices, n_indices, L, n_alive);
   if (!pool || !indices || !L || !n_alive || L->stride <= 0 || n_indices < 0) return fail(h, MPMB_ERR_INVALID, "null argument");
   bool per_kind;
   int ns = 0, rc = aos_scalar_mode(h, L, &per_kind);
@@ -5047,7 +5248,7 @@ int mpmb_download_aos(MpmbHandle h, void *pool, int64_t pool_slots, uint32_t *in
   h->launches++;
   {  // only the window of every slot that holds the layout's fields comes back; the rest of the host pool is untouched
     int lo, hi;
-    aos_window(L, &lo, &hi);
+    aos_window(L, 3, &lo, &hi);
     CUDA_TRY(h, cudaMemcpy2DAsync((char *)pool + lo, (size_t)L->stride, h->aos_pool.get() + lo, (size_t)L->stride, (size_t)(hi - lo), (size_t)pool_slots,
                                   cudaMemcpyDeviceToHost, h->stream));
   }
