@@ -62,3 +62,81 @@ def state_of(got):
     st = {k: got[k].copy() for k in ("x", "v", "F", "b", "mass", "vol", "ps", "group")}
     st["alive"] = np.ones(len(st["x"]), np.uint8)
     return st
+
+
+# ---------------------------------------------------------------------------------------------------- bench_2d.py's column
+def bench_column(res):
+    """bench_2d.py's sand column at any res: the column is res / 2 cells wide and high on the 8-cell floor, dt = 5e-6 * 1024 / res
+    (bench_2d.SIZES at 1024 and 2048, where bench_2d.column itself is used).  Returns (state, dt, scene for the oracle)."""
+    import bench_2d
+    if res in bench_2d.SIZES:
+        st, dt = bench_2d.column(res)
+    else:
+        cells, dt = res // 2, 5e-6 * 1024 / res
+        lo = ((res - cells) // 2, bench_2d.FLOOR)
+        x, mass, vol = scenes.lattice_block2d((res, res), lo, (lo[0] + cells, lo[1] + cells), density=400.0)
+        st = scenes.make_state2d(x, mass, vol, scenes.MAT_SAND)
+    planes = [[0.0, 1.0, 0.0, -float(bench_2d.FLOOR)]]
+    scene = dict(res=(res, res), dx=1.0 / res, dt=dt, gravity=(0.0, -10.0), particle_gravity=1, clean_boundary=1, apic_damping=0.0,
+                 rpic_damping=0.0, mat_kind=np.array([scenes.MAT_SAND], np.int32), mat_params=scenes.material_params(scenes.MAT_SAND)[None],
+                 sdf=scenes.planes_sdf2d((res, res), planes), friction=0.4, route=("planes", planes))
+    return st, dt, scene
+
+
+def _math2(a4):
+    """Column-major [N, 4] -> [N, 2, 2] in math layout, fp64."""
+    return np.asarray(a4, np.float64).reshape(-1, 2, 2).transpose(0, 2, 1)
+
+
+def trial_F2d(scene, F, b):
+    """The trial F = cdg F of G2P, cdg = I + dt b (-4 / dx), from the stored F and the substep's undamped apic_b, fp64."""
+    S = -4.0 / float(np.float32(scene["dx"])) * float(scene["dt"])
+    return (np.eye(2) + S * _math2(b)) @ _math2(F)
+
+
+def sand_case2d(Ft, prm, ps):
+    """SandParticle::project's case with d = 2 (0: expansion, tr >= 0; 1: inside the cone, dg <= 0; 2: projected onto it) of
+    the trial F [N, 2, 2], in fp64: eps = log|sigma| - cohesion, tr = sum(eps) + logJp, hat = eps - tr / 2,
+    dg = |hat| + (2 lambda + 2 mu) / (2 mu) tr alpha."""
+    prm = np.asarray(prm, np.float64)
+    s = np.linalg.svd(Ft, compute_uv=False)
+    eps = np.log(np.maximum(np.abs(s), 1e-4)) - prm[3]
+    tr = eps.sum(1) + np.asarray(ps, np.float64)
+    hat = eps - tr[:, None] / 2
+    dg = np.linalg.norm(hat, axis=1) + (2 * prm[1] + 2 * prm[0]) / (2 * prm[0]) * tr * prm[2]
+    return np.where(tr >= 0, 0, np.where(dg <= 0, 1, 2))
+
+
+def regime2d(S_seed, S, ref, grid_rast, scene):
+    """The numbers that show S (the whole state, rows in id order) is bench_2d.py's developed collapse, in fp64: the floor
+    nodes' Coulomb branches (collapse.floor_branches, whose third components are 0 on a 2-D grid), the sand cases of the
+    return map on the trial F of the oracle's substep `ref` of S, the most particles in one cell, the centre of mass's drop
+    and the footprint width (occupied columns of cells) relative to the seeded column, and the fraction still alive."""
+    from tests.collapse import floor_branches
+    dx = float(scene["dx"])
+    out = floor_branches(grid_rast, scene["sdf"], float(scene["friction"]))
+    case = sand_case2d(trial_F2d(scene, S["F"], ref["b"]), scene["mat_params"][0], S["ps"])
+    out.update({"case%d" % c: int((case == c).sum()) for c in range(3)})
+    cell = np.floor(np.asarray(S["x"], np.float64) / dx).astype(np.int64)
+    _, counts = np.unique(cell[:, 0] * int(scene["res"][1]) + cell[:, 1], return_counts=True)
+    out["ppc_max"] = int(counts.max())
+    out["com_drop"] = float(np.asarray(S_seed["x"], np.float64)[:, 1].mean() - np.asarray(S["x"], np.float64)[:, 1].mean()) / dx
+
+    def width(x):
+        return len(np.unique(np.floor(np.asarray(x, np.float64)[:, 0] / dx)))
+    out["footprint"] = width(S["x"]) / width(S_seed["x"])
+    out["alive"] = len(S["x"]) / len(S_seed["x"])
+    return out
+
+
+# The regime guards of tests/test_gpu_zz_mpm2d_bench.py: about half of what its first H100 run measured (the table in its
+# header; footprint: half of the growth over the seeded column); ppc_max > 4 is compaction beyond the lattice's 4 per cell.
+# Every case of the return map and every Coulomb branch of the floor must be reached.  bench_2d's developed states by res:
+GUARDS_FULL = {1024: dict(stick=480, slide=42, separate=9, case0=99000, case1=138000, case2=285000, ppc_max=4, com_drop=3.5, footprint=1.023),
+               2048: dict(stick=930, slide=96, separate=39, case0=500000, case1=719000, case2=875000, ppc_max=4, com_drop=6.7, footprint=1.025)}
+# the reduced columns by (res, simulated seconds); tests/test_mpm2d_collapse_host.py shows the fp32 oracle reaches the 64^2 ones
+GUARDS_REDUCED = {(64, 0.05): dict(stick=26, slide=6, separate=3, case0=560, case1=120, case2=1360, ppc_max=4, com_drop=0.19, footprint=1.03),
+                  (128, 0.05): dict(stick=56, slide=8, separate=4, case0=2100, case1=670, case2=5400, ppc_max=4, com_drop=0.39, footprint=1.015),
+                  (128, 0.3): dict(stick=94, slide=16, separate=6, case0=1030, case1=1530, case2=5100, ppc_max=4, com_drop=7.0, footprint=1.39),
+                  (256, 0.05): dict(stick=117, slide=12, separate=5, case0=8000, case1=3800, case2=20900, ppc_max=4, com_drop=0.79, footprint=1.023),
+                  (256, 0.3): dict(stick=199, slide=32, separate=13, case0=2087, case1=7536, case2=21818, ppc_max=4, com_drop=14.3, footprint=1.44)}

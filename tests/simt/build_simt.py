@@ -14,6 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 SRC = os.path.join(ROOT, "taichi_mpm_b200", "csrc", "mpmb_engine.cu")
 MATH = os.path.join(ROOT, "taichi_mpm_b200", "csrc", "mpmb_math.cuh")
+MATH2 = os.path.join(ROOT, "taichi_mpm_b200", "csrc", "mpmb_math2d.cuh")   # the 2-D material math, included by SRC
 OUT_DIR = os.path.join(HERE, "_build")
 LIB = os.path.join(OUT_DIR, "libmpmb_simt.so")
 
@@ -65,7 +66,7 @@ def build(defines=(), force=False, asan=None):
     if asan is None:
         asan = os.environ.get("MPMB_SIMT_ASAN", "") == "1"
     ubsan = os.environ.get("MPMB_SIMT_UBSAN", "") == "1"   # UndefinedBehaviorSanitizer (LD_PRELOAD libubsan.so)
-    deps = [SRC, MATH, os.path.join(HERE, "simt.h"), os.path.join(HERE, "simt.cpp"), os.path.join(HERE, "stub", "cub", "simt_cub.h"), __file__]
+    deps = [SRC, MATH, MATH2, os.path.join(HERE, "simt.h"), os.path.join(HERE, "simt.cpp"), os.path.join(HERE, "stub", "cub", "simt_cub.h"), __file__]
     tag = "_".join([d.lower().replace("mpmb_exp_", "") for d in defines] + (["asan"] if asan else []) + (["ubsan"] if ubsan else []))
     lib = LIB if not tag else LIB.replace(".so", "_" + tag + ".so")
     if not force and os.path.exists(lib) and all(os.path.getmtime(d) <= os.path.getmtime(lib) for d in deps):

@@ -36,29 +36,46 @@ def make_engine2d(scene, st, **kw):
     return e
 
 
-def compare2d(e, scene, st, check_grid=True, ids=None):
+def compare2d(e, scene, st, check_grid=True, ids=None, yardstick=False, oracle=None):
     """One substep stage by stage on the engine and on the fp64 oracle; the errors as common.compare_substep measures them.
-    ids: the engine id of every row of `st` (ascending; default the row index, as after an upload)."""
+    ids: the engine id of every row of `st` (ascending; default the row index, as after an upload).
+    yardstick: also err["yardstick"], the fp32 oracle's errors on the same substep (yardstick2d).
+    oracle: the fp64 oracle's substep2d(scene, st) where the caller already has it."""
     from oracle import pyoracle2d as O
-    ref, grid_rast, grid_vel = O.substep2d(scene, st, np.float64)
-    out = {}
+    ref, grid_rast, grid_vel = O.substep2d(scene, st, np.float64) if oracle is None else oracle
     e.sort_particles_and_populate_grid()
     e.rasterize()
-    if check_grid:
-        g0 = e.download_grid(0).astype(np.float64)
-        g1 = e.download_grid(1).astype(np.float64)
-        pmax = max(np.abs(grid_rast[..., :2]).max(), grid_rast[..., 3].max())
-        out["grid_rast"] = np.abs(g0 - grid_rast).max() / pmax
-        active = grid_rast[..., 3] > 0
-        out["grid_vel"] = np.abs(g1[..., :2] - grid_vel[..., :2])[active].max() / max(np.abs(grid_vel[..., :2]).max(), 1e-30)
-        out["grid_mass_outside"] = np.abs(g0[~active]).max() if (~active).any() else 0.0
+    grids = (e.download_grid(0), e.download_grid(1)) if check_grid else None
     e.resample()
     got = e.download()
+    err = errors2d(got, grids, ref, grid_rast, grid_vel, ids)
+    if yardstick:
+        err["yardstick"] = yardstick2d(scene, st, ref, grid_rast, grid_vel, ids)
+    return err, got, ref
+
+
+def errors2d(got, grids, ref, grid_rast, grid_vel, ids=None):
+    """The errors compare2d reports, of any substep result against the fp64 oracle's: got = dict(id, x, v, b, F, ps, mass) of
+    the survivors, grids = (P2G grid, node velocities) or None.  ids: as in compare2d."""
+    out = {}
+    if grids is not None:
+        g0, g1 = (np.asarray(g, np.float64) for g in grids)
+        pmax = max(np.abs(grid_rast[..., :2]).max(), grid_rast[..., 3].max())
+        out["grid_rast"] = np.abs(g0 - grid_rast).max() / pmax
+        m = grid_rast[..., 3]
+        active = m > 0
+        dv = np.abs(g1[..., :2] - grid_vel[..., :2]).max(-1)
+        vmax = max(np.abs(grid_vel[..., :2]).max(), 1e-30)
+        out["grid_vel"] = dv[active].max() / vmax
+        # the worst node's fp64 mass relative to the heaviest node's, and the same error over the heavy nodes only
+        out["grid_vel_node_mass"] = m.flat[np.argmax(np.where(active, dv, -1.0))] / m.max()
+        out["grid_vel_heavy"] = dv[m >= HEAVY * m.max()].max() / vmax
+        out["grid_mass_outside"] = np.abs(g0[~active]).max() if (~active).any() else 0.0
     alive = ref["alive"].astype(bool)
     row_ids = np.arange(len(alive)) if ids is None else np.asarray(ids, np.int64)
     out["alive_match"] = len(got["id"]) == alive.sum() and np.array_equal(got["id"].astype(np.int64), row_ids[alive])
     if not out["alive_match"] or not alive.any():
-        return out, got, ref
+        return out
     ids = np.searchsorted(row_ids, got["id"].astype(np.int64))   # oracle row of every downloaded particle
     out["x"] = np.abs(got["x"] - ref["x"][ids]).max()
     out["v"] = np.abs(got["v"] - ref["v"][ids]).max() / np.abs(ref["v"][alive]).max()
@@ -67,7 +84,53 @@ def compare2d(e, scene, st, check_grid=True, ids=None):
     out["F"] = (np.abs(got["F"] - ref["F"][ids]) / np.maximum(1.0, np.abs(ref["F"][ids]).max(1, keepdims=True))).max()
     out["ps"] = T.ps_err(got["ps"], ref["ps"][ids])
     out["mass"] = np.abs(got["mass"] - ref["mass"][ids]).max()
-    return out, got, ref
+    return out
+
+
+def yardstick2d(scene, st, ref, grid_rast, grid_vel, ids=None):
+    """The fp32 yardstick: the fp32 oracle's own errors on the same substep of `st`, measured as errors2d measures the engine's
+    against the fp64 oracle (ref, grid_rast, grid_vel).  Where the fp32 oracle keeps other survivors (rounding at the band
+    edge) its particle errors are not measured and those metrics are held to their tests/common.py bounds alone."""
+    from oracle import pyoracle2d as O
+    r32, gr32, gv32 = O.substep2d(scene, st, np.float32)
+    alive = r32["alive"].astype(bool)
+    row_ids = np.arange(len(alive)) if ids is None else np.asarray(ids, np.int64)
+    got = {k: r32[k][alive] for k in ("x", "v", "b", "F", "ps", "mass")}
+    got["id"] = row_ids[alive]
+    return errors2d(got, (gr32, gv32), ref, grid_rast, grid_vel, ids)
+
+
+# the metrics the yardstick rule applies to and their tests/common.py bounds: the grid, the velocity-normalised ones, and F
+# and ps, which G2P forms from the velocity gradient b (cdg = I + dt b (-4 / dx)) and which therefore carry its rounding.
+# grid_vel_heavy is grid_vel over the nodes whose fp64 mass is at least HEAVY of the heaviest node's (the 3-D window tests'
+# "heavy" nodes): a node whose mass comes only from weights near 0 gets them from the reference's expanded quadratic
+# 0.5 t^2 - 1.5 t + 1.125, which fp32 evaluates to about 1e-7 absolute, so its velocity (a weighted mean) is not resolved in
+# fp32 and grid_vel there is only held by the yardstick; grid_vel_heavy keeps the node velocities checked on such substeps.
+YARD_TOL = dict(grid_rast=T.TOL_GRID_REL, grid_vel=T.TOL_GRID_REL, grid_vel_heavy=T.TOL_GRID_REL, v=T.TOL_V_REL, b=T.TOL_V_REL,
+                F=T.TOL_F_ABS, ps=T.TOL_PS_ABS)
+YARD_FACTOR = 4.0
+HEAVY = 1e-4
+
+
+def assert_parity_yardstick(err, grid=True, label=""):
+    """assert_parity with the yardstick rule on an err of compare2d(..., yardstick=True): a metric of YARD_TOL passes at its
+    tests/common.py bound or at YARD_FACTOR times the fp32 oracle's error on the same metric.  Where fp32 itself rounds by
+    about that bound (X = x / dx rounded at X ~ 2e3 on a dx that is not a power of two is 6e-5 cells, so dpos, b and cdg of a
+    particle moving most of a cell per substep carry it; velocities of 1e-3 m/s in a resting column; hundreds of particles
+    summed into one node), the engine is held to what fp32 arithmetic can do rather than to a bound it cannot meet;
+    everywhere else the common bound decides.  x keeps its common bound, mass and the mass outside the active nodes stay
+    exactly 0, and the survivors are the oracle's."""
+    yard = err["yardstick"]
+    print(label, {k: "%.3g" % float(v) for k, v in err.items() if k in YARD_TOL or k in ("x", "grid_vel_node_mass")},
+          "yardstick", {k: "%.3g" % float(yard[k]) for k in YARD_TOL if k in yard})
+    assert err["alive_match"], (label, err)
+    for k, tol in YARD_TOL.items():
+        if k in err and (grid or not k.startswith("grid")):
+            assert err[k] <= tol or err[k] <= YARD_FACTOR * yard.get(k, 0.0), (label, k, err[k], tol, yard.get(k))
+    if grid:
+        assert err["grid_mass_outside"] == 0.0, (label, err)
+    assert err["x"] <= T.TOL_X_ABS, (label, err)
+    assert err["mass"] == 0.0, (label, err)
 
 
 def assert_parity(err, grid=True):
@@ -225,6 +288,59 @@ def test_particles_change_cell_every_substep():
         ca = np.floor(got["x"] * res[0] - 0.5).astype(int)
         moved = max(moved, (cb != ca).any(1).mean())
     assert moved > 0.4, moved
+    e.close()
+
+
+def crowded_state(scene, lo, hi, ppc, seed):
+    """n x n particles per cell (ppc = n^2) over cells [lo, hi), jittered within their sub-cells, vol = dx^2 / ppc and mass
+    400 vol (the density of the 4-per-cell lattice), perturbed as scene2d perturbs its blocks."""
+    dx, n = scene["dx"], int(round(np.sqrt(ppc)))
+    rng = np.random.default_rng(seed)
+    c = np.stack(np.meshgrid(np.arange(lo[0], hi[0]), np.arange(lo[1], hi[1]), indexing="ij"), -1).reshape(-1, 1, 2)
+    s = np.stack(np.meshgrid(np.arange(n), np.arange(n), indexing="ij"), -1).reshape(1, -1, 2)
+    X = (c + (s + 0.5 + rng.uniform(-0.3, 0.3, (c.shape[0], s.shape[1], 2))) / n).reshape(-1, 2)
+    vol = np.full(len(X), dx * dx / ppc, np.float32)
+    st = scenes.make_state2d((X * dx).astype(np.float32), vol * np.float32(400.0), vol, scenes.MAT_SAND)
+    return perturb2d(st, scenes.MAT_SAND, dx, seed)
+
+
+# particles per cell and cells per side: the developed column reaches 6 to 8 per cell (DESIGN §10); k2_grid sums every
+# particle of a node's 3 x 3 cells in one fixed-order fp32 loop, so its rounding grows with the count.  Measured on an
+# NVIDIA H100 80GB HBM3 (700 W power limit), grid_rast / grid_vel / v / b / F / ps: 16: 5.1e-7 / 4.2e-7 / 4.4e-7 / 7.3e-6 /
+# 2.9e-7 / 2.7e-7; 64: 7.5e-7 / 6.3e-7 / 6.8e-7 / 9.8e-6 / 3.4e-7 / 2.5e-7; 256: 7.7e-7 / 1.7e-6 / 1.4e-6 / 2.0e-5 / 3.5e-7 /
+# 3.1e-7; 4096 in one cell: 9.7e-7 / 2.1e-6 / 9.8e-7 / 3.7e-5 / 3.6e-7 / 2.9e-7; test_stencil_base_switch: 1.6e-7 / 1.6e-7 /
+# 1.4e-7 / 3.1e-6 / 2.3e-7 / 2.3e-7.  All are inside the tests/common.py bounds: the yardstick rule passes none of them.
+CROWDED = {"16": (16, 8), "64": (64, 6), "256": (256, 4), "4096_in_one_cell": (4096, 1)}
+
+
+@pytest.mark.parametrize("name", list(CROWDED))
+def test_crowded_cells(name):
+    ppc, cells = CROWDED[name]
+    lo = (14, 10)
+    hi = (lo[0] + cells, lo[1] + cells)
+    scene, _ = scene2d(scenes.MAT_SAND, blocks=[(lo, hi)], seed=30)
+    st = crowded_state(scene, lo, hi, ppc, seed=31)
+    cell = np.floor(st["x"].astype(np.float64) / scene["dx"]).astype(int)
+    assert np.unique(cell[:, 0] * 64 + cell[:, 1], return_counts=True)[1].min() == ppc
+    e = make_engine2d(scene, st)
+    err, _, _ = compare2d(e, scene, st, yardstick=True)
+    assert_parity_yardstick(err, label="crowded %s" % name)
+    e.close()
+
+
+def test_stencil_base_switch():
+    """Particles exactly at X = k and X = k + 0.5 on each axis (dx = 2^-5, so X is exact in fp32): at X = k + 0.5 the stencil
+    base int(X - 0.5) switches to k and the fraction is 0, at X = k the base is k - 1 and the fraction 1/2."""
+    lo, hi = (12, 10), (20, 18)
+    scene, _ = scene2d(scenes.MAT_SAND, blocks=[(lo, hi)], seed=32)
+    X = np.stack(np.meshgrid(np.arange(2 * lo[0], 2 * hi[0]) * 0.5, np.arange(2 * lo[1], 2 * hi[1]) * 0.5, indexing="ij"), -1).reshape(-1, 2)
+    vol = np.full(len(X), scene["dx"] ** 2 / 4, np.float32)
+    st = perturb2d(scenes.make_state2d((X * scene["dx"]).astype(np.float32), vol * np.float32(400.0), vol, scenes.MAT_SAND),
+                   scenes.MAT_SAND, scene["dx"], 33)
+    assert np.array_equal(st["x"].astype(np.float64) / scene["dx"], X)
+    e = make_engine2d(scene, st)
+    err, _, _ = compare2d(e, scene, st, yardstick=True)
+    assert_parity_yardstick(err, label="stencil base switch")
     e.close()
 
 

@@ -26,6 +26,17 @@ def test_mpm2d_suite_passes_on_the_simt_emulator():
     assert " passed" in tail and "failed" not in tail and "skipped" not in tail, tail
 
 
+def test_mpm2d_bench_cases_pass_on_the_simt_emulator():
+    # tests/test_gpu_zz_mpm2d_bench.py's cases the emulator runs (about 90 s on 8 host threads): the 64^2 collapse after
+    # 0.05 s and every large grid; the full-size states and the longer collapses carry needs_cuda and are deselected here,
+    # so that "skipped" still means a selected case did not run
+    r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider", "tests/test_gpu_zz_mpm2d_bench.py",
+                        "-k", "64-0.05s or test_large_grids"], cwd=ROOT, env=_env("0"), stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    tail = "\n".join(r.stdout.strip().splitlines()[-15:])
+    assert r.returncode == 0, tail
+    assert "8 passed" in tail and "failed" not in tail and "skipped" not in tail, tail
+
+
 _SCRIPT = r"""
 import os, sys
 import numpy as np
